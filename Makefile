@@ -2,7 +2,7 @@
 PY ?= python
 
 .PHONY: lib oracle hostsim test-cpu test-gpu bench clean
-lib:            ## solo_b200/libsolo_b200.so (nvcc, sm_100a)
+lib:            ## solo_b200/libsolo_b200.so (nvcc, sm_90a)
 	$(PY) -m solo_b200.build
 oracle:         ## the unmodified reference compiled into oracle/_ref (needs /root/reference)
 	$(MAKE) -C oracle -j4

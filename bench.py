@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- SOLO encode+decode packets/s on B200 (BASELINE.json metric), contract of the build brief.
+"""bench.py -- SOLO encode+decode packets/s on H100 (BASELINE.json metric), contract of the build brief.
 
 A "step" is one packet wave: every resident stream encodes one 40 ms / 16 kHz packet and decodes it again
 (lostflag 4).  Workload = BASELINE.json configs[2]: 65 536 concurrent streams per GPU, speech-replay input
@@ -9,10 +9,12 @@ A "step" is one packet wave: every resident stream encodes one 40 ms / 16 kHz pa
   value : packets/s with PCM already resident in HBM (device entry points of the C ABI, CUDA events, max over ranks)
   e2e   : packets/s through the host entry points of the C ABI (pinned host buffers; H2D of the PCM, D2H of the
           payloads, H2D of payloads/flags and D2H of the decoded PCM are all inside the timed region)
-  roofline     : encode kernel (dominant), algorithmic bytes / CUDA-event kernel time vs measured HBM copy peak
+  roofline     : encode kernel (dominant), algorithmic bytes / CUDA-event kernel time vs HBM peak
   cpu_baseline : the unmodified reference (oracle/_ref: FIX encoder + FLP decoder) on all host cores, bounded sample
 
 `--impl reference` times only that CPU baseline and prints the same JSON shape.
+`--dump-outputs DIR` writes, for a fixed sample of rank 0's streams, what the last timed step of the device path and of
+the host path returned (payload rows, length fields, decoded PCM, return codes) as float32 .npy files.
 """
 import argparse
 import json
@@ -33,6 +35,16 @@ UNIT = "packets/s"
 CAP = 128           # bytes per payload row (max observed 117 at 13.6 kb/s; the kernel honours the cap like bits_write)
 RATE = 13600
 MEAN_PAYLOAD = 83.0  # refined with the measured mean below
+PCM_WAVES = 32       # distinct input waves held in pinned host memory and in HBM (2.7 GB at 65 536 streams)
+DUMP_STREAMS = 4096  # streams sampled by --dump-outputs (fixed seed): 2 x 4096 x (640 + 128 + 2 + 1) x 4 B = 25 MB
+
+
+def dump_outputs(dirname, rows, prefix, arrays):
+    """arrays: name -> [N, ...] tensor or array of one step's outputs; writes rows `rows` of each as float32."""
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.cpu().numpy() if hasattr(a, "cpu") else np.asarray(a)
+        np.save(os.path.join(dirname, prefix + name + ".npy"), a[rows].astype(np.float32))
 
 
 def load_clip():
@@ -59,32 +71,21 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
-def ncu_summary():
-    """profiles/ncu_summary.json (tools/profile_round.py): per kernel the DRAM bytes, issue-slot utilisation and warp
-    instructions of one `ncu --set full` launch.  bench.py never runs under a profiler; these are the committed captures."""
-    p = os.path.join(ROOT, "profiles", "ncu_summary.json")
+def gpu_identity(index):
+    """Card name, power limit (W) and maximum SM clock (MHz): an absolute number is only meaningful beside them."""
     try:
-        d = json.load(open(p))
-        return d if "kernels" in d else None
-    except Exception:
-        return None
-
-
-def ncu_traffic(kernel, streams_per_launch):
-    """DRAM bytes (read + write) of `kernel` per launch, scaled from the capture's streams per launch to this run's."""
-    d = ncu_summary()
-    try:
-        k = d["kernels"][kernel]
-        return k["dram_bytes_per_launch"] / k["streams_per_launch"] * streams_per_launch
-    except Exception:
-        return None
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception as ex:
+        return {"error": type(ex).__name__}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons while the timed region runs (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks + throttle reasons while the timed region runs."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -207,6 +208,7 @@ def measure_root_ingest(args, dist, solo_b200, torch, rank, world, local_rank, d
     back -- scatter and gather are fused into the kernels that consume / produce the data, no NCCL transfer step, no staging copy."""
     from solo_b200.shard import share_from_root
     lo = rank * N
+    R = d_pcm.shape[0]      # step t reads wave t % R, as in the rank-ingest measurement
 
     def agree(ok):      # every rank takes part, so that a failure on one rank ends the measurement on all of them together
         f = torch.tensor([1 if ok else 0], dtype=torch.int32, device=dev)
@@ -217,7 +219,7 @@ def measure_root_ingest(args, dist, solo_b200, torch, rank, world, local_rank, d
     r_pcm = r_bits = r_nb = r_out = None
     if rank == 0:
         try:
-            r_pcm = torch.empty((T, world * N, 640), dtype=torch.int16, device=dev)
+            r_pcm = torch.empty((R, world * N, 640), dtype=torch.int16, device=dev)
             r_bits = torch.zeros((world * N, CAP), dtype=torch.uint8, device=dev)
             r_nb = torch.zeros((world * N, 2), dtype=torch.int16, device=dev)
             r_out = torch.zeros((world * N, 640), dtype=torch.int16, device=dev)
@@ -239,7 +241,7 @@ def measure_root_ingest(args, dist, solo_b200, torch, rank, world, local_rank, d
     pb, pn, po = r_bits[lo:lo + N].data_ptr(), r_nb[lo:lo + N].data_ptr(), r_out[lo:lo + N].data_ptr()
 
     def step_root(t):
-        enc_r.encode_device(r_pcm[t, lo:lo + N].data_ptr(), pb, CAP, pn, stream)
+        enc_r.encode_device(r_pcm[t % R, lo:lo + N].data_ptr(), pb, CAP, pn, stream)
         dec_r.decode_device(po, pb, CAP, pn, d_flags.data_ptr(), d_ret.data_ptr(), stream)
 
     for t in range(W):
@@ -309,7 +311,10 @@ def main():
     ap.add_argument("--streams", type=int, default=65536, help="streams per GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-root-ingest", action="store_true", help="skip the single-ingest-point measurement (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (sampled streams) as .npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "solo_b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -343,11 +348,13 @@ def main():
     dec = solo_b200.DecoderBatch(N, device=local_rank)
 
     # ---------------- device-resident throughput (`value`) ----------------
-    # Each step consumes a different 84 MB PCM wave (inputs + 0.9 GB of codec state >> 126 MB L2: no L2 flush needed).
-    host_pcm = torch.from_numpy(speech_replay(clip, sids, T)).pin_memory()      # [T, N, 640] int16
+    # Step t consumes PCM wave t % R, a different 84 MB wave from its neighbours (inputs + 0.9 GB of codec state >> 50 MB
+    # L2: no L2 flush needed).  At most PCM_WAVES waves are resident, so that --steps is not bounded by HBM / pinned memory.
+    R = min(T, PCM_WAVES)
+    host_pcm = torch.from_numpy(speech_replay(clip, sids, R)).pin_memory()      # [R, N, 640] int16
     d_pcm = host_pcm.to(dev, non_blocking=True)
     # Encoder wave then decoder wave on one CUDA stream.  (Running the two batch objects on separate streams so that
-    # decode(t) overlaps encode(t+1) gains nothing -- tools/overlap_check.py, 25.6 vs 25.8 ms: a later grid's blocks are only
+    # decode(t) overlaps encode(t+1) gained nothing in tools/overlap_check.py: a later grid's blocks are only
     # placed once the earlier grid has none left, so the kernels overlap at their tails -- DESIGN.md section 6.)
     d_bits = torch.zeros((N, CAP), dtype=torch.uint8, device=dev)
     d_nb = torch.zeros((N, 2), dtype=torch.int16, device=dev)
@@ -357,7 +364,7 @@ def main():
     stream = torch.cuda.current_stream().cuda_stream
 
     def step_device(t):
-        enc.encode_device(d_pcm[t].data_ptr(), d_bits.data_ptr(), CAP, d_nb.data_ptr(), stream)
+        enc.encode_device(d_pcm[t % R].data_ptr(), d_bits.data_ptr(), CAP, d_nb.data_ptr(), stream)
         dec.decode_device(d_out.data_ptr(), d_bits.data_ptr(), CAP, d_nb.data_ptr(), d_flags.data_ptr(), d_ret.data_ptr(), stream)
 
     for t in range(W):
@@ -365,6 +372,7 @@ def main():
     torch.cuda.synchronize()
     if dist:
         dist.barrier()
+    gpu = gpu_identity(local_rank)
     sampler = ClockSampler(local_rank)
     sampler.start()
     solo_b200.profile_enable(True)
@@ -387,6 +395,11 @@ def main():
         dist.all_reduce(t_, op=dist.ReduceOp.MAX)
         dev_ms = float(t_.item())
     value = world * N * K / (dev_ms / 1e3)
+    dump_rows = None
+    if args.dump_outputs and rank == 0:
+        dump_rows = np.sort(np.random.default_rng(0).choice(N, min(N, DUMP_STREAMS), replace=False))
+        dump_outputs(args.dump_outputs, dump_rows, "device_", {"payload": d_bits, "nbytes": d_nb, "pcm": d_out, "ret": d_ret})
+        np.save(os.path.join(args.dump_outputs, "stream_ids.npy"), dump_rows.astype(np.float64))
 
     # ---------------- configs[3] as BASELINE words it: one ingest point (`root_ingest`, N > 1 only) ----------------
     # Rank 0 owns the PCM of ALL streams and receives all payloads / decoded PCM in its HBM; the other ranks map those buffers
@@ -413,7 +426,7 @@ def main():
     h_ret = torch.zeros((N,), dtype=torch.int32).pin_memory()
 
     def step_host(t):
-        enc.encode_ptr(host_pcm[t].data_ptr(), h_bits.data_ptr(), CAP, h_nb.data_ptr())
+        enc.encode_ptr(host_pcm[t % R].data_ptr(), h_bits.data_ptr(), CAP, h_nb.data_ptr())
         dec.decode_ptr(h_out.data_ptr(), h_bits.data_ptr(), CAP, h_nb.data_ptr(), h_flags.data_ptr(), h_ret.data_ptr())
 
     for t in range(W):
@@ -431,6 +444,8 @@ def main():
         dist.all_reduce(t_, op=dist.ReduceOp.MAX)
         host_ms = float(t_.item())
     clocks = sampler.stop()
+    if dump_rows is not None:
+        dump_outputs(args.dump_outputs, dump_rows, "host_", {"payload": h_bits, "nbytes": h_nb, "pcm": h_out, "ret": h_ret})
     e2e_value = world * N * K / (host_ms / 1e3)
     checksum = int(h_out.to(torch.int64).sum().item())
     h2d = world * N * (1280 + CAP + 4 + 4)      # whole job, per step: PCM in (encoder) + payload, lengths, flags in (decoder)
@@ -455,20 +470,18 @@ def main():
             "config": {"workload": "configs[2]: batch=65536 streams/GPU full encode+decode round trip (lostflag 4), 13.6 kb/s",
                        "arithmetic": "int32/int16 fixed point (encoder, SILK decoder), f32 (decoder high band + QMF synthesis)",
                        "streams_per_gpu": N, "streams_total": world * N, "pipeline_chunks": os.environ.get("SOLO_B200_CHUNKS", "default: 1 (device entry points), 3 (host entry points)"), "payload_cap": CAP, "mean_payload_bytes": mean_payload,
-                       "l2": "no flush: every step reads a new 84 MB PCM wave and ~0.9 GB of per-stream state (> 126 MB L2)",
+                       "l2": "no flush: every step reads another 84 MB PCM wave and ~0.9 GB of per-stream state (> 50 MB L2)",
+                       "pcm_waves": R,
                        "parallelism": "streams sharded contiguously across GPUs, no collective on the data path",
                        "host_binding": numa},
             "streams_rt": value / 25.0,
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": host_ms / K, "streams_rt": e2e_value / 25.0, "pcm_checksum": checksum},
             "gpu_launches": int(launches),
+            "gpu": gpu,
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "sb_enc_nsq_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": ncu_traffic("sb_enc_nsq_kernel", streams_per_launch), "peak_source": peak_src,
-                         "issue_util": ((ncu_summary() or {}).get("issue_util_time_weighted_pct") or 0) / 100.0 or None,
-                         "dram_bytes_per_packet": (ncu_summary() or {}).get("dram_bytes_per_packet"),
-                         "warp_inst_per_packet": (ncu_summary() or {}).get("warp_inst_per_packet"),
-                         "ncu_capture": (ncu_summary() or {}).get("from"),
+                         "frac": (achieved / peak) if achieved else None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes_enc, "kernel_ms": enc_ms,
                          "kernel_ms_all": kms, "kernel_ms_per_wave": kms_wave, "streams_per_launch": streams_per_launch,
                          "decode_algorithmic_bytes_per_launch": alg_bytes_dec,

@@ -6,7 +6,7 @@
  *     /root/reference/JC1_SDK_SRC_{ARM,FLP}/interface/AGR_JC1_SDK_API.h:11-64
  * (implementation replaced: .../src/libBWE/AGR_BWE_SDK_API.c:11-296), so a caller written against the
  * reference links against libsolo_b200.so unchanged.  Behind them every handle owns one stream slot of a
- * device-resident state arena and each call runs the sm_100a kernels on one stream; the batched interface
+ * device-resident state arena and each call runs the sm_90a kernels on one stream; the batched interface
  * for tens of thousands of streams per launch is in solo_b200.h.
  *
  * Contract (reference file:line in brackets):

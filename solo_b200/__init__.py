@@ -1,6 +1,6 @@
-"""solo_b200 -- B200-native batched SOLO speech codec (host-side Python mirror of the C ABI).
+"""solo_b200 -- H100-native batched SOLO speech codec (host-side Python mirror of the C ABI).
 
-The product is ``libsolo_b200.so`` (hand-written sm_100a CUDA behind the reference's C ABI, see
+The product is ``libsolo_b200.so`` (hand-written sm_90a CUDA behind the reference's C ABI, see
 ``include/AGR_JC1_SDK_API.h`` and ``include/solo_b200.h``).  This package only binds it with ctypes for tests
 and benchmarks; it contains no codec arithmetic and no CPU fallback: importing the binding without the built
 library, or creating a codec without a GPU, raises.

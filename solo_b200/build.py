@@ -1,4 +1,4 @@
-"""Build libsolo_b200.so (sm_100a) in-tree with nvcc.  No JIT cache, no arch fall-backs."""
+"""Build libsolo_b200.so (sm_90a, H100) in-tree with nvcc.  No JIT cache, no arch fall-backs."""
 import os
 import shutil
 import subprocess
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRCS = [os.path.join(HERE, "csrc", f) for f in ("solo_b200.cu", "sb_analysis.cu")]
 OUT = os.path.join(HERE, "libsolo_b200.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false",            # decoder float path and the three IEEE ops of the encoder must not be contracted
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared", "-t", "2",
 ]
@@ -17,7 +17,8 @@ NVCC_FLAGS = [
 def sources():
     d = os.path.join(HERE, "csrc")
     return [os.path.join(d, f) for f in sorted(os.listdir(d)) if f.endswith((".cu", ".cuh", ".inc"))] + [
-        os.path.join(os.path.dirname(HERE), "include", f) for f in ("solo_b200.h", "AGR_JC1_SDK_API.h")]
+        os.path.join(os.path.dirname(HERE), "include", f) for f in ("solo_b200.h", "AGR_JC1_SDK_API.h")] + [
+        os.path.abspath(__file__)]     # the flags live here: a library built with other flags (another arch) is stale
 
 
 def up_to_date():

@@ -1,4 +1,4 @@
-// solo_b200 -- encoder stage A as warp-per-stream kernels (sm_100a).
+// solo_b200 -- encoder stage A as warp-per-stream kernels (sm_90a).
 //
 // This translation unit compiles the analysis routines in their cooperative form (sb_coop.cuh): the 32 lanes of a warp work on
 // ONE stream, whose persistent analysis state and per-packet working set live in shared memory for the duration of the packet.

@@ -1,7 +1,7 @@
 // solo_b200 -- level-0 integer arithmetic kit shared by every per-stream codec routine.
 //
 // Every routine in solo_b200/csrc/*.cuh is written once as a __host__ __device__ function:
-//   * nvcc compiles it into the sm_100a kernels of libsolo_b200.so (the product path);
+//   * nvcc compiles it into the sm_90a kernels of libsolo_b200.so (the product path);
 //   * tests/hostsim compiles the same source with g++ so that the kernel logic can be checked
 //     against the compiled reference (oracle/_ref) in a container without a GPU.
 // The host build is test infrastructure only; libsolo_b200.so never executes codec maths on the CPU.

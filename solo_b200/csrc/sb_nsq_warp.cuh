@@ -1,4 +1,4 @@
-// solo_b200 -- MD delayed-decision noise-shaping quantiser, one stream per lane group of a warp (sm_100a device code).
+// solo_b200 -- MD delayed-decision noise-shaping quantiser, one stream per lane group of a warp (sm_90a device code).
 //
 // Same arithmetic as the scalar model in sb_nsq.cuh (which cites the reference line by line); this file only changes
 // WHERE things live and WHO computes them:

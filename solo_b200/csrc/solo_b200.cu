@@ -1,4 +1,4 @@
-// solo_b200 -- sm_100a kernels and the C ABI of libsolo_b200.so.
+// solo_b200 -- sm_90a (H100) kernels and the C ABI of libsolo_b200.so.
 //
 // One packet wave of the encoder = eight launches, of the decoder = two (DESIGN.md section 4):
 //   sb_enc_qmf_kernel            warp per stream       QMF band split, PCM rows fetched by the TMA engine (cp.async.bulk)
@@ -42,7 +42,7 @@ using namespace sb;
 extern "C" int sb_launch_enc_analysis_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
 extern "C" int sb_launch_enc_hb_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
 #ifndef SB_FINISH_MINB
-#define SB_FINISH_MINB 8     // 128 registers: every stream of a chunk resident (0.92 -> 0.65 ms per wave)
+#define SB_FINISH_MINB 8     // 128 registers: every stream of a chunk resident
 #endif
 #ifndef SB_DECODE_MINB
 #define SB_DECODE_MINB 8
@@ -58,8 +58,8 @@ __global__ void __launch_bounds__(SB_TPB) sb_enc_init_kernel(EncState* states, i
 // packet.  A block takes SB_QMF_SPB consecutive streams; their PCM rows are contiguous in HBM, so ONE bulk asynchronous copy
 // (cp.async.bulk -> UBLKCP, completion on an mbarrier) brings the whole tile into shared memory while the warps load their
 // filter memories; each lane then produces output pairs k = lane, lane + 32, ... (products summed mod 2^32: order-free).
-// Measured (65 536 streams, 2 chunks): +3.3 % end-to-end throughput, device-resident unchanged, versus the split inside kernel A;
-// larger blocks (8 streams) cost 2 % device-resident because they cannot start while kernel B holds the shared memory.
+// Against the split inside kernel A this raised end-to-end throughput and left device-resident throughput unchanged;
+// larger blocks (8 streams) were slower device-resident because they cannot start while kernel B holds the shared memory.
 #ifndef SB_QMF_SPB
 #define SB_QMF_SPB 1        // one-warp blocks of 2.8 KB: they fit in the shared memory the quantiser kernel leaves free on an SM
 #endif
@@ -356,9 +356,9 @@ struct Pipe {
     bool ok;
 };
 static int g_chunks = -1;   // -1: SOLO_B200_CHUNKS or the defaults below
-// Default: the host entry points cut a wave in three (the copies of one chunk hide behind the kernels of its neighbours:
-// 26.8 ms per 65 536-stream wave end to end, against 27.2 with two chunks, 27.0 with four, 28.0 with six); the device entry
-// points launch every kernel once for the whole batch.
+// Default: the host entry points cut a wave in three (the copies of one chunk hide behind the kernels of its neighbours;
+// three beat two, four and six in an earlier comparison, not repeated on H100); the device entry points launch every
+// kernel once for the whole batch.
 static int pipe_chunks(int n, bool host_copies) {
     if (g_chunks < 0) {
         const char* e = getenv("SOLO_B200_CHUNKS");

@@ -22,9 +22,8 @@ def _bytes(t):
 
 def _run(ops):
     """Post the point-to-point operations of one scatter / gather, one dist.send / dist.recv each (asynchronous on NCCL's
-    stream, so the transfers to different peers still overlap).  Measured on 2 x B200, 65 536 streams: 0.27 ms per scatter
-    (157 GB/s), 0.15 ms per gather; the grouped form (dist.batch_isend_irecv, SOLO_B200_P2P=grouped) took 46 ms per scatter
-    on the same box -- the 1.3 GB/s of round 1."""
+    stream, so the transfers to different peers still overlap).  The grouped form (dist.batch_isend_irecv,
+    SOLO_B200_P2P=grouped) was far slower than separate sends in an earlier measurement; neither has been timed on H100."""
     import os
     if not ops:
         return

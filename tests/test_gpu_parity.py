@@ -1,4 +1,4 @@
-"""On-device parity: the sm_100a kernels, called through the C ABI of libsolo_b200.so, against
+"""On-device parity: the sm_90a kernels, called through the C ABI of libsolo_b200.so, against
  (a) the committed golden vectors and (b) the unmodified reference (oracle/_ref) run on the same inputs.
 Bar: encoder payloads + length fields byte-identical to the reference FIX build; decoded PCM identical (tolerance
 stated by the north star is +-1 LSB; we require 0) to the reference FLP build."""

@@ -2,7 +2,7 @@ import collections, csv, subprocess, sys, re, os
 rep=sys.argv[1]; kern=sys.argv[2]
 out = subprocess.run(["ncu","-i",rep,"--page","source","--csv","--print-source","cuda,sass","-k","regex:"+kern],capture_output=True,text=True).stdout
 # function starts per file
-root="/root/repo/solo_b200/csrc/"
+root=os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),"solo_b200","csrc","")
 starts={}
 for f in os.listdir(root):
     if not f.endswith((".cuh",".cu")): continue

@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""Turn one round's ncu artefacts into the committed summaries under profiles/.
+"""Turn one round's ncu artefacts into summaries under profiles/ (local output, not committed).
 
 usage: tools/profile_round.py <tag> <launches.csv> <full.ncu-rep> <streams-per-launch> [libsolo_b200.so]
   <launches.csv>  ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file <launches.csv> python tools/ncu_target.py N T dec
   <full.ncu-rep>  ncu --set full --clock-control none --import-source on -k regex:^sb_|sb_enc -o ... python tools/ncu_target.py N T dec
                   (every codec kernel once; the LAST captured launch of a kernel is used)
-writes profiles/<tag>_launches.txt, profiles/<tag>_full.txt, profiles/<tag>_sass.txt and profiles/ncu_summary.json (read by bench.py:
-roofline.traffic / issue_util / dram_bytes_per_packet).  ncu launch times are cold-cache and serialised: compare SHARES."""
+writes profiles/<tag>_launches.txt, profiles/<tag>_full.txt, profiles/<tag>_sass.txt and profiles/ncu_summary.json
+(per kernel DRAM traffic, issue utilisation, warp instructions).  ncu launch times are cold-cache and serialised: compare SHARES."""
 import collections
 import csv
 import json
