@@ -1,6 +1,9 @@
 // solo_b200 -- one SOLO packet through the decoder (float-build semantics: the PCM parity target).
 // Low band: integer SILK decoder (range decode, MD excitation rebuild, LTP + LPC synthesis, PLC, CNG);
 // high band: float LPC synthesis of the folded low-band excitation; float QMF synthesis; truncate to int16.
+// As on the device, a packet takes two steps: dec_packet (the decode kernel) up to the two band signals, and dec_synth (the
+// scalar model of the synthesis kernel, which shares qmf_synth_group) for the filter bank and the int16 output; the host
+// model's dec_packet with a PCM output runs both.
 // Reference (paths under /root/reference/JC1_SDK_SRC_FLP/src/):
 //   libBWE/AGR_BWE_decode_frame_FLP.c:41-232, AGR_BWE_LPC_synthesizer.c:29-52, AGR_BWE_qmf.c:86-182,
 //   AGR_BWE_quant_highband.c:114-128, AGR_BWE_SDK_API.c:172-279,
@@ -640,18 +643,25 @@ SB_HD void qmf_synth_group(const float* xx1, const float* xx2, const float* a, i
     y4[0] = 2.f * y0; y4[1] = 2.f * y1; y4[2] = 2.f * y2; y4[3] = 2.f * y3;
 }
 
-// ---- AGR_Sate_qmf_synth, float branch (AGR_BWE_qmf.c:86-182), N = 2 * N2 = 640 or 320, M = 64 ----------------------
-SB_FN void qmf_synth_f32(const float* x1, const float* x2, float* y, float* mem1, float* mem2, int N2) {
-    enum { M = 64, M2 = 32, N2MAX = PACKET / 2 };
+// ---- scalar model of the synthesis kernel: AGR_Sate_qmf_synth, float branch (AGR_BWE_qmf.c:86-182), N = 2 * N2 = 640
+// or 320, M = 64, then the truncation to int16 (AGR_BWE_decode_frame_FLP.c:222-231).  low / high: the band signals
+// dec_packet handed out.
+SB_FN void dec_synth(DecState* st, const i16* low, const float* high, i16* pcm) {
+    enum { M2 = 32, N2MAX = PACKET / 2 };
+    const int N2 = st->frames_per_packet * FRAME;
     float xx1[M2 + N2MAX], xx2[M2 + N2MAX];
     const float* a = SB_T(qmf_flt);
-    for (int i = 0; i < N2; i++) xx1[i] = x1[N2 - 1 - i];
-    for (int i = 0; i < M2; i++) xx1[N2 + i] = mem1[2 * i + 1];
-    for (int i = 0; i < N2; i++) xx2[i] = x2[N2 - 1 - i];
-    for (int i = 0; i < M2; i++) xx2[N2 + i] = mem2[2 * i + 1];
-    for (int i = 0; i < N2; i += 2) qmf_synth_group(xx1, xx2, a, N2, i, &y[2 * i]);
-    for (int i = 0; i < M2; i++) mem1[2 * i + 1] = xx1[i];
-    for (int i = 0; i < M2; i++) mem2[2 * i + 1] = xx2[i];
+    for (int i = 0; i < N2; i++) { xx1[i] = (float)low[N2 - 1 - i]; xx2[i] = high[N2 - 1 - i]; }
+    for (int i = 0; i < M2; i++) { xx1[N2 + i] = st->g0_mem[2 * i + 1]; xx2[N2 + i] = st->g1_mem[2 * i + 1]; }
+    for (int i = 0; i < N2; i += 2) {
+        float y4[4];
+        qmf_synth_group(xx1, xx2, a, N2, i, y4);
+        for (int q = 0; q < 4; q++) {
+            const i32 t = trunc_i32((double)y4[q]);
+            pcm[2 * i + q] = (i16)(t > 32767 ? 32767 : (t < -32768 ? -32768 : t));
+        }
+    }
+    for (int i = 0; i < M2; i++) { st->g0_mem[2 * i + 1] = xx1[i]; st->g1_mem[2 * i + 1] = xx2[i]; }
 }
 
 // ---- AGR_Bwe_decode_frame_FLP (AGR_BWE_decode_frame_FLP.c:41-130): one 20 ms high-band frame ------------------------
@@ -733,16 +743,17 @@ struct DecPacketWork {
     alignas(16) i16 lowout[PACKET / 2];
     i32 res_Q10[PACKET / 2];
     alignas(16) float OutHigh[PACKET / 2];
-    float OutLow[PACKET / 2], out[PACKET];     // only the scalar model (bands == nullptr) uses these two
 };
 
-// Band signals handed from the decoder kernel to the synthesis-filter-bank kernel (device pipeline): int16 low band and
-// float high band of the packet.  With bands == nullptr dec_packet runs the filter bank itself (scalar model).
+// Band signals handed from the decoder kernel to the synthesis-filter-bank kernel: int16 low band and float high band of
+// the packet (16-byte aligned on the device).
 struct DecBands { i16* low; float* high; };
 
 // bits/cap: payload row as handed in by the caller; nb: {n0, n1} (not modified); returns the reference's return code.
-SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, i16* vout, const u8* bits, int cap, const i16* nb_in, i32 lostflag, DecStale* stale = nullptr,
-                     const DecBands* bands = nullptr) {
+// Everything up to the synthesis filter bank: on 0 the band signals are in `bands`, and dec_synth (the synthesis kernel)
+// turns them into PCM.
+SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, const u8* bits, int cap, const i16* nb_in, i32 lostflag, DecStale* stale,
+                     const DecBands* bands) {
     if (nb_in[0] <= 0) return -1;
     if (lostflag < 1 || lostflag > 4) return -1;
     // frame control starts from zeros: after a rejected (corrupted) frame a few of its fields are read before anything
@@ -759,8 +770,7 @@ SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, i16* vout, const u8* bits, 
     for (int k = 0; k < 2; k++) {   // fully defined even for a description this packet does not carry
         rc[k].base_Q32 = 0; rc[k].range_Q16 = 0; rc[k].bufferIx = 0; rc[k].error = 0; rc[k].bufLen = 0; rc[k].buf = W->pay[k];
     }
-    bool cont = st->moreInternalDecoderFrames != 0;   // only after a corrupted packet, see DecStale
-    if (cont && !stale) { st->moreInternalDecoderFrames = 0; cont = false; }   // no storage given: resynchronise on this packet
+    const bool cont = st->moreInternalDecoderFrames != 0;   // only after a corrupted packet, see DecStale
     if (cont) {
         for (int k = 0; k < 2; k++) {
             for (int i = 0; i < MAX_PAYLOAD + 8; i++) W->pay[k][i] = stale->pay[k][i];
@@ -796,7 +806,7 @@ SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, i16* vout, const u8* bits, 
         if (ret < 0) return ret;
         for (int i = 0; i < FRAME; i++) W->res_Q10[f * FRAME + i] = st->exc_Q10[i];
     }
-    if (st->moreInternalDecoderFrames && stale) {     // the payload outlives this call
+    if (st->moreInternalDecoderFrames) {     // the payload outlives this call
         for (int k = 0; k < 2; k++) {
             for (int i = 0; i < MAX_PAYLOAD + 8; i++) stale->pay[k][i] = W->pay[k][i];
             st->rc_base_Q32[k] = rc[k].base_Q32; st->rc_range_Q16[k] = rc[k].range_Q16;
@@ -812,27 +822,33 @@ SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, i16* vout, const u8* bits, 
         if (!hb_lost) for (int i = 0; i < 4; i++) hb4[i] = bits[hb_off + 4 * f + i];
         hb_decode_frame(st, hb4, W->OutHigh + f * F, res, lostflag);
     }
-    if (bands) {      // device pipeline: the 64-tap synthesis filter bank has no recurrence and runs as its own kernel
+    // the 64-tap synthesis filter bank has no recurrence: on the device it runs as its own kernel
 #ifdef __CUDA_ARCH__
-        const int4* sl = reinterpret_cast<const int4*>(W->lowout);
-        int4* dl = reinterpret_cast<int4*>(bands->low);
-        for (int i = 0; i < half / 8; i++) dl[i] = sl[i];
-        const float4* sh = reinterpret_cast<const float4*>(W->OutHigh);
-        float4* dh = reinterpret_cast<float4*>(bands->high);
-        for (int i = 0; i < half / 4; i++) dh[i] = sh[i];
+    const int4* sl = reinterpret_cast<const int4*>(W->lowout);
+    int4* dl = reinterpret_cast<int4*>(bands->low);
+    for (int i = 0; i < half / 8; i++) dl[i] = sl[i];
+    const float4* sh = reinterpret_cast<const float4*>(W->OutHigh);
+    float4* dh = reinterpret_cast<float4*>(bands->high);
+    for (int i = 0; i < half / 4; i++) dh[i] = sh[i];
 #else
-        for (int i = 0; i < half; i++) { bands->low[i] = W->lowout[i]; bands->high[i] = W->OutHigh[i]; }
+    for (int i = 0; i < half; i++) { bands->low[i] = W->lowout[i]; bands->high[i] = W->OutHigh[i]; }
 #endif
-        return 0;
-    }
-    for (int i = 0; i < half; i++) W->OutLow[i] = (float)W->lowout[i];
-    qmf_synth_f32(W->OutLow, W->OutHigh, W->out, st->g0_mem, st->g1_mem, half);
-    for (int i = 0; i < 2 * half; i++) {
-        i32 t = trunc_i32((double)W->out[i]);
-        if (t > 32767) t = 32767; else if (t < -32768) t = -32768;
-        vout[i] = (i16)t;
-    }
     return 0;
+}
+
+// The whole packet on one thread (host model): the decode kernel's dec_packet, then, for an accepted packet, the synthesis
+// kernel's dec_synth into vout (2 * nf * FRAME samples).  Without DecStale storage a packet that would continue in the
+// previous payload resynchronises on its own bytes instead.
+SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, i16* vout, const u8* bits, int cap, const i16* nb_in, i32 lostflag,
+                     DecStale* stale = nullptr) {
+    DecStale discard;
+    if (!stale) { st->moreInternalDecoderFrames = 0; stale = &discard; }
+    i16 low[PACKET / 2];
+    float high[PACKET / 2];
+    const DecBands bands = {low, high};
+    const i32 r = dec_packet(st, W, bits, cap, nb_in, lostflag, stale, &bands);
+    if (r == 0) dec_synth(st, low, high, vout);
+    return r;
 }
 
 }  // namespace sb

@@ -1,5 +1,10 @@
 // solo_b200 -- one SOLO packet (40 ms, 16 kHz) through the encoder: QMF split, two SILK frames with the
 // MD noise-shaping quantiser, two high-band frames, payload assembly [MD1 | MD2 | HB].
+// enc_packet is the scalar model of the device pipeline, stage by stage: band split, voice activity, core analysis,
+// high-band analysis, shaping filters, gains, prefilter, quantiser, entropy coding.  The band split (sharing
+// qmf_output_pair with its kernel), the core and high-band analysis, the quantiser and the entropy coding have scalar forms
+// here (those kernels run sb_coop.cuh, sb_nsq_warp.cuh and a two-thread form of enc_packet_finish); voice activity, shaping
+// filters, gains and prefilter are the functions their kernels call.
 // Reference: /root/reference/JC1_SDK_SRC_ARM/src/libBWE/AGR_BWE_encode_frame_FIX.c:8-174, AGR_BWE_qmf.c:38-80,
 // AGR_BWE_find_HB_LPC_FIX.c:4-49, AGR_BWE_quant_highband.c:23-147, AGR_BWE_SDK_API.c:11-152,
 // libSATECodec/SKP_Silk_enc_API.c:127-273, SKP_Silk_encode_frame_FIX.c:34-327, SKP_Silk_control_codec_FIX.c:232-389.
@@ -80,23 +85,12 @@ SB_HD void qmf_output_pair(const i16* x, const i16* aa, int k, i16* lo, i16* hi)
 }
 
 // ---- AGR_Sate_qmf_decomp (AGR_BWE_qmf.c:38-80), N = 640 or 320, M = 64, fixed point ------------------------------
+// (scalar model of the band-split kernel, which computes the same output pairs with qmf_output_pair)
 SB_FN void qmf_decomp(const i16* xx, i16* y1, i16* y2, i16* mem, int N) {
     enum { M = 64 };
     i16 x[PACKET + M - 1];
     const i16* aa = SB_T(qmf_fix);
     for (int i = 0; i < M - 1; i++) x[i] = mem[M - i - 2];
-#ifdef __CUDA_ARCH__
-    if ((((size_t)xx) & 15) == 0) {          // PCM rows of the batch buffers: 128-bit loads straight from global memory
-        const int4* src = reinterpret_cast<const int4*>(xx);
-#pragma unroll 2
-        for (int i = 0; i < N / 8; i++) {
-            const int4 v = src[i];
-            i16* d = &x[8 * i + M - 1];
-            d[0] = (i16)((i16)v.x >> 1); d[1] = (i16)(v.x >> 17); d[2] = (i16)((i16)v.y >> 1); d[3] = (i16)(v.y >> 17);
-            d[4] = (i16)((i16)v.z >> 1); d[5] = (i16)(v.z >> 17); d[6] = (i16)((i16)v.w >> 1); d[7] = (i16)(v.w >> 17);
-        }
-    } else
-#endif
     for (int i = 0; i < N; i++) x[i + M - 1] = (i16)(xx[i] >> 1);
     for (int i = 0; i < M - 1; i++) mem[i] = x[N + M - 2 - i];   // == xx[N - i - 1] >> 1
     for (int k = 0; k < N / 2; k++) qmf_output_pair(x, aa, k, &y1[k], &y2[k]);
@@ -184,55 +178,52 @@ SB_FN void hb_pack_frame(i32 lsp_idx, const i32* nrg0, const i16* r16, u8* out4,
     out4[0] = (u8)(w >> 24); out4[1] = (u8)(w >> 16); out4[2] = (u8)(w >> 8); out4[3] = (u8)w;
 }
 
-// Working set of stage A for one stream in the scalar model (tests/hostsim); the device kernels use CoopWork (sb_coop.cuh).
+// Working set of the scalar core analysis (tests/hostsim); the analysis kernel's is CoopWork (sb_coop.cuh).
 struct EncAnalysisWork {
-    i16 low[PACKET / 2], high[PACKET / 2];
+    i16 low[PACKET / 2], high[PACKET / 2];   // band signals of the packet
     i16 pIn_HP[FRAME];
     i16 res_pitch[2 * FRAME + LA_PITCH];
-    EncCtrl c;                 // control of the frame being analysed (copied to EncScratch when the frame is done)
-    i16 xfw[FRAME];
-    i32 vadFlag;
-    const NlsfFastTabs* nlsf_fast;   // optional copies of the NLSF codebooks (null: use the global tables)
+    const NlsfFastTabs* nlsf_fast;   // not read: the scalar model searches the NLSF codebooks in the global tables
 };
 
-// SKP_Silk_encode_frame_FIX (encode_frame_FIX.c:34-131, 151-165, 199-208) up to the quantiser, for one frame (scalar model).
-SB_FN void encode_frame_analysis(EncCore* st, EncAnalysisWork* W, const i16* pIn, int frame_in_packet) {
-    EncCtrl* c = &W->c;
+// SKP_Silk_encode_frame_FIX (encode_frame_FIX.c:34-131) up to the quantised NLSFs, for frame f of the packet: the scalar
+// model of the core-analysis kernel (c_encode_frame_analysis).  Reads the frame's voice activity from scr and writes what
+// the kernel writes there: c[f], x_hp[f], ar_Q24[f], shape_par[f], nlsf_Q15[f], lpc_in_pre[f], local_gains[f].
+SB_FN void encode_frame_analysis(EncSilk* st, EncAnalysisWork* W, EncScratch* scr, int f) {
+    EncCtrl* c = &scr->c[f];
     i16* x_frame = st->x_buf + FRAME;
     c->Seed = st->frameCounter++ & 3;
-    vad_get_sa_q8(&st->vad, &st->speech_activity_Q8, c->input_quality_bands_Q15, &c->input_tilt_Q15, pIn);
-    hp_variable_cutoff(st, c, W->pIn_HP, pIn);
+    st->speech_activity_Q8 = scr->vad_sa_Q8[f];
+    for (int b = 0; b < 4; b++) c->input_quality_bands_Q15[b] = scr->vad_quality_Q15[f][b];
+    c->input_tilt_Q15 = scr->vad_tilt_Q15[f];
+    hp_variable_cutoff(st, c, W->pIn_HP, W->low + f * FRAME);
     for (int i = 0; i < FRAME; i++) x_frame[LA_SHAPE + i] = W->pIn_HP[i];  // LP_variable_cutoff is a copy (transition_frame_no == 0)
     find_pitch_lags(st, c, W->res_pitch, x_frame);
-    noise_shape_analysis(st, c, W->res_pitch + FRAME, x_frame);
-    prefilter(st, c, W->xfw, x_frame);
-    find_pred_coefs(st, c, W->res_pitch, frame_in_packet, W->nlsf_fast);
-    process_gains(st, c, frame_in_packet);
-    vad_flag_and_dtx(st, &W->vadFlag);
+    noise_shape_analysis(st, c, W->res_pitch + FRAME, x_frame, scr->ar_Q24[f], scr->shape_par[f]);
+    find_pred_coefs(st, c, W->res_pitch, scr, f);
+    for (int i = 0; i < FRAME; i++) scr->x_hp[f][i] = x_frame[i];    // the prefilter's input: the frame as the analysis saw it
     for (int i = 0; i < FRAME + LA_SHAPE; i++) st->x_buf[i] = st->x_buf[FRAME + i];
     st->prev_sigtype = c->sigtype;
     st->prevLag = c->pitchL[NB_SUBFR - 1];
     st->first_frame_after_reset = 0;
 }
 
-// stage A (scalar model): band split, two core frames, high-band frames
-SB_FN void enc_packet_analysis(EncCore* st, EncAnalysisWork* W, const i16* pcm, EncScratch* scr, const i16* bands = nullptr) {
+// scalar model of the core-analysis kernel (c_enc_packet_analysis): every frame of the packet
+SB_FN void enc_packet_analysis(EncSilk* st, EncAnalysisWork* W, EncScratch* scr) {
+    for (int f = 0; f < st->frames_per_packet; f++) encode_frame_analysis(st, W, scr, f);
+}
+// scalar model of the high-band kernel: every high-band frame of the packet
+SB_FN void hb_analyse_packet(EncCore* st, const i16* high, EncScratch* scr) {
+    const int nhb = st->frames_per_packet * FRAME / st->hb_frame;
+    for (int f = 0; f < nhb; f++) hb_analyse_frame(st, high + f * st->hb_frame, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
+}
+// the kernels between the analysis and the quantiser, which the device and the scalar model share: shaping filters,
+// gain processing, prefilter
+SB_FN void enc_packet_post_analysis(EncSilk* st, EncScratch* scr) {
     const int nf = st->frames_per_packet;
-    if (bands) {
-        const int half = nf * FRAME;
-        for (int i = 0; i < half; i++) { W->low[i] = bands[i]; W->high[i] = bands[half + i]; }
-    } else {
-        qmf_decomp(pcm, W->low, W->high, st->qmf_mem, nf * 2 * FRAME);
-    }
-    for (int f = 0; f < nf; f++) {
-        encode_frame_analysis(st, W, W->low + f * FRAME, f);
-        scr->c[f] = W->c;
-        for (int i = 0; i < FRAME; i++) scr->xfw[f][i] = W->xfw[i];
-        scr->vadFlag[f] = W->vadFlag;
-    }
-    scr->dtx_drop = (st->useDTX && st->inDTX) ? 1 : 0;
-    const int nhb = nf * FRAME / st->hb_frame;    // high-band frames per packet
-    for (int f = 0; f < nhb; f++) hb_analyse_frame(st, W->high + f * st->hb_frame, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
+    for (int f = 0; f < nf; f++) for (int k = 0; k < NB_SUBFR; k++) shape_post_window(scr, f, k);
+    gains_packet(st, scr, nf);
+    prefilter_packet(st, scr, nf);
 }
 
 // stage C: AGR_Sate_Encoder_Encode tail -- returns the byte count; nBytesOut[0] = total, nBytesOut[1] = len(MD2) + 8
@@ -270,7 +261,7 @@ SB_FN i32 enc_packet_finish(EncCore* st, const EncScratch* scr, u8* rcbuf /* MAX
     return imin(out_cap, total);
 }
 
-// Whole packet on one thread (host model used by tests/hostsim; the device runs stage B as a warp-per-stream kernel).
+// Whole packet on one thread: the scalar model of the device pipeline (tests/hostsim).
 struct EncPacketWork {
     EncAnalysisWork a;
     EncScratch scr;
@@ -278,7 +269,13 @@ struct EncPacketWork {
     i32 r[FRAME];
     u8 rcbuf[MAX_PAYLOAD];
 };
-// stages B (scalar model of the quantiser) + C on one thread
+// band split and voice activity of the packet (the first two kernels)
+SB_FN void enc_packet_bands(EncState* st, EncPacketWork* W, const i16* pcm) {
+    const int nf = st->frames_per_packet;
+    qmf_decomp(pcm, W->a.low, W->a.high, st->qmf_mem, nf * 2 * FRAME);
+    vad_packet(&st->vad, W->a.low, nf, W->scr.vad_sa_Q8, W->scr.vad_quality_Q15, W->scr.vad_tilt_Q15);
+}
+// scalar model of the quantiser kernel, then the entropy coding
 SB_FN i32 enc_packet_quantise_and_code(EncState* st, EncPacketWork* W, u8* out, i32 out_cap, i16* nBytesOut) {
     for (int f = 0; f < st->frames_per_packet; f++) {
         nsq_del_dec(st, &W->scr.c[f], &W->nsq, W->scr.xfw[f], (i8*)0, W->scr.q_md[f][0], W->scr.q_md[f][1], W->r);
@@ -286,8 +283,12 @@ SB_FN i32 enc_packet_quantise_and_code(EncState* st, EncPacketWork* W, u8* out, 
     }
     return enc_packet_finish(st, &W->scr, W->rcbuf, out, out_cap, nBytesOut);
 }
+// the device pipeline's stages in its order
 SB_FN i32 enc_packet(EncState* st, EncPacketWork* W, const i16* pcm, u8* out, i32 out_cap, i16* nBytesOut) {
-    enc_packet_analysis(st, &W->a, pcm, &W->scr);
+    enc_packet_bands(st, W, pcm);
+    enc_packet_analysis(st, &W->a, &W->scr);
+    hb_analyse_packet(st, W->a.high, &W->scr);
+    enc_packet_post_analysis(st, &W->scr);
     return enc_packet_quantise_and_code(st, W, out, out_cap, nBytesOut);
 }
 

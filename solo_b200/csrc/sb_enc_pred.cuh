@@ -553,7 +553,7 @@ SB_FN void nlsf_msvq_encode(i32* NLSFIndices, i32* pNLSF_Q15, const NlsfCb& cb, 
 }
 
 // ---- SKP_Silk_process_NLSFs_FIX.c:31-127 ----------------------------------------------------------------
-// Optional low-latency copies of the two NLSF codebooks (vectors + rates, 4.2 KB): the analysis kernel keeps them in
+// Low-latency copies of the two NLSF codebooks (vectors + rates, 4.2 KB): the analysis kernel keeps them in
 // shared memory because the MSVQ gathers code vectors by data-dependent index ~1 000 times per frame.
 struct NlsfFastTabs {
     i16 cb0[1200], rates0[120], cb1[720], rates1[72];
@@ -564,7 +564,9 @@ SB_FN void nlsf_fast_tabs_fill(NlsfFastTabs* T, int tid, int nthreads) {
     for (int i = tid; i < 720; i += nthreads) T->cb1[i] = SB_T(nlsf_cb1_q15)[i];
     for (int i = tid; i < 72; i += nthreads) T->rates1[i] = SB_T(nlsf_cb1_rates_q5)[i];
 }
-SB_FN void process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, const NlsfFastTabs* fast = nullptr) {
+// Up to the quantised NLSFs of the two half-frames, nlsf_out = {interpolated first half, second half}; gains_packet turns
+// them into the prediction filters (:108-127).
+SB_FN void process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, i32 (*nlsf_out)[LPC_ORDER]) {
     i32 pNLSFW_Q6[LPC_ORDER], pNLSF0_temp_Q15[LPC_ORDER], pNLSFW0_temp_Q6[LPC_ORDER];
     i32 NLSF_mu_Q15, NLSF_mu_fluc_red_Q16;
     if (c->sigtype == 0) {
@@ -583,20 +585,10 @@ SB_FN void process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, const NlsfFast
         i32 i_sqr_Q15 = shl(smulbb(c->NLSFInterpCoef_Q2, c->NLSFInterpCoef_Q2), 11);
         for (int i = 0; i < LPC_ORDER; i++) pNLSFW_Q6[i] = smlawb(pNLSFW_Q6[i] >> 1, pNLSFW0_temp_Q6[i], i_sqr_Q15);
     }
-    NlsfCb cb = nlsf_cb(c->sigtype);
-    if (fast) {
-        cb.cb_q15 = c->sigtype == 0 ? fast->cb0 : fast->cb1;
-        cb.rates_q5 = c->sigtype == 0 ? fast->rates0 : fast->rates1;
-    }
-    nlsf_msvq_encode(c->NLSFIndices, pNLSF_Q15, cb, st->prev_NLSFq_Q15, pNLSFW_Q6, NLSF_mu_Q15, NLSF_mu_fluc_red_Q16,
+    nlsf_msvq_encode(c->NLSFIndices, pNLSF_Q15, nlsf_cb(c->sigtype), st->prev_NLSFq_Q15, pNLSFW_Q6, NLSF_mu_Q15, NLSF_mu_fluc_red_Q16,
                      st->first_frame_after_reset);
-    nlsf2a_stable(c->PredCoef_Q12[1], pNLSF_Q15, LPC_ORDER);
-    if (doInterpolate) {
-        interpolate(pNLSF0_temp_Q15, st->prev_NLSFq_Q15, pNLSF_Q15, c->NLSFInterpCoef_Q2, LPC_ORDER);
-        nlsf2a_stable(c->PredCoef_Q12[0], pNLSF0_temp_Q15, LPC_ORDER);
-    } else {
-        for (int i = 0; i < LPC_ORDER; i++) c->PredCoef_Q12[0][i] = c->PredCoef_Q12[1][i];
-    }
+    for (int i = 0; i < LPC_ORDER; i++) nlsf_out[0][i] = nlsf_out[1][i] = pNLSF_Q15[i];
+    if (doInterpolate) interpolate(nlsf_out[0], st->prev_NLSFq_Q15, pNLSF_Q15, c->NLSFInterpCoef_Q2, LPC_ORDER);
 }
 
 // ---- SKP_Silk_residual_energy_FIX.c:32-92 ------------------------------------------------------------------
@@ -626,11 +618,13 @@ SB_FN void residual_energy(i32* nrgs, i32* nrgsQ, const i16* x, const i16 a_Q12[
 }
 
 // ---- SKP_Silk_find_pred_coefs_FIX.c:31-131 -----------------------------------------------------------------
-SB_FN void find_pred_coefs(EncSilk* st, EncCtrl* c, const i16* res_pitch, int frame_in_packet, const NlsfFastTabs* fast = nullptr) {
+// Up to the quantised NLSFs: frame f's hand-over to gains_packet (nlsf_Q15, lpc_in_pre, local_gains) goes to scr.
+SB_FN void find_pred_coefs(EncSilk* st, EncCtrl* c, const i16* res_pitch, EncScratch* scr, int frame_in_packet) {
     i32 WLTP[NB_SUBFR * LTP_ORDER * LTP_ORDER];
-    i32 invGains_Q16[NB_SUBFR], local_gains[NB_SUBFR], Wght_Q15[NB_SUBFR], LTP_corrs_rshift[NB_SUBFR];
+    i32 invGains_Q16[NB_SUBFR], Wght_Q15[NB_SUBFR], LTP_corrs_rshift[NB_SUBFR];
     i32 NLSF_Q15[LPC_ORDER];
-    i16 LPC_in_pre[NB_SUBFR * LPC_ORDER + FRAME];
+    i32* local_gains = scr->local_gains[frame_in_packet];
+    i16* LPC_in_pre = scr->lpc_in_pre[frame_in_packet];
     i32 min_gain_Q16 = SB_I32_MAX >> 6;
     for (int i = 0; i < NB_SUBFR; i++) min_gain_Q16 = imin(min_gain_Q16, c->Gains_Q16[i]);
     for (int i = 0; i < NB_SUBFR; i++) {
@@ -658,8 +652,7 @@ SB_FN void find_pred_coefs(EncSilk* st, EncCtrl* c, const i16* res_pitch, int fr
     }
     find_lpc(NLSF_Q15, &c->NLSFInterpCoef_Q2, st->prev_NLSFq_Q15, 1 * (1 - st->first_frame_after_reset), LPC_ORDER, LPC_in_pre,
              SUBFR + LPC_ORDER);
-    process_nlsfs(st, c, NLSF_Q15, fast);
-    residual_energy(c->ResNrg, c->ResNrgQ, LPC_in_pre, c->PredCoef_Q12, local_gains);
+    process_nlsfs(st, c, NLSF_Q15, scr->nlsf_Q15[frame_in_packet]);
     for (int i = 0; i < LPC_ORDER; i++) st->prev_NLSFq_Q15[i] = NLSF_Q15[i];
 }
 

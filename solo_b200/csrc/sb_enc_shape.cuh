@@ -105,8 +105,10 @@ SB_FN void limit_warped_coefs(i32* syn_Q24, i32* ana_Q24, i32 lambda_Q16, i32 li
 }
 
 // ---- SKP_Silk_noise_shape_analysis_FIX.c:137-531 ---------------------------------------------------------
-// pitch_res points at res_pitch + FRAME, x at x_buf + FRAME.
-SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, const i16* x) {
+// pitch_res points at res_pitch + FRAME, x at x_buf + FRAME.  Stops, as the analysis kernel does, after the bandwidth
+// expansion of each window: ar_Q24[k] = {AR2, AR1} and shape_par = {warping_Q16, de-essing multiplier Q16} go to
+// shape_post_window, which finishes the filters and the pre-gains.
+SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, const i16* x, i32 (*ar_Q24)[2][SHAPE_ORDER], i32* shape_par) {
     i32 auto_corr[SHAPE_ORDER + 1], refl_coef_Q16[SHAPE_ORDER], AR1_Q24[SHAPE_ORDER], AR2_Q24[SHAPE_ORDER];
     i16 x_windowed[SHAPE_WIN];
     i32 scale = 0, nrg;
@@ -190,16 +192,7 @@ SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, c
         bwexpander_32(AR2_Q24, SHAPE_ORDER, BWExp2_Q16);
         for (int i = 0; i < SHAPE_ORDER; i++) AR1_Q24[i] = AR2_Q24[i];
         bwexpander_32(AR1_Q24, SHAPE_ORDER, BWExp1_Q16);
-        i32 pre_nrg_Q30;
-        lpc_inv_pred_gain_q24(&pre_nrg_Q30, AR2_Q24, SHAPE_ORDER);
-        lpc_inv_pred_gain_q24(&nrg, AR1_Q24, SHAPE_ORDER);
-        pre_nrg_Q30 = shl(smulwb(pre_nrg_Q30, SB_FIXC(0.7, 15)), 1);
-        c->GainsPre_Q14[k] = SB_FIXC(0.3, 14) + div32_varq(pre_nrg_Q30, nrg, 14);
-        limit_warped_coefs(AR2_Q24, AR1_Q24, warping_Q16, SB_FIXC(3.999, 24), SHAPE_ORDER);
-        for (int i = 0; i < SHAPE_ORDER; i++) {
-            c->AR1_Q13[k * SHAPE_ORDER + i] = (i16)sat16(rshift_round(AR1_Q24[i], 11));
-            c->AR2_Q13[k * SHAPE_ORDER + i] = (i16)sat16(rshift_round(AR2_Q24[i], 11));
-        }
+        for (int i = 0; i < SHAPE_ORDER; i++) { ar_Q24[k][0][i] = AR2_Q24[i]; ar_Q24[k][1][i] = AR1_Q24[i]; }
     }
 
     // gain tweaking
@@ -221,8 +214,8 @@ SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, c
     }
 
     // de-essing factor: fs == 8 kHz takes no branch (noise_shape_analysis_FIX.c:438-457)
-    gain_mult_Q16 = SB_FIXC(1.0, 16) + rshift_round(mlaw(SB_FIXC(0.05f, 26), c->coding_quality_Q14, SB_FIXC(0.1f, 12)), 10);
-    for (int k = 0; k < NB_SUBFR; k++) c->GainsPre_Q14[k] = smulwb(gain_mult_Q16, c->GainsPre_Q14[k]);
+    shape_par[0] = warping_Q16;
+    shape_par[1] = SB_FIXC(1.0, 16) + rshift_round(mlaw(SB_FIXC(0.05f, 26), c->coding_quality_Q14, SB_FIXC(0.1f, 12)), 10);
 
     // low-frequency shaping and noise tilt
     strength_Q16 = mulw(SB_FIXC(3.0f, 0), SB_FIXC(1.0, 16) + smulbb(SB_FIXC(0.5f, 1), c->input_quality_bands_Q15[0] - SB_FIXC(1.0, 15)));
@@ -296,8 +289,12 @@ SB_FN void warped_lpc_analysis_filter(i32* state, i16* res, const i16* coef_Q13,
 }
 
 // ---- SKP_Silk_prefilter_FIX.c:85-224 -------------------------------------------------------------------
-// ST: EncSilk, or any struct with the pf_* fields (the prefilter kernel works on a thread-private PrefState)
-template <class ST> SB_FN void prefilter(ST* st, const EncCtrl* c, i16* xw, const i16* x) {
+struct PrefState {      // the prefilter's part of EncSilk
+    i16 pf_sLTP_shp[LTP_BUF];
+    i32 pf_sAR_shp[SHAPE_ORDER + 1];
+    i32 pf_sLTP_shp_buf_idx, pf_sLF_AR_shp_Q12, pf_sLF_MA_shp_Q12, pf_sHarmHP, pf_lagPrev;
+};
+SB_FN void prefilter(PrefState* st, const EncCtrl* c, i16* xw, const i16* x) {
     i32 x_filt_Q12[SUBFR];
     i16 st_res[SUBFR];
     const i16* px = x;
@@ -371,11 +368,6 @@ SB_FN void shape_post_window(EncScratch* scr, int f, int k) {
     c->GainsPre_Q14[k] = smulwb(scr->shape_par[f][1], gains_pre);
 }
 // (2) the prefilter of every frame of the packet (its output feeds only the quantiser)
-struct PrefState {      // the prefilter's part of EncSilk
-    i16 pf_sLTP_shp[LTP_BUF];
-    i32 pf_sAR_shp[SHAPE_ORDER + 1];
-    i32 pf_sLTP_shp_buf_idx, pf_sLF_AR_shp_Q12, pf_sLF_MA_shp_Q12, pf_sHarmHP, pf_lagPrev;
-};
 SB_FN void prefilter_packet(EncSilk* st, EncScratch* scr, int nf) {
     PrefState ps;        // thread-private copy: on the device the recursion then runs out of registers / local memory
     for (int i = 0; i < LTP_BUF; i++) ps.pf_sLTP_shp[i] = st->pf_sLTP_shp[i];

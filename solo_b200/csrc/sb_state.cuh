@@ -134,9 +134,15 @@ struct EncCtrl {
 };
 
 // ---- per-packet hand-over between the encoder stages (device: global scratch, one slot per stream) -------------------
-//   stage A (analysis, one thread per stream)   : [QMF split, its own kernel on the device,] VAD .. process_gains per frame, high-band analysis
-//   stage B (MD noise-shaping quantiser)         : consumes c[f], xfw[f]; produces q_md[f], r16[f], c[f].Seed
-//   stage C (entropy coding + packing)           : range-codes both descriptions, high-band gains, payload assembly
+// The scalar model (sb_enc.cuh enc_packet) fills the same fields in the same order.
+//   stage A (analysis): VAD of the packet's frames           -> vad_*
+//                       core analysis (warp per stream)      -> c[f], x_hp, ar_Q24, shape_par, nlsf_Q15, lpc_in_pre, local_gains
+//                       high-band analysis (warp per stream) -> hb_lsp_idx, hb_nrg0
+//                       shaping filters (thread per window)  -> c[f] AR1 / AR2 / GainsPre
+//                       gains (thread per stream)            -> c[f] prediction filters, gains, vadFlag, dtx_drop
+//                       prefilter (thread per stream)        -> xfw
+//   stage B (MD noise-shaping quantiser)                     : consumes c[f], xfw[f]; produces q_md[f], r16[f], c[f].Seed
+//   stage C (entropy coding + packing)                       : range-codes both descriptions, high-band gains, payload assembly
 struct EncScratch {
     EncCtrl c[2];
     i16 xfw[2][FRAME];

@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(D
     DecPacketWork W;
     i16 nb[2] = {nbytes[2 * s], nbytes[2 * s + 1]};
     const DecBands bands = {band_low + (size_t)s * (spp / 2), band_high + (size_t)s * (spp / 2)};
-    i32 r = dec_packet(&states[s], &W, nullptr, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
+    i32 r = dec_packet(&states[s], &W, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
     if (ret) ret[s] = r;
     ret_int[s] = r;
 }

@@ -162,25 +162,16 @@ struct HsEnc { sb::EncState st; sb::EncPacketWork w; };
 void* hs_enc_create3(int rate, int dtx, int mdi, int framesize_ms, int joint_hb) {
     HsEnc* h = (HsEnc*)calloc(1, sizeof(HsEnc));
     sb::enc_state_init(&h->st, rate, dtx, mdi, framesize_ms, joint_hb);
-    h->w.a.nlsf_fast = nullptr;
     return h;
 }
-void* hs_enc_create2(int rate, int dtx, int mdi, int framesize_ms) { return hs_enc_create3(rate, dtx, mdi, framesize_ms, 0); }
-void* hs_enc_create(int rate, int dtx, int mdi) { return hs_enc_create2(rate, dtx, mdi, 40); }
 #ifdef SB_EMU
-// the device pipeline up to the quantiser: band split (kernel A0), VAD, core analysis (cooperative), the thread-per-stream
-// kernels behind it, high-band analysis (cooperative)
-static void emu_front(HsEnc* h, const short* pcm) {
+// the core and high-band analysis kernels' code (sb_coop.cuh) on emulated lanes
+static void emu_analysis(HsEnc* h) {
     static sb::CoopWork cw;
-    const int nf = h->st.frames_per_packet;
-    sb::qmf_decomp(pcm, h->w.a.low, h->w.a.high, h->st.qmf_mem, nf * 2 * sb::FRAME);
-    for (int i = 0; i < nf * sb::FRAME; i++) cw.low[i] = h->w.a.low[i];
-    sb::vad_packet(&h->st.vad, h->w.a.low, nf, h->w.scr.vad_sa_Q8, h->w.scr.vad_quality_Q15, h->w.scr.vad_tilt_Q15);   // the VAD kernel
-    sb::emu::run32([=]() { sb::c_enc_packet_analysis(&h->st, &cw, &h->w.scr); });
-    for (int f = 0; f < nf; f++) for (int k = 0; k < sb::NB_SUBFR; k++) sb::shape_post_window(&h->w.scr, f, k);   // shaping-filter kernel
-    sb::gains_packet(&h->st, &h->w.scr, nf);                                                                      // gain kernel
-    sb::prefilter_packet(&h->st, &h->w.scr, nf);                                                                  // prefilter kernel
     static sb::HbScr hs;
+    const int nf = h->st.frames_per_packet;
+    for (int i = 0; i < nf * sb::FRAME; i++) cw.low[i] = h->w.a.low[i];
+    sb::emu::run32([=]() { sb::c_enc_packet_analysis(&h->st, &cw, &h->w.scr); });
     sb::emu::run32([=]() {
         for (int f = 0; f < nf * sb::FRAME / h->st.hb_frame; f++) {
             if (h->st.hb_frame == sb::HB_FRAME) sb::c_hb_analyse_frame<sb::HB_FRAME>(&h->st, &hs, h->w.a.high + f * h->st.hb_frame, &h->w.scr.hb_lsp_idx[f], h->w.scr.hb_nrg0[f]);
@@ -201,19 +192,28 @@ static void emu_nsq(HsEnc* const* hh) {
         });
 }
 #endif
+// the stages of sb::enc_packet up to the quantiser; the emulated build swaps in the cooperative analysis
+static void enc_front(HsEnc* h, const short* pcm) {
+    sb::enc_packet_bands(&h->st, &h->w, pcm);
+#ifdef SB_EMU
+    emu_analysis(h);
+#else
+    sb::enc_packet_analysis(&h->st, &h->w.a, &h->w.scr);
+    sb::hb_analyse_packet(&h->st, h->w.a.high, &h->w.scr);
+#endif
+    sb::enc_packet_post_analysis(&h->st, &h->w.scr);
+}
 int hs_enc_encode(void* p, const short* pcm, unsigned char* out, int cap, short* nb) {
     HsEnc* h = (HsEnc*)p;
+    enc_front(h, pcm);
 #ifdef SB_EMU
-    emu_front(h, pcm);
     if (g_emu_nsq) {      // second lane group (SB_NSQ_GW = 16): shadows the same stream, as the kernel does for an odd batch
         HsEnc* hh[2] = {h, h};
         emu_nsq(hh);
         return sb::enc_packet_finish(&h->st, &h->w.scr, h->w.rcbuf, out, cap, nb);
     }
-    return sb::enc_packet_quantise_and_code(&h->st, &h->w, out, cap, nb);
-#else
-    return sb::enc_packet(&h->st, &h->w, pcm, out, cap, nb);
 #endif
+    return sb::enc_packet_quantise_and_code(&h->st, &h->w, out, cap, nb);
 }
 // two DIFFERENT streams through one emulated quantiser warp (SB_NSQ_GW = 16 build): the lane groups take their own paths
 // between the full-warp sample loops.  Both encoders must have the same packet length.  ret[g] = bytes of stream g.
@@ -222,8 +222,8 @@ int hs_enc_encode_pair(void* pa, void* pb, const short* pcm_a, const short* pcm_
 #if defined(SB_EMU) && defined(SB_EMU_GW16)
     HsEnc* hh[2] = {(HsEnc*)pa, (HsEnc*)pb};
     if (hh[0]->st.frames_per_packet != hh[1]->st.frames_per_packet) return -1;
-    emu_front(hh[0], pcm_a);
-    emu_front(hh[1], pcm_b);
+    enc_front(hh[0], pcm_a);
+    enc_front(hh[1], pcm_b);
     emu_nsq(hh);
     ret[0] = sb::enc_packet_finish(&hh[0]->st, &hh[0]->w.scr, hh[0]->w.rcbuf, out_a, cap, nb_a);
     ret[1] = sb::enc_packet_finish(&hh[1]->st, &hh[1]->w.scr, hh[1]->w.rcbuf, out_b, cap, nb_b);
@@ -240,10 +240,6 @@ int hs_is_emu() {
     return 0;
 #endif
 }
-int hs_enc_state_size() { return (int)sizeof(sb::EncState); }
-int hs_enc_work_size() { return (int)sizeof(sb::EncPacketWork); }
-void* hs_enc_state(void* p) { return &((HsEnc*)p)->st; }
-void* hs_enc_ctrl(void* p) { return &((HsEnc*)p)->w.scr.c[1]; }
 
 struct HsDec { sb::DecState st; sb::DecPacketWork w; sb::DecStale stale; };
 void* hs_dec_create3(int mdi, int framesize_ms, int joint_hb) {
@@ -251,14 +247,10 @@ void* hs_dec_create3(int mdi, int framesize_ms, int joint_hb) {
     sb::dec_state_init(&h->st, mdi, framesize_ms, joint_hb);
     return h;
 }
-void* hs_dec_create2(int mdi, int framesize_ms) { return hs_dec_create3(mdi, framesize_ms, 0); }
-void* hs_dec_create(int mdi) { return hs_dec_create2(mdi, 40); }
 // same calling convention as AGR_Sate_Decoder_Decode (payload pre-trimmed by the caller); nb is not modified
 int hs_dec_decode(void* p, short* pcm, const unsigned char* bits, int cap, const short* nb, int lostflag) {
     HsDec* h = (HsDec*)p;
     return sb::dec_packet(&h->st, &h->w, pcm, bits, cap, nb, lostflag, &h->stale);
 }
 void hs_dec_destroy(void* p) { free(p); }
-int hs_dec_state_size() { return (int)sizeof(sb::DecState); }
-int hs_dec_work_size() { return (int)sizeof(sb::DecPacketWork); }
 }

@@ -16,20 +16,12 @@ def lib(emu=None):
     emu = EMU if emu is None else emu
     if emu not in _libs:
         L = C.CDLL(build_hostsim.build(emu=emu))
-        L.hs_enc_create.restype = C.c_void_p
-        L.hs_enc_create.argtypes = [C.c_int, C.c_int, C.c_int]
-        L.hs_enc_create2.restype = C.c_void_p
-        L.hs_enc_create2.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
-        L.hs_dec_create2.restype = C.c_void_p
-        L.hs_dec_create2.argtypes = [C.c_int, C.c_int]
         L.hs_enc_create3.restype = C.c_void_p
         L.hs_enc_create3.argtypes = [C.c_int] * 5
         L.hs_dec_create3.restype = C.c_void_p
         L.hs_dec_create3.argtypes = [C.c_int] * 3
         L.hs_enc_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.hs_enc_destroy.argtypes = [C.c_void_p]
-        L.hs_dec_create.restype = C.c_void_p
-        L.hs_dec_create.argtypes = [C.c_int]
         L.hs_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.hs_dec_destroy.argtypes = [C.c_void_p]
         if emu:

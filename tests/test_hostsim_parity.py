@@ -1,10 +1,12 @@
 """Kernel arithmetic on the CPU: solo_b200/csrc/*.cuh compiled by g++ (tests/hostsim) against the golden fixtures and,
 where oracle/_ref is built, against the unmodified reference on inputs the fixtures do not cover.
 
-The headers are written once as __host__ __device__ code, so what passes here is the same source nvcc compiles into
-libsolo_b200.so (the warp-per-stream quantiser sb_nsq_warp.cuh is device-only; its scalar model sb_nsq.cuh runs here and
-the `-m gpu` suite pins the device version).  Bar: payloads and length fields byte-identical to the FIX build, PCM
-identical to the FLP build (north star allows +-1 LSB)."""
+The headers are written once as __host__ __device__ code, and the host model runs the device pipeline's stages in its
+order, so what passes here is the same source nvcc compiles into libsolo_b200.so: every encoder stage after the analysis
+and the decoder up to the synthesis filter bank are the kernels' own functions.  The warp-per-stream stages run here in
+their scalar forms, and in their device code (sb_coop.cuh, sb_nsq_warp.cuh) on 32 emulated lanes in the last two tests.
+Bar: payloads and length fields byte-identical to the FIX build, PCM identical to the FLP build (north star allows
++-1 LSB)."""
 import hashlib
 import struct
 
