@@ -73,12 +73,7 @@ __global__ void __launch_bounds__(SB_HB_WARPS * 32) sb_enc_hb_warp_kernel(EncSta
     copy16(&S->hb, static_cast<EncBands*>(&states[s]), (int)sizeof(EncBands), lane);
     copy16(S->high, bands + (size_t)s * spp + spp / 2, spp, lane);  // high band = second half of the row
     __syncwarp();
-    const int F = states[s].hb_frame, nhb = (spp / 2) / F;
-    EncScratch* scr = &scratch[s];
-    for (int f = 0; f < nhb; f++) {
-        if (F == HB_FRAME) c_hb_analyse_frame<HB_FRAME>(&S->hb, &S->H, S->high + f * F, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
-        else c_hb_analyse_frame<2 * HB_FRAME>(&S->hb, &S->H, S->high + f * F, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
-    }
+    c_hb_analyse_packet(&S->hb, &S->H, S->high, spp / 2, states[s].hb_frame, &scratch[s]);
     __syncwarp();
     // qmf_mem belongs to the band-split kernel: only the high-band ring and its flag go back
     copy16(static_cast<EncBands*>(&states[s])->x_hb_buf, S->hb.x_hb_buf, (int)(sizeof(EncBands) - offsetof(EncBands, x_hb_buf)), lane);
@@ -124,4 +119,3 @@ extern "C" int sb_phase_times_read(long long* stamps, int* lines, int cap) {
     return n;
 }
 #endif
-extern "C" int sb_analysis_smem_bytes(int which) { return which == 0 ? (int)sizeof(AnaSmem) : (int)sizeof(HbSmem); }

@@ -75,7 +75,6 @@ SB_HD i32 smulbb(i32 a, i32 b) { return (i32)(i16)a * (i32)(i16)b; }
 SB_HD i32 smlabb(i32 a, i32 b, i32 c) { return addw(a, smulbb(b, c)); }
 SB_HD i32 smulbt(i32 a, i32 b) { return (i32)(i16)a * (b >> 16); }
 SB_HD i32 smlabt(i32 a, i32 b, i32 c) { return addw(a, smulbt(b, c)); }
-SB_HD i32 smultt(i32 a, i32 b) { return (a >> 16) * (b >> 16); }
 // (a * (int16)b) >> 16, exact (macros.h:34)
 // Device form: (a * b16) >> 16 == high word of a * (b16 << 16); one IMAD.HI instead of a 64-bit product.
 SB_HD i32 smulwb(i32 a, i32 b) {
@@ -167,17 +166,6 @@ SB_HD i32 sqrt_approx(i32 x) {
     y >>= (lz >> 1);
     return smlawb(y, y, smulbb(213, frac));
 }
-SB_HD i32 norm16(i16 a) {
-    i32 a32 = a;
-    if (a32 == 0) return 0;
-    a32 ^= (a32 >> 31);
-    return clz32(a32) - 17;
-}
-SB_HD i32 norm32(i32 a) {
-    if (shl(a, 1) == 0) return 0;
-    a ^= (a >> 31);
-    return clz32(a) - 1;
-}
 // lin2log.c:41-48 ; log2lin.c:40-60
 SB_HD i32 lin2log(i32 x) {
     i32 lz, frac;
@@ -254,29 +242,6 @@ SB_HD_DIV i32 inverse32_varq(i32 b32, int qres) {
     if (lshift < 32) return result >> lshift;
     return 0;
 }
-
-// Inlines.h:219-275 (sine approximation, input 65536 == 2*pi)
-SB_HD i32 sin_approx_q24(i32 x) {
-    i32 y_q30;
-    x &= 65535;
-    if (x <= 32768) {
-        if (x < 16384) x = 16384 - x; else x -= 16384;
-        if (x < 1100) return smlawb(1 << 24, mulw(x, x), -5053);
-        x = smulwb(shl(x, 8), x);
-        y_q30 = smlawb(1059577, x, -5013);
-        y_q30 = smlaww(-82778932, x, y_q30);
-        y_q30 = smlaww(1073735400 + 66, x, y_q30);
-    } else {
-        if (x < 49152) x = 49152 - x; else x -= 49152;
-        if (x < 1100) return smlawb(-(1 << 24), mulw(x, x), 5053);
-        x = smulwb(shl(x, 8), x);
-        y_q30 = smlawb(-1059577, x, 5013);
-        y_q30 = smlaww(82778932, x, y_q30);
-        y_q30 = smlaww(-1073735400, x, y_q30);
-    }
-    return rshift_round(y_q30, 6);
-}
-SB_HD i32 cos_approx_q24(i32 x) { return sin_approx_q24(x + 16384); }
 
 // dither / PLC / CNG generator (SigProc_FIX.h:650)
 SB_HD i32 lcg_rand(i32 seed) { return mlaw(907633515, seed, 196314165); }

@@ -62,26 +62,6 @@ template <int ORD, bool SAT> SB_CFN void c_fir_zero_state(const i16* in, const i
     }
 }
 
-// SKP_Silk_sum_sqr_shift (sum_sqr_shift.c:40-98) over the whole warp.  The reference accumulates pair by pair and starts
-// shifting once the running sum reaches bit 31; the running sums are monotone, so when the exact total stays below 2^31
-// no shift ever happened and the result follows from the total (lanes over terms).  Otherwise lane 0 replays the scalar
-// routine.  All lanes return the same values.
-SB_CFN void c_sum_sqr_shift(i32* energy, i32* shift, const i16* x, int len, int odd_start) {
-    i64 part = 0;
-    SB_PARFOR(i, 0, len) part += (i64)((i32)x[i] * (i32)x[i]);
-    const i64 total = wsum64(part);
-    if (total < ((i64)1 << 31)) {      // uniform branch
-        i32 nrg = (i32)total, shft = 0;
-        if (nrg & 0xC0000000) { nrg = (i32)((u32)nrg >> 2); shft = 2; }
-        *energy = nrg; *shift = shft;
-        return;
-    }
-    i32 e = 0, s = 0;
-    if (SB_LANE0) sum_sqr_shift(&e, &s, x, len, odd_start);
-    *energy = wbcast(e, 0);
-    *shift = wbcast(s, 0);
-}
-
 // SKP_Silk_schur (schur.c:40-93), order <= 31: lane n keeps C[n][1] and C[n+k+1][0] in registers; the second slides down
 // one lane per step.  c: correlations (shared memory); rc_Q15: shared; returns the residual energy on every lane.
 SB_CFN i32 c_schur(i16* rc_Q15, const i32* c, int order) {
@@ -103,28 +83,6 @@ SB_CFN i32 c_schur(i16* rc_Q15, const i32* c, int order) {
     }
     return wbcast(a, 0);
 }
-// SKP_Silk_schur64 (schur64.c:42-91)
-SB_CFN i32 c_schur64(i32* rc_Q16, const i32* c, int order) {
-    const int lane = SB_LANE;
-    if (c[0] <= 0) {        // uniform
-        if (lane < order) rc_Q16[lane] = 0;
-        return 0;
-    }
-    i32 a = lane <= order ? c[lane] : 0;
-    i32 b = wshfl_down(a, 1);
-    for (int k = 0; k < order; k++) {
-        const i32 c00 = wbcast(b, 0), c01 = wbcast(a, 0);
-        const i32 rc_Q31 = div32_varq(negw(c00), c01, 31);
-        if (lane == 0) rc_Q16[k] = rshift_round(rc_Q31, 15);
-        if (lane < order - k) {
-            const i32 t1 = b, t2 = a;
-            b = addw(t1, smmul(shl(t2, 1), rc_Q31));
-            a = addw(t2, smmul(shl(t1, 1), rc_Q31));
-        }
-        b = wshfl_down(b, 1);
-    }
-    return wbcast(a, 0);
-}
 // SKP_Silk_k2a (k2a.c:40-60): lane n keeps A[n]; returns it (valid for n < order).  rc_Q15: shared memory.
 SB_CFN i32 c_k2a(const i16* rc_Q15, int order) {
     const int lane = SB_LANE;
@@ -134,18 +92,6 @@ SB_CFN i32 c_k2a(const i16* rc_Q15, int order) {
         const i32 t = wshfl(A, (k - lane - 1) & 31);
         if (lane < k) A = smlawb(A, shl(t, 1), rc);
         if (lane == k) A = negw(shl(rc, 9));
-    }
-    return A;
-}
-// SKP_Silk_k2a_Q16 (k2a_Q16.c:40-60)
-SB_CFN i32 c_k2a_q16(const i32* rc_Q16, int order) {
-    const int lane = SB_LANE;
-    i32 A = 0;
-    for (int k = 0; k < order; k++) {
-        const i32 rc = rc_Q16[k];
-        const i32 t = wshfl(A, (k - lane - 1) & 31);
-        if (lane < k) A = smlaww(A, t, rc);
-        if (lane == k) A = negw(shl(rc, 8));
     }
     return A;
 }
@@ -546,8 +492,8 @@ SB_CFN void c_warped_autocorr4(ShapeScr* S, i32 warping_Q16) {
 
 // ---- the per-window recursions with every array in registers (fixed order, fully unrolled): on the device these run as
 // one scalar instance per window, where a local-memory array would put a ~30-cycle load into every step of a long
-// dependent chain.  Same arithmetic as schur64 / k2a_q16 / lpc_inv_pred_gain_qa / limit_warped_coefs (sb_sigproc.cuh,
-// sb_enc_shape.cuh), which remain the reference statements.
+// dependent chain.  Same arithmetic as schur64 / k2a_q16 / bwexpander_32 (sb_sigproc.cuh), which remain the reference
+// statements.
 template <int ORD> SB_CFN i32 schur64_r(i32 (&rc_Q16)[ORD], const i32 (&c)[ORD + 1]) {
     i32 C0[ORD + 1], C1[ORD + 1];
     if (c[0] <= 0) {
@@ -581,96 +527,11 @@ template <int ORD> SB_CFN void k2a_q16_r(i32 (&A_Q24)[ORD], const i32 (&rc_Q16)[
         A_Q24[k] = negw(shl(rc_Q16[k], 8));
     }
 }
-// SKP_Silk_LPC_inverse_pred_gain_Q24 (LPC_inv_pred_gain.c:42-153 + :170-185); returns 1 when unstable
-template <int ORD> SB_CFN int lpc_inv_pred_gain_q24_r(i32* invGain_Q30, const i32 (&A_Q24)[ORD]) {
-    const i32 A_LIMIT = SB_FIXC(0.99975, 16);
-    i32 A[ORD];
-#pragma unroll
-    for (int k = 0; k < ORD; k++) A[k] = rshift_round(A_Q24[k], 8);
-    i32 inv = 1 << 30;
-    bool bad = false;
-#pragma unroll
-    for (int k = ORD - 1; k > 0; k--) {
-        if (!bad) {
-            if (A[k] > A_LIMIT || A[k] < -A_LIMIT) bad = true;
-            else {
-                const i32 rc_Q31 = negw(shl(A[k], 31 - 16));
-                const i32 rc_mult1_Q30 = (SB_I32_MAX >> 1) - smmul(rc_Q31, rc_Q31);
-                i32 rc_mult2_Q16 = inverse32_varq(rc_mult1_Q30, 46);
-                inv = shl(smmul(inv, rc_mult1_Q30), 2);
-                const int headrm = clz32(rc_mult2_Q16) - 1;
-                rc_mult2_Q16 = shl(rc_mult2_Q16, headrm);
-                i32 An[ORD];
-#pragma unroll
-                for (int n = 0; n < k; n++) {
-                    const i32 tmp = subw(A[n], shl(smmul(A[k - n - 1], rc_Q31), 1));
-                    An[n] = shl(smmul(tmp, rc_mult2_Q16), 16 - headrm);
-                }
-#pragma unroll
-                for (int n = 0; n < k; n++) A[n] = An[n];
-            }
-        }
-    }
-    if (bad) { *invGain_Q30 = inv; return 1; }
-    if (A[0] > A_LIMIT || A[0] < -A_LIMIT) { *invGain_Q30 = inv; return 1; }
-    const i32 rc_Q31 = negw(shl(A[0], 31 - 16));
-    const i32 rc_mult1_Q30 = (SB_I32_MAX >> 1) - smmul(rc_Q31, rc_Q31);
-    *invGain_Q30 = shl(smmul(inv, rc_mult1_Q30), 2);
-    return 0;
-}
 template <int ORD> SB_CFN void bwexpander_32_r(i32 (&ar)[ORD], i32 chirp_Q16) {
     i32 t = chirp_Q16;
 #pragma unroll
     for (int i = 0; i < ORD - 1; i++) { ar[i] = smulww(ar[i], t); t = smulww(chirp_Q16, t); }
     ar[ORD - 1] = smulww(ar[ORD - 1], t);
-}
-// SKP_Silk_noise_shape_analysis_FIX.c:52-132
-template <int ORD> SB_CFN void limit_warped_coefs_r(i32 (&syn)[ORD], i32 (&ana)[ORD], i32 lambda_Q16, i32 limit_Q24) {
-    i32 nom_Q16, den_Q24, gain_syn_Q16, gain_ana_Q16;
-    lambda_Q16 = -lambda_Q16;
-#pragma unroll
-    for (int i = ORD - 1; i > 0; i--) { syn[i - 1] = smlawb(syn[i - 1], syn[i], lambda_Q16); ana[i - 1] = smlawb(ana[i - 1], ana[i], lambda_Q16); }
-    lambda_Q16 = -lambda_Q16;
-    nom_Q16 = smlawb(SB_FIXC(1.0, 16), -lambda_Q16, lambda_Q16);
-    den_Q24 = smlawb(SB_FIXC(1.0, 24), syn[0], lambda_Q16);
-    gain_syn_Q16 = div32_varq(nom_Q16, den_Q24, 24);
-    den_Q24 = smlawb(SB_FIXC(1.0, 24), ana[0], lambda_Q16);
-    gain_ana_Q16 = div32_varq(nom_Q16, den_Q24, 24);
-#pragma unroll
-    for (int i = 0; i < ORD; i++) { syn[i] = smulww(gain_syn_Q16, syn[i]); ana[i] = smulww(gain_ana_Q16, ana[i]); }
-    for (int iter = 0; iter < 10; iter++) {
-        i32 maxabs_Q24 = -1; int ind = 0;
-#pragma unroll
-        for (int i = 0; i < ORD; i++) {
-            i32 a = syn[i], b = ana[i];
-            a = (a ^ (a >> 31)) - (a >> 31);
-            b = (b ^ (b >> 31)) - (b >> 31);
-            const i32 tmp = imax(a, b);
-            if (tmp > maxabs_Q24) { maxabs_Q24 = tmp; ind = i; }
-        }
-        if (maxabs_Q24 <= limit_Q24) return;
-#pragma unroll
-        for (int i = 1; i < ORD; i++) { syn[i - 1] = smlawb(syn[i - 1], syn[i], lambda_Q16); ana[i - 1] = smlawb(ana[i - 1], ana[i], lambda_Q16); }
-        gain_syn_Q16 = inverse32_varq(gain_syn_Q16, 32);
-        gain_ana_Q16 = inverse32_varq(gain_ana_Q16, 32);
-#pragma unroll
-        for (int i = 0; i < ORD; i++) { syn[i] = smulww(gain_syn_Q16, syn[i]); ana[i] = smulww(gain_ana_Q16, ana[i]); }
-        const i32 chirp_Q16 = SB_FIXC(0.99, 16) - div32_varq(
-            smulwb(maxabs_Q24 - limit_Q24, smlabb(SB_FIXC(0.8, 10), SB_FIXC(0.1, 10), iter)), mulw(maxabs_Q24, ind + 1), 22);
-        bwexpander_32_r<ORD>(syn, chirp_Q16);
-        bwexpander_32_r<ORD>(ana, chirp_Q16);
-        lambda_Q16 = -lambda_Q16;
-#pragma unroll
-        for (int i = ORD - 1; i > 0; i--) { syn[i - 1] = smlawb(syn[i - 1], syn[i], lambda_Q16); ana[i - 1] = smlawb(ana[i - 1], ana[i], lambda_Q16); }
-        lambda_Q16 = -lambda_Q16;
-        nom_Q16 = smlawb(SB_FIXC(1.0, 16), -lambda_Q16, lambda_Q16);
-        den_Q24 = smlawb(SB_FIXC(1.0, 24), syn[0], lambda_Q16);
-        gain_syn_Q16 = div32_varq(nom_Q16, den_Q24, 24);
-        den_Q24 = smlawb(SB_FIXC(1.0, 24), ana[0], lambda_Q16);
-        gain_ana_Q16 = div32_varq(nom_Q16, den_Q24, 24);
-#pragma unroll
-        for (int i = 0; i < ORD; i++) { syn[i] = smulww(gain_syn_Q16, syn[i]); ana[i] = smulww(gain_ana_Q16, ana[i]); }
-    }
 }
 
 // pitch_res points at res_pitch + FRAME, x at x_buf + FRAME.
@@ -1661,6 +1522,13 @@ template <int F> SB_CFN void c_hb_analyse_frame(EncBands* hb, HbScr* H, const i1
         SB_PARFOR(i, 0, 20) xb[F / 2 + i] = xb[F + i];
         if (lane == 0) hb->hb_first = 0;
         SB_SYNC();
+    }
+}
+// Every high-band frame of the packet: n new samples in frames of F (the stream's hb_frame) -> scr->hb_lsp_idx, hb_nrg0.
+SB_CFN void c_hb_analyse_packet(EncBands* hb, HbScr* H, const i16* high, int n, int F, EncScratch* scr) {
+    for (int f = 0; f < n / F; f++) {
+        if (F == HB_FRAME) c_hb_analyse_frame<HB_FRAME>(hb, H, high + f * F, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
+        else c_hb_analyse_frame<2 * HB_FRAME>(hb, H, high + f * F, &scr->hb_lsp_idx[f], scr->hb_nrg0[f]);
     }
 }
 

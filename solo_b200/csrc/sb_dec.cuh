@@ -617,10 +617,11 @@ SB_FN i32 dec_silk_frame(DecState* st, DecCtrl* c, RangeDec* rc, i32 (*Pulses)[F
     return ret;
 }
 
-// One group of four outputs of the synthesis filter bank (AGR_BWE_qmf.c:125-176): xx1 / xx2 = time-reversed band signals
-// followed by the filter memories, i = even output-pair index.  The order of the float operations is the reference's; the
-// groups are independent of each other, which is what the synthesis kernel uses (one group per lane and step).
-SB_HD void qmf_synth_group(const float* xx1, const float* xx2, const float* a, int N2, int i, float* y4) {
+// One group of four outputs of the synthesis filter bank (AGR_BWE_qmf.c:125-176) as int16 PCM, truncated and saturated
+// (AGR_BWE_decode_frame_FLP.c:222-231): xx1 / xx2 = time-reversed band signals followed by the filter memories, i = even
+// output-pair index.  The order of the float operations is the reference's; the groups are independent of each other,
+// which is what the synthesis kernel uses (one group per lane and step).
+SB_HD void qmf_synth_group(const float* xx1, const float* xx2, const float* a, int N2, int i, i16* pcm4) {
     enum { M2 = 32 };
     float y0 = 0, y1 = 0, y2 = 0, y3 = 0;
     float x10 = xx1[N2 - 2 - i], x20 = xx2[N2 - 2 - i];
@@ -640,12 +641,16 @@ SB_HD void qmf_synth_group(const float* xx1, const float* xx2, const float* a, i
         y2 = y2 + a0 * (x11 - x21);
         y3 = y3 + a1 * (x11 + x21);
     }
-    y4[0] = 2.f * y0; y4[1] = 2.f * y1; y4[2] = 2.f * y2; y4[3] = 2.f * y3;
+    const float y4[4] = {2.f * y0, 2.f * y1, 2.f * y2, 2.f * y3};
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const i32 t = trunc_i32((double)y4[q]);
+        pcm4[q] = (i16)(t > 32767 ? 32767 : (t < -32768 ? -32768 : t));
+    }
 }
 
 // ---- scalar model of the synthesis kernel: AGR_Sate_qmf_synth, float branch (AGR_BWE_qmf.c:86-182), N = 2 * N2 = 640
-// or 320, M = 64, then the truncation to int16 (AGR_BWE_decode_frame_FLP.c:222-231).  low / high: the band signals
-// dec_packet handed out.
+// or 320, M = 64, into int16 PCM.  low / high: the band signals dec_packet handed out.
 SB_FN void dec_synth(DecState* st, const i16* low, const float* high, i16* pcm) {
     enum { M2 = 32, N2MAX = PACKET / 2 };
     const int N2 = st->frames_per_packet * FRAME;
@@ -653,14 +658,7 @@ SB_FN void dec_synth(DecState* st, const i16* low, const float* high, i16* pcm) 
     const float* a = SB_T(qmf_flt);
     for (int i = 0; i < N2; i++) { xx1[i] = (float)low[N2 - 1 - i]; xx2[i] = high[N2 - 1 - i]; }
     for (int i = 0; i < M2; i++) { xx1[N2 + i] = st->g0_mem[2 * i + 1]; xx2[N2 + i] = st->g1_mem[2 * i + 1]; }
-    for (int i = 0; i < N2; i += 2) {
-        float y4[4];
-        qmf_synth_group(xx1, xx2, a, N2, i, y4);
-        for (int q = 0; q < 4; q++) {
-            const i32 t = trunc_i32((double)y4[q]);
-            pcm[2 * i + q] = (i16)(t > 32767 ? 32767 : (t < -32768 ? -32768 : t));
-        }
-    }
+    for (int i = 0; i < N2; i += 2) qmf_synth_group(xx1, xx2, a, N2, i, pcm + 2 * i);
     for (int i = 0; i < M2; i++) { st->g0_mem[2 * i + 1] = xx1[i]; st->g1_mem[2 * i + 1] = xx2[i]; }
 }
 

@@ -2,9 +2,9 @@
 // MD noise-shaping quantiser, two high-band frames, payload assembly [MD1 | MD2 | HB].
 // enc_packet is the scalar model of the device pipeline, stage by stage: band split, voice activity, core analysis,
 // high-band analysis, shaping filters, gains, prefilter, quantiser, entropy coding.  The band split (sharing
-// qmf_output_pair with its kernel), the core and high-band analysis, the quantiser and the entropy coding have scalar forms
-// here (those kernels run sb_coop.cuh, sb_nsq_warp.cuh and a two-thread form of enc_packet_finish); voice activity, shaping
-// filters, gains and prefilter are the functions their kernels call.
+// qmf_output_pair with its kernel), the core and high-band analysis and the quantiser have scalar forms here, the
+// specification of what those kernels run (sb_coop.cuh, sb_nsq_warp.cuh); voice activity, shaping filters, gains,
+// prefilter and the entropy-coding steps are the functions their kernels call.
 // Reference: /root/reference/JC1_SDK_SRC_ARM/src/libBWE/AGR_BWE_encode_frame_FIX.c:8-174, AGR_BWE_qmf.c:38-80,
 // AGR_BWE_find_HB_LPC_FIX.c:4-49, AGR_BWE_quant_highband.c:23-147, AGR_BWE_SDK_API.c:11-152,
 // libSATECodec/SKP_Silk_enc_API.c:127-273, SKP_Silk_encode_frame_FIX.c:34-327, SKP_Silk_control_codec_FIX.c:232-389.
@@ -183,7 +183,6 @@ struct EncAnalysisWork {
     i16 low[PACKET / 2], high[PACKET / 2];   // band signals of the packet
     i16 pIn_HP[FRAME];
     i16 res_pitch[2 * FRAME + LA_PITCH];
-    const NlsfFastTabs* nlsf_fast;   // not read: the scalar model searches the NLSF codebooks in the global tables
 };
 
 // SKP_Silk_encode_frame_FIX (encode_frame_FIX.c:34-131) up to the quantised NLSFs, for frame f of the packet: the scalar
@@ -226,38 +225,59 @@ SB_FN void enc_packet_post_analysis(EncSilk* st, EncScratch* scr) {
     prefilter_packet(st, scr, nf);
 }
 
-// stage C: AGR_Sate_Encoder_Encode tail -- returns the byte count; nBytesOut[0] = total, nBytesOut[1] = len(MD2) + 8
-SB_FN i32 enc_packet_finish(EncCore* st, const EncScratch* scr, u8* rcbuf /* MAX_PAYLOAD scratch */, u8* out, i32 out_cap, i16* nBytesOut) {
-    int nb[2];
-    int ok = 1;
-    int written = 0;
-    const int nf = st->frames_per_packet, nhb = nf * FRAME / st->hb_frame, hb_bytes = 4 * nhb;
-    for (int k = 0; k < 2; k++) {
-        RangeEnc rc;
-        rc_enc_init(&rc, rcbuf, MAX_PAYLOAD);
-        for (int f = 0; f < nf; f++) {
-            encode_parameters(&rc, st, &scr->c[f], k, f, scr->vadFlag[f], scr->q_md[f][k]);
-            // frame terminator: MORE_FRAMES (1) while frames follow in this packet, LAST_FRAME (0) after the last one
-            rc_encode(&rc, f < nf - 1 ? 1 : 0, SB_T(frame_term_cdf));
-        }
-        rc_get_length(&rc, &nb[k]);
-        if (rc.error) ok = 0;
-        if (k == 1 && nb[0] + nb[1] > MAX_PAYLOAD) ok = 0;  // pnBytesOut[0] >= nMDBytes (encode_frame_FIX.c:245)
-        if (ok) {
-            rc_enc_wrap_up(&rc);
-            for (int i = 0; i < nb[k]; i++) if (written + i < out_cap) out[written + i] = rcbuf[i];
-            written += nb[k];
-        }
+// ---- stage C: AGR_Sate_Encoder_Encode tail, in the three steps of one description k (0 or 1) that the entropy-coding
+// kernel runs on thread k of a pair; all description stores come before any high-band store.  The payload row is
+// [MD1 | MD2 | HB]; nBytesOut[0] = total, nBytesOut[1] = len(MD2) + high-band bytes.
+// (1) range-code description k of every frame of the packet into buf (MAX_PAYLOAD bytes); rc stays live for step 2.
+// Returns the byte count, *ok = 0 when the coder overflowed.
+SB_HD int enc_code_description(RangeEnc* rc, u8* buf, EncCore* st, const EncScratch* scr, int k, int* ok) {
+    const int nf = st->frames_per_packet;
+    rc_enc_init(rc, buf, MAX_PAYLOAD);
+    for (int f = 0; f < nf; f++) {
+        encode_parameters(rc, st, &scr->c[f], k, f, scr->vadFlag[f], scr->q_md[f][k]);
+        // frame terminator: MORE_FRAMES (1) while frames follow in this packet, LAST_FRAME (0) after the last one
+        rc_encode(rc, f < nf - 1 ? 1 : 0, SB_T(frame_term_cdf));
     }
-    if (!ok) { nb[0] = nb[1] = 0; }
-    if (scr->dtx_drop) { nb[0] = nb[1] = 0; }
-    u8 hb[8];
-    for (int f = 0; f < nhb; f++) hb_pack_frame(scr->hb_lsp_idx[f], scr->hb_nrg0[f], &scr->r16[0][0] + f * st->hb_frame, hb + 4 * f, st->hb_frame >> 2);
-    int lb = nb[0] + nb[1];
-    int total = lb + hb_bytes;
-    for (int i = 0; i < hb_bytes; i++) if (lb + i < out_cap) out[lb + i] = hb[i];
-    if (lb) { nBytesOut[0] = (i16)total; nBytesOut[1] = (i16)(nb[1] + hb_bytes); }
-    else { nBytesOut[0] = 0; nBytesOut[1] = 0; }
+    int nb;
+    rc_get_length(rc, &nb);
+    *ok = rc->error ? 0 : 1;
+    return nb;
+}
+// (2) with both descriptions' lengths and status: description 0 is kept when its own coder succeeded, description 1 when
+// both did and they fit MAX_PAYLOAD (pnBytesOut[0] >= nMDBytes, encode_frame_FIX.c:245); a kept description is finished
+// and copied to offset k ? nb0 : 0, bytes at or past out_cap dropped.  Returns the low-band bytes the packet carries:
+// nb0 + nb1, or 0 for a rejected or DTX-dropped packet.
+SB_HD int enc_store_description(RangeEnc* rc, const EncScratch* scr, int k, int nb0, int nb1, int ok0, int ok1, u8* out, i32 out_cap) {
+    const int ok = ok0 && ok1 && nb0 + nb1 <= MAX_PAYLOAD;
+    if (k == 0 ? ok0 : ok) {
+        rc_enc_wrap_up(rc);
+        const int off = k ? nb0 : 0, nb = k ? nb1 : nb0;
+        for (int i = 0; i < nb; i++) if (off + i < out_cap) out[off + i] = rc->buf[i];
+    }
+    return (ok && !scr->dtx_drop) ? nb0 + nb1 : 0;
+}
+// (3) high-band frame k (if the packet has one) behind the lb low-band bytes -- so a rejected or dropped packet's
+// high-band bytes land on top of its descriptions' -- and, for k = 0, the length fields.  Returns the packet's total size.
+SB_HD int enc_store_high_band(const EncCore* st, const EncScratch* scr, int k, int lb, int nb1, u8* out, i32 out_cap, i16* nBytesOut) {
+    const int nhb = st->frames_per_packet * FRAME / st->hb_frame, hb_bytes = 4 * nhb;
+    if (k < nhb) {
+        u8 hb[4];
+        hb_pack_frame(scr->hb_lsp_idx[k], scr->hb_nrg0[k], &scr->r16[0][0] + k * st->hb_frame, hb, st->hb_frame >> 2);
+        for (int i = 0; i < 4; i++) if (lb + 4 * k + i < out_cap) out[lb + 4 * k + i] = hb[i];
+    }
+    if (k == 0) {
+        nBytesOut[0] = lb ? (i16)(lb + hb_bytes) : 0;
+        nBytesOut[1] = lb ? (i16)(nb1 + hb_bytes) : 0;
+    }
+    return lb + hb_bytes;
+}
+// stage C on one thread: the kernel's two threads one after the other.  Returns min(out_cap, total).
+SB_FN i32 enc_packet_finish(EncCore* st, const EncScratch* scr, u8 (*rcbuf)[MAX_PAYLOAD], u8* out, i32 out_cap, i16* nBytesOut) {
+    RangeEnc rc[2];
+    int nb[2], ok[2], lb = 0, total = 0;
+    for (int k = 0; k < 2; k++) nb[k] = enc_code_description(&rc[k], rcbuf[k], st, scr, k, &ok[k]);
+    for (int k = 0; k < 2; k++) lb = enc_store_description(&rc[k], scr, k, nb[0], nb[1], ok[0], ok[1], out, out_cap);
+    for (int k = 0; k < 2; k++) total = enc_store_high_band(st, scr, k, lb, nb[1], out, out_cap, nBytesOut);
     return imin(out_cap, total);
 }
 
@@ -267,7 +287,7 @@ struct EncPacketWork {
     EncScratch scr;
     NsqWork nsq;
     i32 r[FRAME];
-    u8 rcbuf[MAX_PAYLOAD];
+    u8 rcbuf[2][MAX_PAYLOAD];   // both descriptions' coders are live at once
 };
 // band split and voice activity of the packet (the first two kernels)
 SB_FN void enc_packet_bands(EncState* st, EncPacketWork* W, const i16* pcm) {

@@ -546,5 +546,12 @@ SB_NSQ_KFN void nsq_del_dec_warp(NsqSmem& S, NsqState* ns3, EncCtrl* c, const i1
     }
 }
 
+// The nf frames of a packet for the stream of this lane group: frame controls and prefiltered input from the scratch slot,
+// pulses and centre excitation back into it.
+SB_NSQ_DEV void nsq_packet_warp(NsqSmem& S, NsqState* ns3, EncScratch* scr, int nf) {
+    for (int f = 0; f < nf; f++)
+        nsq_del_dec_warp(S, ns3, &scr->c[f], scr->xfw[f], scr->q_md[f][0], scr->q_md[f][1], scr->r16[f], &scr->nsq_rand[0][0][0]);
+}
+
 }  // namespace sb
 #endif  // __CUDACC__ || SB_EMU

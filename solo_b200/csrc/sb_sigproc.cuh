@@ -306,22 +306,6 @@ SB_FN void biquad_alt(const i16* __restrict__ in, const i32* B_Q28, const i32* A
 }
 
 // ---- SKP_Silk_sort.c:34-124 (partial insertion sorts; tie-breaking is part of the bitstream, Q22)
-SB_FN void insertion_sort_increasing(i32* a, i32* index, int L, int K) {
-    for (int i = 0; i < K; i++) index[i] = i;
-    for (int i = 1; i < K; i++) {
-        i32 value = a[i]; int j;
-        for (j = i - 1; j >= 0 && value < a[j]; j--) { a[j + 1] = a[j]; index[j + 1] = index[j]; }
-        a[j + 1] = value; index[j + 1] = i;
-    }
-    for (int i = K; i < L; i++) {
-        i32 value = a[i];
-        if (value < a[K - 1]) {
-            int j;
-            for (j = K - 2; j >= 0 && value < a[j]; j--) { a[j + 1] = a[j]; index[j + 1] = index[j]; }
-            a[j + 1] = value; index[j + 1] = i;
-        }
-    }
-}
 SB_FN void insertion_sort_decreasing_i16(i16* a, i32* index, int L, int K) {
     for (int i = 0; i < K; i++) index[i] = i;
     for (int i = 1; i < K; i++) {

@@ -143,6 +143,7 @@ struct EncCtrl {
 //                       prefilter (thread per stream)        -> xfw
 //   stage B (MD noise-shaping quantiser)                     : consumes c[f], xfw[f]; produces q_md[f], r16[f], c[f].Seed
 //   stage C (entropy coding + packing)                       : range-codes both descriptions, high-band gains, payload assembly
+//                                                              (the same three steps per description in both builds, sb_enc.cuh)
 struct EncScratch {
     EncCtrl c[2];
     i16 xfw[2][FRAME];

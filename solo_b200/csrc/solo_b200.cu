@@ -152,15 +152,12 @@ __global__ void __launch_bounds__(SB_NSQ_WARPS * 32, SB_NSQ_MINB) sb_enc_nsq_ker
     // arithmetic in its own shared-memory slot, identical values stored twice.  This keeps the sample loop's full-warp
     // collectives valid for every warp.
     if (s >= n) s = n - 1;
-    EncScratch* scr = &scratch[s];
-    const int nf = states[s].frames_per_packet;
-    for (int f = 0; f < nf; f++)
-        nsq_del_dec_warp(*S, states[s].nsq, &scr->c[f], scr->xfw[f], scr->q_md[f][0], scr->q_md[f][1], scr->r16[f], &scr->nsq_rand[0][0][0]);
+    nsq_packet_warp(*S, states[s].nsq, &scratch[s], states[s].frames_per_packet);
 }
 
-// Entropy coding and payload assembly, TWO threads per stream: thread k range-codes description k of both frames (the two
-// coders share nothing but read-only frame parameters) and packs high-band frame k; the pair exchanges lengths and status
-// by shuffle and writes the row [MD1 | MD2 | HB].  Same result as the one-thread model enc_packet_finish() (sb_enc.cuh).
+// Entropy coding and payload assembly, TWO threads per stream: thread k runs the stage-C steps of description k
+// (sb_enc.cuh; the two coders share nothing but read-only frame parameters) and exchanges lengths and status with its
+// partner by shuffle between coding and storing.  enc_packet_finish runs the same steps for both k on one thread.
 __global__ void __launch_bounds__(SB_TPB, SB_FINISH_MINB) sb_enc_finish_kernel(EncState* states, const EncScratch* scratch, u8* __restrict__ bits, int cap,
                                                                i16* __restrict__ nbytes, int n) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -171,36 +168,14 @@ __global__ void __launch_bounds__(SB_TPB, SB_FINISH_MINB) sb_enc_finish_kernel(E
     const EncScratch* scr = &scratch[s];
     u8* out = bits + (size_t)s * cap;
     u8 rcbuf[MAX_PAYLOAD];
-    const int nf = st->frames_per_packet, nhb = nf * FRAME / st->hb_frame, hb_bytes = 4 * nhb;
     RangeEnc rc;
-    rc_enc_init(&rc, rcbuf, MAX_PAYLOAD);
-    for (int f = 0; f < nf; f++) {
-        encode_parameters(&rc, st, &scr->c[f], k, f, scr->vadFlag[f], scr->q_md[f][k]);
-        // frame terminator: MORE_FRAMES (1) while frames follow in this packet, LAST_FRAME (0) after the last one
-        rc_encode(&rc, f < nf - 1 ? 1 : 0, SB_T(frame_term_cdf));
-    }
-    int nb_k;
-    rc_get_length(&rc, &nb_k);
-    const int ok_k = rc.error ? 0 : 1;
+    int ok_k;
+    const int nb_k = enc_code_description(&rc, rcbuf, st, scr, k, &ok_k);
     const int nb_o = __shfl_xor_sync(m, nb_k, 1), ok_o = __shfl_xor_sync(m, ok_k, 1);
     const int nb0 = k ? nb_o : nb_k, nb1 = k ? nb_k : nb_o, ok0 = k ? ok_o : ok_k, ok1 = k ? ok_k : ok_o;
-    const int ok = ok0 && ok1 && nb0 + nb1 <= MAX_PAYLOAD;        // pnBytesOut[0] >= nMDBytes (encode_frame_FIX.c:245)
-    const int dtx = scr->dtx_drop;
-    if (k == 0 ? ok0 : ok) {
-        rc_enc_wrap_up(&rc);
-        const int off = k ? nb0 : 0;
-        for (int i = 0; i < nb_k; i++) if (off + i < cap) out[off + i] = rcbuf[i];
-    }
-    u8 hb[4];
-    const int my_hb = k < nhb;
-    if (my_hb) hb_pack_frame(scr->hb_lsp_idx[k], scr->hb_nrg0[k], &scr->r16[0][0] + k * st->hb_frame, hb, st->hb_frame >> 2);
+    const int lb = enc_store_description(&rc, scr, k, nb0, nb1, ok0, ok1, out, cap);
     __syncwarp(m);      // a rejected or dropped packet's high-band bytes land on top of description 1's
-    const int lb = (ok && !dtx) ? nb0 + nb1 : 0;
-    if (my_hb) for (int i = 0; i < 4; i++) if (lb + 4 * k + i < cap) out[lb + 4 * k + i] = hb[i];
-    if (k == 0) {
-        nbytes[2 * s] = lb ? (i16)(lb + hb_bytes) : 0;
-        nbytes[2 * s + 1] = lb ? (i16)(nb1 + hb_bytes) : 0;
-    }
+    enc_store_high_band(st, scr, k, lb, nb1, out, cap, &nbytes[2 * s]);
 }
 
 __global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecState* states, int n, int mdi, int framesize_ms, int joint_hb) {
@@ -247,14 +222,11 @@ __global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecStat
     __syncwarp();
     i16* out = pcm + (size_t)s * spp;
     for (int g = lane; g < N2 / 2; g += 32) {
-        float y4[4];
-        qmf_synth_group(xx1, xx2, coef, N2, 2 * g, y4);
-        i32 t[4];
-#pragma unroll
-        for (int q = 0; q < 4; q++) { i32 v = trunc_i32((double)y4[q]); t[q] = v > 32767 ? 32767 : (v < -32768 ? -32768 : v); }
+        i16 y[4];
+        qmf_synth_group(xx1, xx2, coef, N2, 2 * g, y);
         int2 pk;
-        pk.x = (t[0] & 0xffff) | (t[1] << 16);
-        pk.y = (t[2] & 0xffff) | (t[3] << 16);
+        pk.x = (int)((u16)y[0] | ((u32)(u16)y[1] << 16));
+        pk.y = (int)((u16)y[2] | ((u32)(u16)y[3] << 16));
         reinterpret_cast<int2*>(out)[g] = pk;
     }
     __syncwarp();

@@ -27,7 +27,6 @@ int main(int argc, char** argv) {
         const int fs_ms = mode == 1 ? 20 : 40, joint = mode == 2;
         const int spp = 16 * fs_ms;
         sb::enc_state_init(est, 13600 + 4000 * mode, 0, mode == 1, fs_ms, joint);
-        ew->a.nlsf_fast = nullptr;
         sb::dec_state_init(dst, mode == 1, fs_ms, joint);
         double ph = 0;
         for (int it = 0; it < iters; it++) {

@@ -172,24 +172,15 @@ static void emu_analysis(HsEnc* h) {
     const int nf = h->st.frames_per_packet;
     for (int i = 0; i < nf * sb::FRAME; i++) cw.low[i] = h->w.a.low[i];
     sb::emu::run32([=]() { sb::c_enc_packet_analysis(&h->st, &cw, &h->w.scr); });
-    sb::emu::run32([=]() {
-        for (int f = 0; f < nf * sb::FRAME / h->st.hb_frame; f++) {
-            if (h->st.hb_frame == sb::HB_FRAME) sb::c_hb_analyse_frame<sb::HB_FRAME>(&h->st, &hs, h->w.a.high + f * h->st.hb_frame, &h->w.scr.hb_lsp_idx[f], h->w.scr.hb_nrg0[f]);
-            else sb::c_hb_analyse_frame<2 * sb::HB_FRAME>(&h->st, &hs, h->w.a.high + f * h->st.hb_frame, &h->w.scr.hb_lsp_idx[f], h->w.scr.hb_nrg0[f]);
-        }
-    });
+    sb::emu::run32([=]() { sb::c_hb_analyse_packet(&h->st, &hs, h->w.a.high, nf * sb::FRAME, h->st.hb_frame, &h->w.scr); });
 }
 // the quantiser kernel's code for one warp: lane group g works on stream hh[g] (one group with SB_NSQ_GW = 32)
 static void emu_nsq(HsEnc* const* hh) {
     static sb::NsqSmem S[2];
-    const int nf = hh[0]->st.frames_per_packet;
-    for (int f = 0; f < nf; f++)
-        sb::emu::run32m([=]() {
-            const int g = sb::emu::lane / SB_NSQ_GW;
-            HsEnc* h = hh[g];
-            sb::EncScratch* scr = &h->w.scr;
-            sb::nsq_del_dec_warp(S[g], h->st.nsq, &scr->c[f], scr->xfw[f], scr->q_md[f][0], scr->q_md[f][1], scr->r16[f], &scr->nsq_rand[0][0][0]);
-        });
+    sb::emu::run32m([=]() {
+        const int g = sb::emu::lane / SB_NSQ_GW;
+        sb::nsq_packet_warp(S[g], hh[g]->st.nsq, &hh[g]->w.scr, hh[g]->st.frames_per_packet);
+    });
 }
 #endif
 // the stages of sb::enc_packet up to the quantiser; the emulated build swaps in the cooperative analysis

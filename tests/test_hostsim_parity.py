@@ -2,9 +2,11 @@
 where oracle/_ref is built, against the unmodified reference on inputs the fixtures do not cover.
 
 The headers are written once as __host__ __device__ code, and the host model runs the device pipeline's stages in its
-order, so what passes here is the same source nvcc compiles into libsolo_b200.so: every encoder stage after the analysis
-and the decoder up to the synthesis filter bank are the kernels' own functions.  The warp-per-stream stages run here in
-their scalar forms, and in their device code (sb_coop.cuh, sb_nsq_warp.cuh) on 32 emulated lanes in the last two tests.
+order, so what passes here is the same source nvcc compiles into libsolo_b200.so: voice activity, shaping filters, gains,
+prefilter, the entropy-coding steps of the two descriptions, the decoder and the int16 output groups of its synthesis
+filter bank are the kernels' own functions.  The
+warp-per-stream stages (analysis, quantiser) run here in their scalar forms, and in their device code with the kernels'
+packet drivers (sb_coop.cuh, sb_nsq_warp.cuh) on 32 emulated lanes in the last two tests.
 Bar: payloads and length fields byte-identical to the FIX build, PCM identical to the FLP build (north star allows
 +-1 LSB)."""
 import hashlib
