@@ -46,6 +46,29 @@ int solo_b200_enc_batch_encode_device(solo_b200_enc_batch *b, const int16_t *d_p
                                       int16_t *d_nbytes, void *cuda_stream);
 void solo_b200_enc_batch_destroy(solo_b200_enc_batch *b);
 
+/* Per-stream encoder settings that may change between packets, as the reference's SILK core re-reads them from the
+   handle at the start of every packet (SKP_Silk_enc_API.c:161-191):
+     rate_bps  : target rate as USER_Ctrl_enc.targetRate_bps (>= 1; the core gets it less 1600 b/s, or less 800 b/s with
+                 joint mode 1, clamped to [5000, 100000])
+     dtx       : 0 or 1, as USER_Ctrl_enc.dtx_enable
+     loss_perc : expected packet loss in percent, 0-100 (Init starts at 0).  The encoder then trades long-term prediction
+                 gain for robustness (SKP_Silk_LTP_scale_ctrl_FIX.c:39-81); the decoder needs no change.
+   Arrays are int32 [N].  A NULL array leaves that setting unchanged for every stream, an entry of -1 for that stream.  New
+   settings apply from the next packet; both frames of a 40 ms packet use the same settings.
+     set_control_host   : host arrays.  Returns -1 and applies nothing if any entry is out of range; otherwise returns once
+                          the settings are in place, after every packet wave already enqueued for the batch.
+     set_control_device : device arrays; only enqueues a kernel on `cuda_stream`, in order with the encode_device calls
+                          on that stream.  The arrays are not checked on the host: an out-of-range entry leaves that
+                          stream's setting unchanged, like -1.
+   Create followed by set_control before the first packet is the same as creating the stream with those settings. */
+int solo_b200_enc_batch_set_control_host(solo_b200_enc_batch *b, const int32_t *rate_bps, const int32_t *dtx,
+                                         const int32_t *loss_perc);
+int solo_b200_enc_batch_set_control_device(solo_b200_enc_batch *b, const int32_t *d_rate_bps, const int32_t *d_dtx,
+                                           const int32_t *d_loss_perc, void *cuda_stream);
+/* The same for one AGR_Sate_Encoder_Init handle (scalars, -1 = unchanged): 0, or -1 for a NULL or foreign handle or an
+   out-of-range value (nothing applied). */
+int solo_b200_encoder_set_control(void *SATEEnc_State, int32_t rate_bps, int32_t dtx, int32_t loss_perc);
+
 solo_b200_dec_batch *solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_dec *ctrl, int device);
 int solo_b200_dec_batch_decode_host(solo_b200_dec_batch *b, int16_t *pcm, const uint8_t *bits, int cap,
                                     const int16_t *nbytes, const int32_t *lostflag, int32_t *ret);

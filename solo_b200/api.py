@@ -50,6 +50,9 @@ def lib():
         L.solo_b200_enc_batch_encode_host.argtypes = [vp, vp, vp, C.c_int, vp]
         L.solo_b200_enc_batch_encode_device.argtypes = [vp, vp, vp, C.c_int, vp, vp]
         L.solo_b200_enc_batch_destroy.argtypes = [vp]
+        L.solo_b200_enc_batch_set_control_host.argtypes = [vp, vp, vp, vp]
+        L.solo_b200_enc_batch_set_control_device.argtypes = [vp, vp, vp, vp, vp]
+        L.solo_b200_encoder_set_control.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
         L.solo_b200_dec_batch_create.restype = vp
         L.solo_b200_dec_batch_create.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int]
         L.solo_b200_dec_batch_decode_host.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
@@ -126,6 +129,13 @@ class SoloEncoder:
         self._nb[:] = 0
         n = lib().AGR_Sate_Encoder_Encode(self.h, pcm.ctypes.data, self._bits.ctypes.data, bufsize, self._nb.ctypes.data)
         return bytes(self._bits[:max(n, 0)]), (int(self._nb[0]), int(self._nb[1])), n
+
+    def set_control(self, rate=None, dtx=None, loss=None):
+        """Target rate (b/s), DTX on / off and expected packet loss (%) from the next packet on; None leaves a setting as
+        it is (see solo_b200_encoder_set_control in include/solo_b200.h)."""
+        r = lib().solo_b200_encoder_set_control(self.h, *(-1 if v is None else int(v) for v in (rate, dtx, loss)))
+        if r:
+            raise SoloError("set_control failed (%d): %s" % (r, "setting out of range" if r == -1 else _err()))
 
     def close(self):
         if getattr(self, "h", None):
@@ -211,6 +221,32 @@ class EncoderBatch:
         r = lib().solo_b200_enc_batch_encode_device(self.h, d_pcm, d_bits, cap, d_nbytes, stream)
         if r:
             raise SoloError("encode_device failed (%d): %s" % (r, _err()))
+
+    def set_control(self, rate=None, dtx=None, loss=None):
+        """Per-stream target rate (b/s), DTX (0 / 1) and expected packet loss (0-100 %) from the next packet on.  Each is
+        None (unchanged), a scalar for every stream or an int array [N] whose -1 entries leave that stream alone.  Raises
+        SoloError, with nothing applied, if a value is out of range."""
+        keep = []
+
+        def arg(v):
+            if v is None:
+                return None
+            a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, np.int64), (self.n,)))
+            if (a < np.iinfo(np.int32).min).any() or (a > np.iinfo(np.int32).max).any():
+                raise SoloError("set_control: a setting is out of range")
+            keep.append(a.astype(np.int32))
+            return keep[-1].ctypes.data
+
+        r = lib().solo_b200_enc_batch_set_control_host(self.h, arg(rate), arg(dtx), arg(loss))
+        if r:
+            raise SoloError("set_control failed (%d): %s" % (r, _err()))
+
+    def set_control_device(self, d_rate=None, d_dtx=None, d_loss=None, stream=0):
+        """Device int32 arrays [N] (addresses, None = unchanged), enqueued on `stream` in order with encode_device; an
+        out-of-range entry leaves that stream's setting unchanged."""
+        r = lib().solo_b200_enc_batch_set_control_device(self.h, d_rate, d_dtx, d_loss, stream)
+        if r:
+            raise SoloError("set_control_device failed (%d): %s" % (r, _err()))
 
     def close(self):
         if getattr(self, "h", None):

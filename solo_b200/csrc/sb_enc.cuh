@@ -17,17 +17,47 @@
 
 namespace sb {
 
+// ---- per-packet control: what SKP_Silk_SDK_Encode reads from the handle's encControl at the start of every packet
+// (enc_API.c:161-191) and SKP_Silk_control_encoder_FIX applies (control_codec_FIX.c:56-130) -------------------------
+// rate_bps >= 1: the user rate; the SILK core gets it less (1600 * 20) / bwe_framesize_ms (AGR_BWE_SDK_API.c:118),
+// clamped to [5000, 100000], and both SNR targets follow (setup_rate, :319-389).  dtx 0 / 1: useDTX.  loss_perc 0-100:
+// the expected packet loss of LTP_scale_ctrl.  A value outside those ranges (-1 by convention) leaves its setting as it is.
+// Takes effect from the next packet; both frames of a 40 ms packet see the same settings, as in the reference.
+SB_FN void enc_set_control(EncSilk* st, i32 rate_bps, i32 dtx, i32 loss_perc) {
+    if (rate_bps >= 1) {
+        const i32 silk_rate = limit(rate_bps - (st->hb_frame == 320 ? 800 : 1600), 5000, 100000);
+        st->targetRate_bps = silk_rate;
+        // setup_rate: both tables end at 100000, so each search finds its interval
+        const i32* rt = SB_T(target_rate_table_nb);
+        const i32* snr = SB_T(snr_table_q1);
+        const i32 md_rate = silk_rate / 2;
+        for (int k = 1; k < 8; k++) {
+            if (md_rate < rt[k]) {
+                i32 frac_Q6 = shl(md_rate - rt[k - 1], 6) / (rt[k] - rt[k - 1]);
+                st->SNRPerMD_dB_Q7 = shl(snr[k - 1], 6) + mulw(frac_Q6, snr[k] - snr[k - 1]);
+                break;
+            }
+        }
+        for (int k = 1; k < 8; k++) {
+            if (silk_rate <= rt[k]) {
+                i32 frac_Q6 = shl(silk_rate - rt[k - 1], 6) / (rt[k] - rt[k - 1]);
+                st->SNR_dB_Q7 = shl(snr[k - 1], 6) + mulw(frac_Q6, snr[k] - snr[k - 1]);
+                break;
+            }
+        }
+    }
+    if (dtx == 0 || dtx == 1) st->useDTX = dtx;
+    if (loss_perc >= 0 && loss_perc <= 100) st->packetLoss_perc = loss_perc;
+}
+
 // ---- Init: AGR_Sate_Encoder_Init + SKP_Silk_init_encoder_FIX + first SKP_Silk_control_encoder_FIX --------------
 // Returns 0, or -1 for a configuration the reference rejects / this build does not cover.
 SB_FN int enc_state_init(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0) {
     memset(st, 0, sizeof(EncState));
     st->frames_per_packet = framesize_ms == 20 ? 1 : 2;
     st->hb_frame = joint_hb ? 320 : HB_FRAME;
-    if (targetRate_bps <= 0) targetRate_bps = 15600;
-    i32 silk_rate = targetRate_bps - (joint_hb ? 800 : 1600);  // (1600 * 20) / bwe_framesize_ms (AGR_BWE_SDK_API.c:118)
-    silk_rate = limit(silk_rate, 5000, 100000);
-    st->targetRate_bps = silk_rate;
-    st->useDTX = dtx_enable ? 1 : 0;
+    // the Init settings go through the per-packet control; the reference starts with no expected loss (AGR_BWE_SDK_API.c:38)
+    enc_set_control(st, targetRate_bps <= 0 ? 15600 : targetRate_bps, dtx_enable ? 1 : 0, 0);
     st->useMDIndex = useMDIndex;
     st->variable_HP_smth1_Q15 = 200844;
     st->variable_HP_smth2_Q15 = 200844;
@@ -40,24 +70,6 @@ SB_FN int enc_state_init(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 u
     st->pf_lagPrev = 100;
     st->LastGainIndex = 1;
     st->nsq[0].lagPrev = 100;
-    // setup_rate (control_codec_FIX.c:319-389)
-    const i32* rt = SB_T(target_rate_table_nb);
-    const i32* snr = SB_T(snr_table_q1);
-    i32 md_rate = silk_rate / 2;
-    for (int k = 1; k < 8; k++) {
-        if (md_rate < rt[k]) {
-            i32 frac_Q6 = shl(md_rate - rt[k - 1], 6) / (rt[k] - rt[k - 1]);
-            st->SNRPerMD_dB_Q7 = shl(snr[k - 1], 6) + mulw(frac_Q6, snr[k] - snr[k - 1]);
-            break;
-        }
-    }
-    for (int k = 1; k < 8; k++) {
-        if (silk_rate <= rt[k]) {
-            i32 frac_Q6 = shl(silk_rate - rt[k - 1], 6) / (rt[k] - rt[k - 1]);
-            st->SNR_dB_Q7 = shl(snr[k - 1], 6) + mulw(frac_Q6, snr[k] - snr[k - 1]);
-            break;
-        }
-    }
     st->hb_first = 1;
     return 0;
 }

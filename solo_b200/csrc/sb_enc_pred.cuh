@@ -330,7 +330,7 @@ SB_FN void quant_ltp_gains(i16* B_Q14, i32* cbk_index, i32* periodicity_index, c
         for (int k = 0; k < LTP_ORDER; k++) B_Q14[j * LTP_ORDER + k] = cbk[cbk_index[j] * LTP_ORDER + k];
 }
 
-// ---- SKP_Silk_LTP_scale_ctrl_FIX.c:39-81 (PacketLoss_perc == 0) ---------------------------------------------------
+// ---- SKP_Silk_LTP_scale_ctrl_FIX.c:39-81 ---------------------------------------------------------------------------
 SB_FN void ltp_scale_ctrl(EncSilk* st, EncCtrl* c, int frame_in_packet) {
     st->HPLTPredCodGain_Q7 = imax(c->LTPredCodGain_Q7 - st->prevLTPredCodGain_Q7, 0) + rshift_round(st->HPLTPredCodGain_Q7, 1);
     st->prevLTPredCodGain_Q7 = c->LTPredCodGain_Q7;
@@ -338,7 +338,7 @@ SB_FN void ltp_scale_ctrl(EncSilk* st, EncCtrl* c, int frame_in_packet) {
     i32 g_limit_Q15 = sigm_q15(g_out_Q5 - (3 << 5));
     c->LTP_scaleIndex = 0;
     if (frame_in_packet == 0) {
-        int round_loss = 0 + (st->frames_per_packet - 1);
+        int round_loss = st->packetLoss_perc + (st->frames_per_packet - 1);
         i32 thrld1 = SB_T(ltpscale_thresholds_q15)[imin(round_loss, 10)];
         i32 thrld2 = SB_T(ltpscale_thresholds_q15)[imin(round_loss + 1, 10)];
         if (g_limit_Q15 > thrld1) c->LTP_scaleIndex = 2;

@@ -11,6 +11,7 @@
 //   sb_enc_finish_kernel         2 threads per stream  range coding of one description each, high-band gains, payload assembly
 //   sb_decode_kernel             thread per stream     range decoding, synthesis, concealment, comfort noise, high band
 //   sb_dec_synth_kernel          warp per stream       QMF synthesis filter bank + float -> int16
+// Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -42,6 +43,13 @@ extern "C" int sb_launch_enc_hb_warp(void* states, void* scratch, const void* ba
 __global__ void __launch_bounds__(SB_TPB) sb_enc_init_kernel(EncState* states, int n, int rate, int dtx, int mdi, int framesize_ms, int joint_hb) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) enc_state_init(&states[s], rate, dtx, mdi, framesize_ms, joint_hb);
+}
+// rate / DTX / expected loss of each stream from the next packet on; a NULL array leaves that setting alone for every stream,
+// an entry outside its range (-1 by convention) for that stream
+__global__ void __launch_bounds__(SB_TPB) sb_enc_control_kernel(EncState* states, int n, const i32* __restrict__ rate, const i32* __restrict__ dtx,
+                                                                const i32* __restrict__ loss) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < n) enc_set_control(&states[s], rate ? rate[s] : -1, dtx ? dtx[s] : -1, loss ? loss[s] : -1);
 }
 
 // ---- stage A0: QMF band split, one warp per stream, PCM tile fetched by the TMA engine ----------------------------------
@@ -342,7 +350,8 @@ struct solo_b200_enc_batch : Batch {
     EncState* d_states;
     EncScratch* d_scratch;
     i16* d_bands;               // [n][spp]: low band | high band of the packet, written by the QMF kernel
-    ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); }
+    i32* d_ctrl;                // [3][n]: rate | DTX | loss staging of the set_control host entry points (allocated on first use)
+    ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); cudaFree(d_ctrl); }
 };
 struct solo_b200_dec_batch : Batch {
     DecState* d_states;
@@ -395,7 +404,8 @@ template <class B> static B* batch_destroy(B* b) {
     return nullptr;
 }
 
-// staging allocated on first use; the payload rows grow with `cap`
+// staging allocated on first use; the payload rows grow with `cap`.  The *_host calls copy whole rows back, so the payload
+// rows start zeroed: bytes past a packet are then a function of the stream's history, never of what the memory held before.
 static int staging(Batch* b, int cap) {
     if (!b->d_pcm) CK(cudaMalloc(&b->d_pcm, sizeof(i16) * b->spp * (size_t)b->n));
     if (!b->d_nbytes) CK(cudaMalloc(&b->d_nbytes, sizeof(i16) * 2 * (size_t)b->n));
@@ -404,6 +414,8 @@ static int staging(Batch* b, int cap) {
         b->d_bits = nullptr;
         CK(cudaMalloc(&b->d_bits, (size_t)cap * b->n));
         b->bits_cap = cap;
+        CK(cudaMemsetAsync(b->d_bits, 0, (size_t)cap * b->n, b->st[0]));
+        CK(cudaStreamSynchronize(b->st[0]));    // the batch's other streams do not wait for st[0]
     }
     return 0;
 }
@@ -546,6 +558,54 @@ int solo_b200_enc_batch_encode_host(solo_b200_enc_batch* b, const int16_t* pcm, 
         CK(cudaMemcpyAsync(nbytes + 2 * (size_t)lo, b->d_nbytes + 2 * (size_t)lo, sizeof(i16) * 2 * m, cudaMemcpyDeviceToHost, st));
         return 0;
     });
+}
+
+// ---- per-stream rate / DTX / expected loss between packets (enc_set_control) ----------------------------------------------
+// What the host entry points accept: -1 (leave the setting alone), rate >= 1, dtx 0 or 1, loss 0-100.  A NULL array is fine.
+static bool control_in_range(const i32* rate, const i32* dtx, const i32* loss, int n) {
+    for (int i = 0; i < n; i++) {
+        if (rate && rate[i] != -1 && rate[i] < 1) return false;
+        if (dtx && dtx[i] != -1 && dtx[i] != 0 && dtx[i] != 1) return false;
+        if (loss && loss[i] != -1 && (loss[i] < 0 || loss[i] > 100)) return false;
+    }
+    return true;
+}
+// the control kernel for streams [lo, lo + n); the arrays hold those n streams' entries
+static int enc_control_launch(solo_b200_enc_batch* b, int lo, int n, const i32* d_rate, const i32* d_dtx, const i32* d_loss, cudaStream_t st) {
+    sb_enc_control_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(b->d_states + lo, n, d_rate, d_dtx, d_loss);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+// host arrays of streams [lo, lo + n) through the batch's staging into the control kernel on st; returns when it is done
+static int enc_control_host(solo_b200_enc_batch* b, int lo, int n, const i32* rate, const i32* dtx, const i32* loss, cudaStream_t st) {
+    if (!b->d_ctrl) CK(cudaMalloc(&b->d_ctrl, sizeof(i32) * 3 * (size_t)b->n));
+    const i32* src[3] = {rate, dtx, loss};
+    const i32* dev[3] = {nullptr, nullptr, nullptr};
+    for (int k = 0; k < 3; k++) {
+        if (!src[k]) continue;
+        i32* d = b->d_ctrl + (size_t)k * b->n + lo;
+        CK(cudaMemcpyAsync(d, src[k], sizeof(i32) * (size_t)n, cudaMemcpyHostToDevice, st));
+        dev[k] = d;
+    }
+    if (int e = enc_control_launch(b, lo, n, dev[0], dev[1], dev[2], st)) return e;
+    CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int solo_b200_enc_batch_set_control_device(solo_b200_enc_batch* b, const int32_t* d_rate_bps, const int32_t* d_dtx, const int32_t* d_loss_perc, void* cuda_stream) {
+    if (!b) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    CK(cudaSetDevice(b->device));
+    if (!d_rate_bps && !d_dtx && !d_loss_perc) return 0;
+    return enc_control_launch(b, 0, b->n, d_rate_bps, d_dtx, d_loss_perc, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_enc_batch_set_control_host(solo_b200_enc_batch* b, const int32_t* rate_bps, const int32_t* dtx, const int32_t* loss_perc) {
+    if (!b) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (!control_in_range(rate_bps, dtx, loss_perc, b->n)) { snprintf(g_err, sizeof g_err, "set_control: a setting is out of range"); return -1; }
+    CK(cudaSetDevice(b->device));
+    CK(cudaDeviceSynchronize());    // after the packet waves already enqueued, on the batch's streams and on caller streams
+    return enc_control_host(b, 0, b->n, rate_bps, dtx, loss_perc, b->st[0]);
 }
 
 void solo_b200_enc_batch_destroy(solo_b200_enc_batch* b) { batch_destroy(b); }
@@ -815,6 +875,18 @@ SKP_int32 AGR_Sate_Encoder_Encode(void* SATEEnc_State, const SKP_int16* AGR_Sate
     return n;
 }
 int AGR_Sate_Encoder_Uninit(void* SATEEnc_State) { return arena_close<solo_b200_enc_batch>(SATEEnc_State, ENC_MAGIC); }
+// the handle's slot gets the settings of the batched call (-1 leaves one alone); encodes of the handle are synchronous, so
+// the next one sees them
+int solo_b200_encoder_set_control(void* SATEEnc_State, int32_t rate_bps, int32_t dtx, int32_t loss_perc) {
+    EncHandle* h = (EncHandle*)SATEEnc_State;
+    if (!h || h->magic != ENC_MAGIC) return -1;
+    const i32 v[3] = {rate_bps, dtx, loss_perc};
+    if (!control_in_range(&v[0], &v[1], &v[2], 1)) return -1;
+    solo_b200_enc_batch* b = h->seg->b;
+    std::lock_guard<std::mutex> lk(h->seg->mu);
+    CK(cudaSetDevice(b->device));
+    return enc_control_host(b, h->slot, 1, v[0] != -1 ? &v[0] : nullptr, v[1] != -1 ? &v[1] : nullptr, v[2] != -1 ? &v[2] : nullptr, b->st[0]);
+}
 
 void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
     if (!dec_Ctrl) return nullptr;
