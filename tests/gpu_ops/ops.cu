@@ -1,0 +1,350 @@
+// Test-only harness: single routines of the analysis kernel's warp-cooperative form (sb_coop.cuh) and of the level-0 kit
+// (sb_common.cuh), compiled for sm_90a exactly as sb_analysis.cu compiles them, one warp per case.  Each kernel reads its
+// case from global memory, stages the routine's scratch struct and arrays in shared memory as the analysis kernel does,
+// calls the routine and writes every output back.  tests/test_gpu_ops.py compares the results with the reference.
+// Every launcher takes host arrays, copies them to the device and back, and returns a CUDA error code (0 = success).
+#define SB_COOP 1
+#define SB_DIV_OUTLINE 1
+#define SB_BLOCK_STREAMS 8
+#include <cuda_runtime.h>
+#include "sb_coop.cuh"
+
+using namespace sb;
+
+namespace {
+
+// ---- level-0 primitives, one thread per element -------------------------------------------------------------------------
+enum PrimOp {
+    OP_SMULWB, OP_SMULWT, OP_SMMUL, OP_ADD_SAT32, OP_SUB_SAT32, OP_CLZ32, OP_CLZ64, OP_DIV_Q29, OP_DIV32_VARQ,
+    OP_INVERSE32_VARQ, OP_SQRT_APPROX, OP_LIN2LOG, OP_LOG2LIN, OP_SIGM_Q15, OP_LSHIFT_SAT32, OP_POPC32, OP_CTZ32,
+    OP_FLOAT2INT, OP_TRUNC_I32, OP_SMULWW,
+};
+
+__global__ void prim_kernel(int op, const long long* a, const long long* b, const long long* c, const double* f, long long* out, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const i32 x = (i32)a[i], y = (i32)b[i];
+    long long r = 0;
+    switch (op) {
+        case OP_SMULWB: r = smulwb(x, y); break;
+        case OP_SMULWT: r = smulwt(x, y); break;
+        case OP_SMMUL: r = smmul(x, y); break;
+        case OP_ADD_SAT32: r = add_sat32(x, y); break;
+        case OP_SUB_SAT32: r = sub_sat32(x, y); break;
+        case OP_CLZ32: r = clz32(x); break;
+        case OP_CLZ64: r = clz64((i64)a[i]); break;
+        case OP_DIV_Q29: r = div_q29(x); break;
+        case OP_DIV32_VARQ: r = div32_varq(x, y, (int)c[i]); break;
+        case OP_INVERSE32_VARQ: r = inverse32_varq(x, (int)c[i]); break;
+        case OP_SQRT_APPROX: r = sqrt_approx(x); break;
+        case OP_LIN2LOG: r = lin2log(x); break;
+        case OP_LOG2LIN: r = log2lin(x); break;
+        case OP_SIGM_Q15: r = sigm_q15(x); break;
+        case OP_LSHIFT_SAT32: r = lshift_sat32(x, y); break;
+        case OP_POPC32: r = popc32((u32)x); break;
+        case OP_CTZ32: r = ctz32((u32)x); break;
+        case OP_FLOAT2INT: r = float2int(f[i]); break;
+        case OP_TRUNC_I32: r = trunc_i32(f[i]); break;
+        case OP_SMULWW: r = smulww(x, y); break;
+        default: r = 0x7fffffffffffffffLL;
+    }
+    out[i] = r;
+}
+
+// ---- c_schur (order <= 16) and c_k2a: c [17] and rc_in [16] per case -> rc_Q15 [16], residual energy, A_Q24 [16] -----
+__global__ void schur_kernel(const i32* c, const i16* rc_in, int order, i16* rc_out, i32* nrg_out, i32* A_out) {
+    __shared__ i32 cs[32];
+    __shared__ i16 rc[32], rk[32];
+    const int lane = threadIdx.x, cse = blockIdx.x;
+    cs[lane] = lane <= 16 ? c[cse * 17 + lane] : 0;
+    rc[lane] = 0;
+    rk[lane] = lane < 16 ? rc_in[cse * 16 + lane] : 0;
+    __syncwarp();
+    const i32 nrg = c_schur(rc, cs, order);
+    __syncwarp();
+    const i32 A = c_k2a(rk, order);
+    if (lane < 16) { rc_out[cse * 16 + lane] = rc[lane]; A_out[cse * 16 + lane] = lane < order ? A : 0; }
+    if (lane == 0) nrg_out[cse] = nrg;
+}
+
+// ---- schur64_r / k2a_q16_r at the shaping order, one thread per case: c [17] -> rc_Q16 [16], energy; rc_in -> A_Q24 ------
+__global__ void schur64_kernel(const i32* c, const i32* rc_in, i32* rc_out, i32* nrg_out, i32* A_out, int n) {
+    const int cse = blockIdx.x * blockDim.x + threadIdx.x;
+    if (cse >= n) return;
+    i32 cc[SHAPE_ORDER + 1], rc[SHAPE_ORDER], rk[SHAPE_ORDER], A[SHAPE_ORDER];
+#pragma unroll
+    for (int i = 0; i <= SHAPE_ORDER; i++) cc[i] = c[cse * 17 + i];
+#pragma unroll
+    for (int i = 0; i < SHAPE_ORDER; i++) rk[i] = rc_in[cse * 16 + i];
+    nrg_out[cse] = schur64_r<SHAPE_ORDER>(rc, cc);
+    k2a_q16_r<SHAPE_ORDER>(A, rk);
+#pragma unroll
+    for (int i = 0; i < SHAPE_ORDER; i++) { rc_out[cse * 16 + i] = rc[i]; A_out[cse * 16 + i] = A[i]; }
+}
+
+// ---- c_burg2<D>: two analyses per case, x [2][XMAX] (one signal per half of the warp) -----------------------------------
+enum { XMAX = NB_SUBFR * (80 + HB_ORDER) };
+struct BurgCase { i32 nb[2], L, wnf; };
+template <int D> __global__ void burg_kernel(const BurgCase* cases, const i16* x, i32* nrg_out, i32* q_out, i32* A_out) {
+    __shared__ __align__(16) i16 xs[2][XMAX];
+    __shared__ i32 A[2][16];
+    __shared__ BurgScr B;
+    const int lane = threadIdx.x, cse = blockIdx.x;
+    const BurgCase k = cases[cse];
+    for (int i = lane; i < 2 * XMAX; i += 32) xs[i / XMAX][i % XMAX] = x[(size_t)cse * 2 * XMAX + i];
+    A[lane >> 4][lane & 15] = 0;
+    __syncwarp();
+    i32 rn, rq;
+    c_burg2<D>(&rn, &rq, A, &B, xs[0], k.nb[0], xs[1], k.nb[1], k.L, k.wnf);
+    __syncwarp();
+    if ((lane & 15) == 0) { nrg_out[cse * 2 + (lane >> 4)] = rn; q_out[cse * 2 + (lane >> 4)] = rq; }
+    A_out[cse * 32 + lane] = A[lane >> 4][lane & 15];
+}
+
+// ---- c_a2nlsf<D>: a_Q16 [16] in / out (widened in place), NLSF [16] ----------------------------------------------------
+template <int D> __global__ void a2nlsf_kernel(i32* a, i32* nlsf_out) {
+    __shared__ i32 as[16], nl[16];
+    __shared__ A2nlsfScr Z;
+    const int lane = threadIdx.x, cse = blockIdx.x;
+    if (lane < 16) { as[lane] = a[cse * 16 + lane]; nl[lane] = -1; }
+    __syncwarp();
+    c_a2nlsf<D>(nl, as, &Z);
+    __syncwarp();
+    if (lane < 16) { a[cse * 16 + lane] = as[lane]; nlsf_out[cse * 16 + lane] = nl[lane]; }
+}
+
+// ---- c_warped_autocorr4: four windows [4][SHAPE_WIN] per case -> corr [4][17], scale [4] --------------------------------
+__global__ void warped_kernel(const i16* x, const i32* warping, i32* corr_out, i32* scale_out) {
+    __shared__ ShapeScr S;
+    const int lane = threadIdx.x, cse = blockIdx.x;
+    for (int i = lane; i < NB_SUBFR * SHAPE_WIN; i += 32) S.xw[i / SHAPE_WIN][i % SHAPE_WIN] = x[(size_t)cse * NB_SUBFR * SHAPE_WIN + i];
+    for (int i = lane; i < NB_SUBFR * (SHAPE_ORDER + 1); i += 32) S.acorr[i / (SHAPE_ORDER + 1)][i % (SHAPE_ORDER + 1)] = 0x5a5a5a5a;
+    __syncwarp();
+    c_warped_autocorr4(&S, warping[cse]);
+    __syncwarp();
+    for (int i = lane; i < NB_SUBFR * (SHAPE_ORDER + 1); i += 32) corr_out[cse * NB_SUBFR * (SHAPE_ORDER + 1) + i] = S.acorr[i / (SHAPE_ORDER + 1)][i % (SHAPE_ORDER + 1)];
+    if (lane < NB_SUBFR) scale_out[cse * NB_SUBFR + lane] = S.scale[lane];
+}
+
+// ---- c_quant_ltp_gains: B_Q14 [20] in / out, W_Q18 [100] -> cbk_index [4], periodicity index ---------------------------
+__global__ void ltp_kernel(i16* B, const i32* W, const i32* mu, i32* cbk_out, i32* per_out) {
+    __shared__ i16 Bs[NB_SUBFR * LTP_ORDER];
+    __shared__ i32 Ws[NB_SUBFR * LTP_ORDER * LTP_ORDER];
+    __shared__ i32 cbk[NB_SUBFR], per;
+    const int lane = threadIdx.x, cse = blockIdx.x;
+    if (lane < NB_SUBFR * LTP_ORDER) Bs[lane] = B[cse * NB_SUBFR * LTP_ORDER + lane];
+    for (int i = lane; i < NB_SUBFR * LTP_ORDER * LTP_ORDER; i += 32) Ws[i] = W[cse * NB_SUBFR * LTP_ORDER * LTP_ORDER + i];
+    if (lane < NB_SUBFR) cbk[lane] = -1;
+    if (lane == 0) per = -1;
+    __syncwarp();
+    c_quant_ltp_gains(Bs, cbk, &per, Ws, mu[cse]);
+    __syncwarp();
+    if (lane < NB_SUBFR * LTP_ORDER) B[cse * NB_SUBFR * LTP_ORDER + lane] = Bs[lane];
+    if (lane < NB_SUBFR) cbk_out[cse * NB_SUBFR + lane] = cbk[lane];
+    if (lane == 0) per_out[cse] = per;
+}
+
+// ---- routines with scalar instances (c_instances): the analysis kernel's block layout ----------------------------------
+// SB_BLOCK_STREAMS warps per block, one case each, every warp with an AnaSmem slot (sb_slot_bytes() apart) in dynamic shared
+// memory behind the NLSF codebook copy, as sb_enc_analysis_warp_kernel lays them out.  The instances of a block run on
+// consecutive threads and reach the other warps' slots, so every warp takes part: a warp beyond the last case repeats it
+// and writes nothing back.
+#define SB_OPS_TABS_BYTES ((sizeof(NlsfFastTabs) + 15) & ~15)
+constexpr int kSlotSmem = (int)SB_OPS_TABS_BYTES + SB_BLOCK_STREAMS * (int)sizeof(AnaSmem);
+__device__ __forceinline__ AnaSmem* ops_slot(unsigned char* smem_raw, int w) {
+    return reinterpret_cast<AnaSmem*>(smem_raw + SB_OPS_TABS_BYTES) + w;
+}
+
+// c_pitch_analysis_core on a 320-sample 8 kHz signal.  case: prevLag, search_thres1_Q16, search_thres2_Q15, LTPCorr_Q15 in.
+// out [8]: pitch lags [4], lagIndex, contourIndex, LTPCorr_Q15, returned signal type
+struct PitchCase { i32 prevLag, thres1_Q16, thres2_Q15, ltpcorr_Q15; };
+enum { PITCH_LEN = 320 };
+__global__ void __launch_bounds__(SB_BLOCK_STREAMS * 32) pitch_kernel(const PitchCase* cases, const i16* sig, int n, i32* out) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ i32 res[SB_BLOCK_STREAMS][8];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int s = blockIdx.x * SB_BLOCK_STREAMS + w;
+    const bool live = s < n;
+    if (!live) s = n - 1;
+    AnaSmem* S = ops_slot(smem_raw, w);
+    PitchScr* P = &S->W.u.pitch;
+    i16* signal = S->W.res_pitch;
+    static_assert(sizeof(S->W.res_pitch) >= PITCH_LEN * sizeof(i16), "pitch signal fits the residual buffer");
+    for (int i = lane; i < PITCH_LEN; i += 32) signal[i] = sig[(size_t)s * PITCH_LEN + i];
+    const PitchCase k = cases[s];
+    if (lane < 8) res[w][lane] = -1;
+    __syncwarp();
+    if (lane == 0) res[w][6] = k.ltpcorr_Q15;
+    __syncwarp();
+    const int sigtype = c_pitch_analysis_core(P, signal, &res[w][0], &res[w][4], &res[w][5], &res[w][6], k.prevLag, k.thres1_Q16, k.thres2_Q15);
+    __syncwarp();
+    if (lane == 0) res[w][7] = sigtype;
+    __syncwarp();
+    if (live && lane < 8) out[(size_t)s * 8 + lane] = res[w][lane];
+}
+
+// c_nlsf_msvq_encode, order 10.  case: NLSF_mu_Q15, NLSF_mu_fluc_red_Q16, deactivate_fluc_red, sigtype; nlsf / prev / w [10].
+// out: indices [6], quantised NLSF [10].  The target, the previous quantised vector, the weights and the results live where
+// c_process_nlsfs keeps them: PredScr, EncSilk and EncCtrl of the slot.
+struct MsvqCase { i32 mu_Q15, fluc_red_Q16, deactivate, sigtype; };
+__global__ void __launch_bounds__(SB_BLOCK_STREAMS * 32) msvq_kernel(const MsvqCase* cases, const i32* nlsf, const i32* prev, const i32* wts, int n,
+                                                                     i32* idx_out, i32* nlsf_out) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    NlsfFastTabs* tabs = reinterpret_cast<NlsfFastTabs*>(smem_raw);
+    nlsf_fast_tabs_fill(tabs, threadIdx.x, blockDim.x);
+    __syncthreads();
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int s = blockIdx.x * SB_BLOCK_STREAMS + w;
+    const bool live = s < n;
+    if (!live) s = n - 1;
+    AnaSmem* S = ops_slot(smem_raw, w);
+    PredScr* Q = &S->W.u.pred;
+    const MsvqCase k = cases[s];
+    if (lane < LPC_ORDER) {
+        Q->NLSF_Q15[lane] = nlsf[s * LPC_ORDER + lane];
+        S->st.prev_NLSFq_Q15[lane] = prev[s * LPC_ORDER + lane];
+        Q->NLSFW_Q6[lane] = wts[s * LPC_ORDER + lane];
+    }
+    if (lane < 6) S->W.c.NLSFIndices[lane] = -1;
+    __syncwarp();
+    NlsfCb cb = nlsf_cb(k.sigtype);
+    cb.cb_q15 = k.sigtype == 0 ? tabs->cb0 : tabs->cb1;
+    cb.rates_q5 = k.sigtype == 0 ? tabs->rates0 : tabs->rates1;
+    c_nlsf_msvq_encode(S->W.c.NLSFIndices, Q->NLSF_Q15, cb, S->st.prev_NLSFq_Q15, Q->NLSFW_Q6, k.mu_Q15, k.fluc_red_Q16, k.deactivate,
+                       k.sigtype, Q);
+    __syncthreads();
+    if (live && lane < 6) idx_out[s * 6 + lane] = S->W.c.NLSFIndices[lane];
+    if (live && lane < LPC_ORDER) nlsf_out[s * LPC_ORDER + lane] = Q->NLSF_Q15[lane];
+}
+
+template <class T> struct Dev {
+    T* p = nullptr;
+    size_t n = 0;
+    cudaError_t err = cudaSuccess;
+    Dev(const T* h, size_t count) : n(count) {
+        err = cudaMalloc(&p, sizeof(T) * (n ? n : 1));
+        if (err == cudaSuccess && h && n) err = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
+    }
+    cudaError_t back(T* h) const { return cudaMemcpy(h, p, sizeof(T) * n, cudaMemcpyDeviceToHost); }
+    ~Dev() { if (p) cudaFree(p); }
+};
+
+#define SB_CHECK(e) do { const cudaError_t e_ = (e); if (e_ != cudaSuccess) return (int)e_; } while (0)
+cudaError_t finish() {
+    const cudaError_t e = cudaGetLastError();
+    return e != cudaSuccess ? e : cudaDeviceSynchronize();
+}
+
+}  // namespace
+
+extern "C" int sb_ops_prim(int op, const long long* a, const long long* b, const long long* c, const double* f, long long* out, int n) {
+    if (n <= 0) return 0;
+    Dev<long long> da(a, n), db(b, n), dc(c, n), dout(nullptr, n);
+    Dev<double> df(f, n);
+    SB_CHECK(da.err); SB_CHECK(db.err); SB_CHECK(dc.err); SB_CHECK(dout.err); SB_CHECK(df.err);
+    prim_kernel<<<(n + 255) / 256, 256>>>(op, da.p, db.p, dc.p, df.p, dout.p, n);
+    SB_CHECK(finish());
+    return (int)dout.back(out);
+}
+
+extern "C" int sb_ops_schur(const int32_t* c, const int16_t* rc_in, int order, int n, int16_t* rc, int32_t* nrg, int32_t* A) {
+    if (order < 1 || order > 16) return -1;
+    Dev<i32> dc(c, 17 * (size_t)n), dA(nullptr, 16 * (size_t)n), dn(nullptr, n);
+    Dev<i16> dri(rc_in, 16 * (size_t)n), drc(nullptr, 16 * (size_t)n);
+    SB_CHECK(dc.err); SB_CHECK(dA.err); SB_CHECK(dn.err); SB_CHECK(dri.err); SB_CHECK(drc.err);
+    schur_kernel<<<n, 32>>>(dc.p, dri.p, order, drc.p, dn.p, dA.p);
+    SB_CHECK(finish());
+    SB_CHECK(drc.back(rc)); SB_CHECK(dn.back(nrg));
+    return (int)dA.back(A);
+}
+
+extern "C" int sb_ops_schur64(const int32_t* c, const int32_t* rc_in, int n, int32_t* rc, int32_t* nrg, int32_t* A) {
+    Dev<i32> dc(c, 17 * (size_t)n), dri(rc_in, 16 * (size_t)n), drc(nullptr, 16 * (size_t)n), dn(nullptr, n), dA(nullptr, 16 * (size_t)n);
+    SB_CHECK(dc.err); SB_CHECK(dri.err); SB_CHECK(drc.err); SB_CHECK(dn.err); SB_CHECK(dA.err);
+    schur64_kernel<<<(n + 63) / 64, 64>>>(dc.p, dri.p, drc.p, dn.p, dA.p, n);
+    SB_CHECK(finish());
+    SB_CHECK(drc.back(rc)); SB_CHECK(dn.back(nrg));
+    return (int)dA.back(A);
+}
+
+extern "C" int sb_ops_burg_xmax() { return XMAX; }
+
+// cases: int32 [n][4] = nb0, nb1, L, WhiteNoiseFrac_Q32; x: int16 [n][2][XMAX]; outputs per half
+extern "C" int sb_ops_burg(int D, const int32_t* cases, const int16_t* x, int n, int32_t* nrg, int32_t* q, int32_t* A) {
+    if (D != 10 && D != 8) return -1;
+    for (int i = 0; i < n; i++) {
+        const int32_t* k = cases + 4 * i;
+        if (k[0] < 1 || k[0] > NB_SUBFR || k[1] < 1 || k[1] > NB_SUBFR || k[2] <= D || k[0] * k[2] > XMAX || k[1] * k[2] > XMAX) return -1;
+    }
+    Dev<BurgCase> dk(reinterpret_cast<const BurgCase*>(cases), n);
+    Dev<i16> dx(x, (size_t)n * 2 * XMAX);
+    Dev<i32> dn(nullptr, 2 * (size_t)n), dq(nullptr, 2 * (size_t)n), dA(nullptr, 32 * (size_t)n);
+    SB_CHECK(dk.err); SB_CHECK(dx.err); SB_CHECK(dn.err); SB_CHECK(dq.err); SB_CHECK(dA.err);
+    if (D == 10) burg_kernel<10><<<n, 32>>>(dk.p, dx.p, dn.p, dq.p, dA.p);
+    else burg_kernel<8><<<n, 32>>>(dk.p, dx.p, dn.p, dq.p, dA.p);
+    SB_CHECK(finish());
+    SB_CHECK(dn.back(nrg)); SB_CHECK(dq.back(q));
+    return (int)dA.back(A);
+}
+
+// a: int32 [n][16] in / out; nlsf: int32 [n][16]
+extern "C" int sb_ops_a2nlsf(int D, int32_t* a, int n, int32_t* nlsf) {
+    if (D != 10 && D != 8) return -1;
+    Dev<i32> da(a, 16 * (size_t)n), dn(nullptr, 16 * (size_t)n);
+    SB_CHECK(da.err); SB_CHECK(dn.err);
+    if (D == 10) a2nlsf_kernel<10><<<n, 32>>>(da.p, dn.p);
+    else a2nlsf_kernel<8><<<n, 32>>>(da.p, dn.p);
+    SB_CHECK(finish());
+    SB_CHECK(da.back(a));
+    return (int)dn.back(nlsf);
+}
+
+// x: int16 [n][4][SHAPE_WIN]; warping: int32 [n]; corr: int32 [n][4][17]; scale: int32 [n][4]
+extern "C" int sb_ops_warped_autocorr(const int16_t* x, const int32_t* warping, int n, int32_t* corr, int32_t* scale) {
+    Dev<i16> dx(x, (size_t)n * NB_SUBFR * SHAPE_WIN);
+    Dev<i32> dw(warping, n), dc(nullptr, (size_t)n * NB_SUBFR * (SHAPE_ORDER + 1)), ds(nullptr, (size_t)n * NB_SUBFR);
+    SB_CHECK(dx.err); SB_CHECK(dw.err); SB_CHECK(dc.err); SB_CHECK(ds.err);
+    warped_kernel<<<n, 32>>>(dx.p, dw.p, dc.p, ds.p);
+    SB_CHECK(finish());
+    SB_CHECK(dc.back(corr));
+    return (int)ds.back(scale);
+}
+
+// B: int16 [n][20] in / out; W: int32 [n][100]; mu: int32 [n]; cbk: int32 [n][4]; per: int32 [n]
+extern "C" int sb_ops_quant_ltp_gains(int16_t* B, const int32_t* W, const int32_t* mu, int n, int32_t* cbk, int32_t* per) {
+    Dev<i16> dB(B, (size_t)n * NB_SUBFR * LTP_ORDER);
+    Dev<i32> dW(W, (size_t)n * NB_SUBFR * LTP_ORDER * LTP_ORDER), dm(mu, n), dc(nullptr, (size_t)n * NB_SUBFR), dp(nullptr, n);
+    SB_CHECK(dB.err); SB_CHECK(dW.err); SB_CHECK(dm.err); SB_CHECK(dc.err); SB_CHECK(dp.err);
+    ltp_kernel<<<n, 32>>>(dB.p, dW.p, dm.p, dc.p, dp.p);
+    SB_CHECK(finish());
+    SB_CHECK(dB.back(B)); SB_CHECK(dc.back(cbk));
+    return (int)dp.back(per);
+}
+
+// cases: int32 [n][4] (PitchCase); sig: int16 [n][320]; out: int32 [n][8]
+extern "C" int sb_ops_pitch(const int32_t* cases, const int16_t* sig, int n, int32_t* out) {
+    if (n <= 0) return 0;
+    SB_CHECK(cudaFuncSetAttribute(pitch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSlotSmem));
+    Dev<PitchCase> dk(reinterpret_cast<const PitchCase*>(cases), n);
+    Dev<i16> ds(sig, (size_t)n * PITCH_LEN);
+    Dev<i32> dout(nullptr, (size_t)n * 8);
+    SB_CHECK(dk.err); SB_CHECK(ds.err); SB_CHECK(dout.err);
+    pitch_kernel<<<(n + SB_BLOCK_STREAMS - 1) / SB_BLOCK_STREAMS, SB_BLOCK_STREAMS * 32, kSlotSmem>>>(dk.p, ds.p, n, dout.p);
+    SB_CHECK(finish());
+    return (int)dout.back(out);
+}
+
+// cases: int32 [n][4] (MsvqCase); nlsf, prev, w: int32 [n][10]; idx: int32 [n][6]; nlsf_q: int32 [n][10]
+extern "C" int sb_ops_msvq(const int32_t* cases, const int32_t* nlsf, const int32_t* prev, const int32_t* w, int n, int32_t* idx, int32_t* nlsf_q) {
+    if (n <= 0) return 0;
+    for (int i = 0; i < n; i++) if (cases[4 * i + 3] != 0 && cases[4 * i + 3] != 1) return -1;
+    SB_CHECK(cudaFuncSetAttribute(msvq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSlotSmem));
+    Dev<MsvqCase> dk(reinterpret_cast<const MsvqCase*>(cases), n);
+    Dev<i32> dn(nlsf, (size_t)n * LPC_ORDER), dp(prev, (size_t)n * LPC_ORDER), dw(w, (size_t)n * LPC_ORDER);
+    Dev<i32> di(nullptr, (size_t)n * 6), dq(nullptr, (size_t)n * LPC_ORDER);
+    SB_CHECK(dk.err); SB_CHECK(dn.err); SB_CHECK(dp.err); SB_CHECK(dw.err); SB_CHECK(di.err); SB_CHECK(dq.err);
+    msvq_kernel<<<(n + SB_BLOCK_STREAMS - 1) / SB_BLOCK_STREAMS, SB_BLOCK_STREAMS * 32, kSlotSmem>>>(dk.p, dn.p, dp.p, dw.p, n, di.p, dq.p);
+    SB_CHECK(finish());
+    SB_CHECK(di.back(idx));
+    return (int)dq.back(nlsf_q);
+}
