@@ -1,7 +1,7 @@
 """ctypes binding of the UNMODIFIED reference codec built by oracle/Makefile into oracle/_ref/.
 
-TEST / BASELINE INFRASTRUCTURE ONLY.  Only tests/, __graft_entry__.smoke() and bench.py's
-cpu_baseline / --impl reference legs may import this module.  Nothing under solo_b200/ does.
+TEST INFRASTRUCTURE ONLY.  Only tests/ and __graft_entry__.smoke() import this module (bench.py runs the
+reference's own executable).  Nothing under solo_b200/ does.
 
 API bound: JC1_SDK_SRC_{ARM,FLP}/interface/AGR_JC1_SDK_API.h:33-64 (six functions).
 Internal reference functions (exported by the .so because they are non-static C) are reachable
@@ -26,6 +26,17 @@ class DecCtrl(C.Structure):
     # AGR_JC1_SDK_API.h:23-31
     _fields_ = [(n, C.c_int32) for n in ("packetLoss_perc", "samplerate", "framesize_ms",
                                          "joint_enable", "joint_mode", "useMDIndex")]
+
+
+class SilkEncControl(C.Structure):
+    # SKP_SILK_SDK_EncControlStruct (interface/SKP_Silk_control.h:41-69): nine ints
+    _fields_ = [(n, C.c_int32) for n in ("API_sampleRate", "maxInternalSampleRate", "packetSize", "bitRate", "packetLossPercentage",
+                                         "complexity", "useInBandFEC", "useDTX", "useMDIndex")]
+
+
+class SateEncHead(C.Structure):
+    # the leading fields of SATEEncCtl (libBWE/AGR_BWE_structs.h:61-67): SILK state, high-band state, SILK control
+    _fields_ = [("stEnc", C.c_void_p), ("stHBEnc", C.c_void_p), ("encControl", SilkEncControl)]
 
 
 def available():
@@ -63,6 +74,7 @@ class RefEncoder:
     """One reference encoder handle (kind = 'fix' | 'flp')."""
 
     def __init__(self, kind="fix", rate=13600, dtx=0, use_md_index=0, framesize_ms=40, joint_hb=0):
+        self.kind = kind
         self.L = lib(kind).lib
         self.samples = 16 * framesize_ms
         self.ctrl = EncCtrl(2, rate, 16000, dtx, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
@@ -76,6 +88,28 @@ class RefEncoder:
         C.memset(self._nb, 0, 12)
         n = self.L.AGR_Sate_Encoder_Encode(self.h, pcm.ctypes.data, self._bits, 1024, self._nb)
         return bytes(self._bits[:max(n, 0)]), (int(self._nb[0]), int(self._nb[1])), n
+
+    def head(self):
+        return C.cast(C.c_void_p(self.h), C.POINTER(SateEncHead)).contents
+
+    def set_control(self, rate=None, dtx=None, loss=None):
+        """From the next packet on: target rate (b/s, less 1600 -- or 800 with joint mode 1 -- as Init computes bitRate,
+        AGR_BWE_SDK_API.c:118), useDTX, packetLossPercentage.  None leaves a field as it is.
+
+        The SDK sets these three once, in AGR_Sate_Encoder_Init (AGR_BWE_SDK_API.c:38-119), but its SILK core re-reads them
+        from the handle's encControl at the start of every packet (SKP_Silk_enc_API.c:161-191), so writing them into a live
+        handle the way Init does makes the reference follow a settings schedule.  The handle description above
+        (SateEncHead) has only been checked against the FIX library, by tests/test_enc_control.py; the FLP build keeps its
+        own SILK structures, so an "flp" handle is refused rather than written through an unchecked layout."""
+        if self.kind != "fix":
+            raise ValueError("set_control: only the FIX library's handle layout is known")
+        c = self.head().encControl
+        if rate is not None:
+            c.bitRate = int(rate) - (800 if self.ctrl.joint_enable and self.ctrl.joint_mode == 1 else 1600)
+        if dtx is not None:
+            c.useDTX = int(dtx)
+        if loss is not None:
+            c.packetLossPercentage = int(loss)
 
     def close(self):
         if self.h:

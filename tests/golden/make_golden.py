@@ -15,7 +15,6 @@ Writes:
 """
 import hashlib
 import os
-import struct
 import sys
 
 import numpy as np
@@ -23,24 +22,10 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from oracle import ref  # noqa: E402
-from tests.util import loss_flags, synth_inputs, trim_payload  # noqa: E402
+from tests.util import bitfile, encode_signal, loss_flags, synth_inputs, trim_payload  # noqa: E402
 
 CLIP = "/root/reference/JC1_SDK_SRC_ARM/bin/Ch_f1_raw.pcm"
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def encode_stream(pcm, rate=13600, dtx=0, mdi=0):
-    e = ref.RefEncoder("fix", rate=rate, dtx=dtx, use_md_index=mdi)
-    pk = []
-    for i in range(len(pcm) // 640):
-        b, nb, n = e.encode(pcm[i * 640:(i + 1) * 640])
-        pk.append((b, nb, n))
-    e.close()
-    return pk
-
-
-def bitfile(pk):
-    return b"".join(struct.pack("<hh", *nb) + (b if nb[0] else b"") for b, nb, n in pk)
 
 
 def decode_stream(pk, flags, mdi=0):
@@ -58,7 +43,7 @@ def main():
     clip = np.fromfile(CLIP, dtype=np.int16)
     np.savez_compressed(os.path.join(HERE, "speech_clip.npz"), pcm=clip)
     g = {}
-    pk = encode_stream(clip)
+    pk = encode_signal(ref.RefEncoder("fix", rate=13600), clip)
     cap = 128
     bits = np.zeros((len(pk), cap), np.uint8)
     nbytes = np.zeros((len(pk), 2), np.int16)
@@ -79,7 +64,7 @@ def main():
     g["flp_pcm_loss50_md5"] = hashlib.md5(pcm.tobytes()).hexdigest()
     # synthetic inputs: md5 of the FIX payload stream
     for name, x, kw in synth_inputs(clip):
-        p = encode_stream(x, **kw)
+        p = encode_signal(ref.RefEncoder("fix", **kw), x)
         g["synth_" + name] = hashlib.md5(bitfile(p)).hexdigest()
     np.savez_compressed(os.path.join(HERE, "golden.npz"), **g)
     for k in sorted(g):

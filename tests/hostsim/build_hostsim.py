@@ -1,9 +1,15 @@
 """Build the host (g++) compilation of the per-stream kernel source -- CPU test infrastructure only."""
 import os
 import subprocess
+import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from solo_b200 import build as sb_build  # noqa: E402
+
 OUT_DIR = os.path.join(ROOT, "tests", "_hostsim")
 OUT = os.path.join(OUT_DIR, "libsb_hostsim.so")
 SRC = os.path.join(HERE, "hostsim.cpp")
@@ -21,8 +27,7 @@ def build(force=False, emu=False):
 
 def _build(OUT, extra, force):
     os.makedirs(OUT_DIR, exist_ok=True)
-    csrc = os.path.join(ROOT, "solo_b200", "csrc")
-    deps = [SRC] + [os.path.join(csrc, f) for f in os.listdir(csrc)]
+    deps = sb_build.sources() + [SRC, os.path.abspath(__file__)]     # the flags live here: a flag change rebuilds
     if not force and os.path.exists(OUT) and all(os.path.getmtime(d) <= os.path.getmtime(OUT) for d in deps):
         return OUT
     subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w"] + extra + [SRC, "-o", OUT])

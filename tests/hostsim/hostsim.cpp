@@ -223,6 +223,9 @@ int hs_enc_encode_pair(void* pa, void* pb, const short* pcm_a, const short* pcm_
     return -1;
 #endif
 }
+// rate (b/s), DTX, expected loss (%) from the next packet on: the body of the device's control kernel on the host model's
+// state; -1 or any other out-of-range value leaves a setting alone
+void hs_enc_set_control(void* p, int rate, int dtx, int loss) { sb::enc_set_control(&((HsEnc*)p)->st, rate, dtx, loss); }
 void hs_enc_destroy(void* p) { free(p); }
 int hs_is_emu() {
 #ifdef SB_EMU

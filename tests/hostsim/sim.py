@@ -22,6 +22,7 @@ def lib(emu=None):
         L.hs_dec_create3.argtypes = [C.c_int] * 3
         L.hs_enc_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.hs_enc_destroy.argtypes = [C.c_void_p]
+        L.hs_enc_set_control.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.hs_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.hs_dec_destroy.argtypes = [C.c_void_p]
         if emu:
@@ -50,6 +51,10 @@ class SimEncoder:
             self.L.hs_set_emu_nsq(1 if self.emu_nsq else 0)
         n = self.L.hs_enc_encode(self.h, x.ctypes.data, self.out.ctypes.data, self.cap, self.nb.ctypes.data)
         return bytes(self.out[:max(n, 0)]), (int(self.nb[0]), int(self.nb[1])), n
+
+    def set_control(self, rate=None, dtx=None, loss=None):
+        """Rate (b/s), DTX and expected loss (%) from the next packet on, through enc_set_control; None = unchanged."""
+        self.L.hs_enc_set_control(self.h, *(-1 if v is None else int(v) for v in (rate, dtx, loss)))
 
     def close(self):
         if self.h:

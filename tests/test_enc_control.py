@@ -1,31 +1,15 @@
 """Encoder settings changed between packets -- target rate, DTX and expected packet loss per stream (enc_set_control) --
 on the CPU: the host model of the kernel source (tests/hostsim) against the unmodified FIX reference fed the same settings
-schedule through its handle (tests/enc_control_ref.py).  Bar: payloads and both length fields byte-identical."""
+schedule through its handle (oracle.ref.RefEncoder.set_control).  Bar: payloads and both length fields byte-identical."""
 import numpy as np
 import pytest
 
-from tests.test_gpu_hetero import signal_classes
-from tests.util import load_clip
+from tests.parity import ref, sim  # noqa: F401  (fixtures)
+from tests.util import load_clip, signal_classes
 
 MODES = {"40ms": dict(), "20ms": dict(framesize_ms=20), "joint1": dict(joint_hb=1)}
 P = 48                      # packets per schedule
 SILENCE = (12, 26)          # packets [12, 26) of every input are silent, so DTX is switched while there is nothing to code
-
-
-@pytest.fixture(scope="module")
-def sim():
-    from tests.hostsim import enc_control as s
-    s.lib()
-    return s
-
-
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built")
-    from tests import enc_control_ref
-    return enc_control_ref
 
 
 def inputs(spp):
@@ -112,6 +96,8 @@ def test_reference_handle_layout(ref):
             e.L.SKP_Silk_SDK_QueryEncoder(e.head().stEnc, C.byref(q))
             assert (q.bitRate, q.packetLossPercentage, q.useDTX) == (want_rate, loss, dtx), kw
         e.close()
+    with pytest.raises(ValueError):                     # the FLP build's layout is not described
+        ref.RefEncoder("flp").set_control(rate=13600)
 
 
 def test_loss_schedule_through_the_32_lane_analysis(sim, ref):

@@ -6,14 +6,8 @@ import hashlib
 import numpy as np
 import pytest
 
+from tests.parity import sb  # noqa: F401  (fixture)
 from tests.util import load_golden, trim_payload
-
-
-@pytest.fixture(scope="module")
-def sb():
-    import solo_b200
-    solo_b200.lib()
-    return solo_b200
 
 
 def rows():

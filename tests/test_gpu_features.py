@@ -3,16 +3,10 @@
 import numpy as np
 import pytest
 
+from tests.parity import DevicePath, RefRows, batch_packets, received, ref, sb  # noqa: F401  (fixtures)
 from tests.util import load_clip, load_golden, loss_flags, speech_replay, trim_payload
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def sb():
-    import solo_b200
-    solo_b200.lib()
-    return solo_b200
 
 
 def run_streams(sb, N, T, cap=128, flags=None, rate=13600):
@@ -130,35 +124,26 @@ def test_loss_trimming_on_device_matches_the_receiver_restatement(sb):
     eb.close(); db.close(); db_ref.close()
 
 
-def test_config2_batch_4096_streams_50_packets_sampled_against_reference(sb):
+def test_config2_batch_4096_streams_50_packets_sampled_against_reference(sb, ref):
     """BASELINE config 2: 4 096 concurrent streams, encode only, 50 packets (2 s).  Every stream runs on the GPU; 64 of
     them (spread over the batch, all four input gains) are replayed through libjc1_fix.so and must match byte for byte."""
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref not built")
     N, T, cap = 4096, 50, 160
     clip = load_clip()
     sample = sorted(set(list(range(0, N, 67)) + [1, 2, 3, N - 1]))[:64]
-    refs = {s: ref.RefEncoder("fix", rate=13600) for s in sample}
-    eb = sb.EncoderBatch(N, rate=13600)
+    eb, rr = sb.EncoderBatch(N, rate=13600), RefRows(ref, sample, rate=13600)
     for p in range(T):
         x = speech_replay(clip, N, 1, first_packet=p)[0]
         bits, nb = eb.encode(x, cap=cap)
         assert (nb[:, 0] <= cap).all()
-        for s in sample:
-            b, rnb, n = refs[s].encode(x[s])
-            assert tuple(nb[s]) == rnb and bytes(bits[s, :n]) == b, (p, s)
+        rr.step(x[sample], bits[sample], nb[sample])
+    rr.close()
     eb.close()
 
 
-def test_config5_full_batch_with_per_stream_loss_sampled_against_reference(sb):
+def test_config5_full_batch_with_per_stream_loss_sampled_against_reference(sb, ref):
     """BASELINE configs 3 + 5 at full size: 65 536 streams, encode -> receiver-side trimming on the device -> decode with
-    a 50 % loss process per stream (seed 1 + stream id, dec_main.c:229-241); 48 sampled streams against libjc1_flp.so fed
-    the same payloads and flags (PCM identical; the north star allows +-1 LSB)."""
-    import torch
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref not built")
+    a 50 % loss process per stream (seed 1 + stream id, dec_main.c:229-241); 48 sampled streams against libjc1_fix.so and
+    against libjc1_flp.so fed the same payloads and flags (PCM identical; the north star allows +-1 LSB)."""
     N, T, cap = 65536, 8, 128
     clip = load_clip()
     sample = [0, 1, 2, 3] + list(range(997, N, 1489))[:44]
@@ -169,28 +154,16 @@ def test_config5_full_batch_with_per_stream_loss_sampled_against_reference(sb):
     other = rng.integers(1, 5, size=(N, T)).astype(np.int32)       # everybody else: arbitrary flags
     mask = np.ones(N, bool); mask[sample] = False
     flags[mask] = other[mask]
-    dev = torch.device("cuda", 0)
     eb, db = sb.EncoderBatch(N), sb.DecoderBatch(N)
-    rdec = {s: ref.RefDecoder("flp") for s in sample}
-    d_bits, d_nb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
-    d_tb, d_tnb = torch.zeros_like(d_bits), torch.zeros_like(d_nb)
-    d_pcm, d_ret = torch.zeros((N, 640), dtype=torch.int16, device=dev), torch.zeros(N, dtype=torch.int32, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
+    dp, rr = DevicePath(sb, eb, db, cap=cap), RefRows(ref, sample, decode="gpu")
     for p in range(T):
-        x = torch.from_numpy(speech_replay(clip, N, 1, first_packet=p)[0]).to(dev)
-        f = torch.from_numpy(flags[:, p].copy()).to(dev)
-        eb.encode_device(x.data_ptr(), d_bits.data_ptr(), cap, d_nb.data_ptr(), st)
-        sb.apply_loss_device(d_bits.data_ptr(), d_nb.data_ptr(), f.data_ptr(), d_tb.data_ptr(), d_tnb.data_ptr(), cap, N, st)
-        db.decode_device(d_pcm.data_ptr(), d_tb.data_ptr(), cap, d_tnb.data_ptr(), f.data_ptr(), d_ret.data_ptr(), st)
-        torch.cuda.synchronize()
-        assert int((d_ret != 0).sum().item()) == 0
-        idx = torch.tensor(sample, device=dev)
-        bits, nb, pcm = d_bits[idx].cpu().numpy(), d_nb[idx].cpu().numpy(), d_pcm[idx].cpu().numpy()
-        for i, s in enumerate(sample):
-            pb, pnb = trim_payload(bytes(bits[i, :nb[i, 0]]), nb[i], int(flags[s, p]))
-            want, r = rdec[s].decode(pb, pnb, int(flags[s, p]))
-            assert r == 0
-            assert np.abs(pcm[i].astype(np.int32) - want.astype(np.int32)).max() <= 0, (p, s, int(flags[s, p]))
+        x = speech_replay(clip, N, 1, first_packet=p)[0]
+        dp.encode(x)
+        dp.decode(flags[:, p])
+        bits, nb, pcm = dp.rows(sample)
+        rr.step(x[sample], bits, nb, flags[sample, p])
+        rr.check_pcm(pcm)
+    rr.close()
     eb.close(); db.close()
 
 
@@ -207,33 +180,23 @@ def test_single_stream_small_output_buffer(sb):
         e.close()
 
 
-def test_20ms_packets_on_device(sb):
+def test_20ms_packets_on_device(sb, ref):
     """framesize_ms = 20 through the batched ABI and the drop-in ABI against the reference (FIX bytes, FLP PCM)."""
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref not built")
     N, T, cap = 130, 40, 128
     clip = load_clip()
     eb, db = sb.EncoderBatch(N, rate=13600, framesize_ms=20), sb.DecoderBatch(N, framesize_ms=20)
     sample = [0, 1, 64, 65, 129]
-    renc = {s: ref.RefEncoder("fix", rate=13600, framesize_ms=20) for s in sample}
-    rdec = {s: ref.RefDecoder("flp", framesize_ms=20) for s in sample}
+    rr = RefRows(ref, sample, decode="gpu", rate=13600, framesize_ms=20)
     off = (np.arange(N) * 7919 * 320) % (len(clip) - 320 * (T + 1))
     flags = np.array([loss_flags(T, 40, seed=3 + s) for s in range(N)], np.int32)
     for p in range(T):
         x = np.stack([clip[o + p * 320:o + (p + 1) * 320] for o in off]).astype(np.int16)
         bits, nb = eb.encode(x, cap=cap)
-        tb, tnb = np.zeros_like(bits), np.zeros_like(nb)
-        for s in range(N):
-            pb, pnb = trim_payload(bytes(bits[s, :nb[s, 0]]), nb[s], flags[s, p])
-            tb[s, :len(pb)] = np.frombuffer(pb, np.uint8); tnb[s] = pnb
-        pcm, ret = db.decode(tb, tnb, flags[:, p].copy())
+        pcm, ret = db.decode(*received(batch_packets(bits, nb), flags[:, p], cap))
         assert pcm.shape == (N, 320) and (ret == 0).all()
-        for s in sample:
-            b, rnb, n = renc[s].encode(x[s])
-            assert tuple(nb[s]) == rnb and bytes(bits[s, :n]) == b, (p, s)
-            want, r = rdec[s].decode(bytes(tb[s, :tnb[s, 0]]), tuple(tnb[s]), int(flags[s, p]))
-            assert np.array_equal(pcm[s], want), (p, s)
+        rr.step(x[sample], bits[sample], nb[sample], flags[sample, p])
+        rr.check_pcm(pcm[sample])
+    rr.close()
     eb.close(); db.close()
     e, d = sb.SoloEncoder(rate=13600, framesize_ms=20), sb.SoloDecoder(framesize_ms=20)
     r0 = ref.RefEncoder("fix", rate=13600, framesize_ms=20)
@@ -266,31 +229,21 @@ def test_example_file_codec_reproduces_the_reference_cli_files(sb, tmp_path):
         assert hashlib.md5(out.read_bytes()).hexdigest() == str(g[key]), key
 
 
-def test_joint_mode1_on_device(sb):
+def test_joint_mode1_on_device(sb, ref):
     """The reference's joint mode 1 through the batched ABI and the drop-in ABI (unsupported modes are refused)."""
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref not built")
     N, T, cap = 67, 20, 192
     x = speech_replay(load_clip(), N, T)
     eb, db = sb.EncoderBatch(N, rate=13600, joint_hb=1), sb.DecoderBatch(N, joint_hb=1)
     sample = [0, 1, 33, 66]
-    renc = {s: ref.RefEncoder("fix", rate=13600, joint_hb=1) for s in sample}
-    rdec = {s: ref.RefDecoder("flp", joint_hb=1) for s in sample}
+    rr = RefRows(ref, sample, decode="gpu", rate=13600, joint_hb=1)
     flags = np.array([loss_flags(T, 40, seed=11 + s) for s in range(N)], np.int32)
     for p in range(T):
         bits, nb = eb.encode(x[p], cap=cap)
-        tb, tnb = np.zeros_like(bits), np.zeros_like(nb)
-        for s in range(N):
-            pb, pnb = trim_payload(bytes(bits[s, :nb[s, 0]]), nb[s], flags[s, p])
-            tb[s, :len(pb)] = np.frombuffer(pb, np.uint8); tnb[s] = pnb
-        pcm, ret = db.decode(tb, tnb, flags[:, p].copy())
+        pcm, ret = db.decode(*received(batch_packets(bits, nb), flags[:, p], cap))
         assert (ret == 0).all()
-        for s in sample:
-            b, rnb, n = renc[s].encode(x[p, s])
-            assert tuple(nb[s]) == rnb and bytes(bits[s, :n]) == b, (p, s)
-            want, r = rdec[s].decode(bytes(tb[s, :tnb[s, 0]]), tuple(tnb[s]), int(flags[s, p]))
-            assert np.array_equal(pcm[s], want), (p, s)
+        rr.step(x[p, sample], bits[sample], nb[sample], flags[sample, p])
+        rr.check_pcm(pcm[sample])
+    rr.close()
     eb.close(); db.close()
     e = sb.SoloEncoder(rate=13600, joint_enable=1, joint_mode=1)
     b, nb2, n = e.encode(x[0, 0])

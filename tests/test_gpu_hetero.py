@@ -4,106 +4,31 @@ two lane groups of a quantiser warp and the 64 threads of an entropy-coding / de
 Every row is compared with the unmodified reference run per stream: payload bytes + length fields against libjc1_fix.so,
 decoded PCM under a per-stream 50 % loss process against libjc1_flp.so fed the same payloads and flags.
 Tolerances: payloads bit-exact; PCM 0 LSB (the north star allows +-1)."""
-from concurrent.futures import ThreadPoolExecutor
-
 import numpy as np
 import pytest
 
-from tests.util import load_clip, loss_flags, speech_replay, trim_payload
+from tests.parity import DevicePath, RefRows, ref, sb  # noqa: F401  (fixtures)
+from tests.util import load_clip, loss_flags, signal_classes, speech_replay
 
 pytestmark = pytest.mark.gpu
-PCM_TOL = 0
 
 
-@pytest.fixture(scope="module")
-def sb():
-    import solo_b200
-    solo_b200.lib()
-    return solo_b200
-
-
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built")
-    return r
-
-
-def signal_classes(clip, n_rows, n_packets, seed=5):
-    """int16 [n_packets, n_rows, 640]; row s belongs to class s % 8:
-    0 speech, 1 noise sigma 2000, 2 noise sigma 20000, 3 zeros, 4 DC 1000, 5 +-32767 square, 6 200 Hz sine, 7 4x clipped speech."""
-    rng = np.random.Generator(np.random.PCG64(seed))
-    L = n_packets * 640
-    t = np.arange(L)
-    out = np.zeros((n_rows, L), np.int16)
-    for s in range(n_rows):
-        k = s % 8
-        off = (s * 7919 * 640) % (len(clip) - 1)
-        sp = np.take(clip, (off + t) % len(clip))
-        if k == 0:
-            out[s] = sp
-        elif k == 1:
-            out[s] = np.clip(rng.normal(0, 2000, L), -32768, 32767).astype(np.int16)
-        elif k == 2:
-            out[s] = np.clip(rng.normal(0, 20000, L), -32768, 32767).astype(np.int16)
-        elif k == 3:
-            out[s] = 0
-        elif k == 4:
-            out[s] = 1000
-        elif k == 5:
-            out[s] = np.where(((t + 13 * s) // 80) % 2 == 0, 32767, -32767).astype(np.int16)
-        elif k == 6:
-            out[s] = (8000 * np.sin(2 * np.pi * 200 * (t + 7 * s) / 16000)).astype(np.int16)
-        else:
-            out[s] = np.clip(sp.astype(np.int32) * 4, -32768, 32767).astype(np.int16)
-    return np.ascontiguousarray(out.reshape(n_rows, n_packets, 640).transpose(1, 0, 2))
-
-
-def run_against_reference(sb, ref, x, rate, loss_perc=50, workers=16):
-    """x: [T, N, 640].  GPU batch vs one reference encoder + decoder per row (driven by a thread pool: the reference is
-    plain C behind ctypes, which releases the GIL)."""
+def run_against_reference(sb, ref, x, rate, loss_perc=50):
+    """x: [T, N, 640].  GPU batch vs one reference encoder + decoder per row; the batch decoder gets what the receiver makes
+    of the reference's payloads."""
     T, N, _ = x.shape
     cap = 1024 if rate > 40000 else 256
     eb, db = sb.EncoderBatch(N, rate=rate), sb.DecoderBatch(N)
-    renc = [ref.RefEncoder("fix", rate=rate) for _ in range(N)]
-    rdec = [ref.RefDecoder("flp") for _ in range(N)]
+    rr = RefRows(ref, range(N), decode="ref", rate=rate)
     flags = np.array([loss_flags(T, loss_perc, seed=1 + s) for s in range(N)], np.int32)
     flags[::5] = 4           # every fifth row loss-free
-
-    def ref_row(args):
-        s, p = args
-        b, rnb, n = renc[s].encode(x[p, s])
-        f = int(flags[s, p])
-        if rnb[0] <= 0:      # DTX packet: nothing is sent, the receiver conceals
-            pb, pnb, f = bytes(16), (16, 8), 1
-        else:
-            pb, pnb = trim_payload(b, rnb, f)
-        y, r = rdec[s].decode(pb, pnb, f)
-        return b, rnb, n, pb, pnb, f, y, r
-
-    with ThreadPoolExecutor(workers) as pool:
-        for p in range(T):
-            bits, nb = eb.encode(x[p], cap=cap)
-            rows = list(pool.map(ref_row, [(s, p) for s in range(N)]))
-            dbits = np.zeros((N, cap), np.uint8)
-            dnb = np.zeros((N, 2), np.int16)
-            f_eff = np.zeros(N, np.int32)
-            want = np.zeros((N, 640), np.int16)
-            for s, (b, rnb, n, pb, pnb, f, y, r) in enumerate(rows):
-                assert tuple(nb[s]) == rnb, ("length fields", p, s, s % 8)
-                assert bytes(bits[s, :max(n, 0)]) == b[:max(n, 0)], ("payload", p, s, s % 8)
-                assert r == 0
-                dbits[s, :len(pb)] = np.frombuffer(pb, np.uint8)
-                dnb[s] = pnb
-                f_eff[s] = f
-                want[s] = y
-            pcm, ret = db.decode(dbits, dnb, f_eff)
-            assert (ret == 0).all()
-            d = np.abs(pcm.astype(np.int32) - want.astype(np.int32)).max(axis=1)
-            assert d.max() <= PCM_TOL, ("pcm", p, int(d.argmax()), int(d.argmax()) % 8, int(d.max()))
-    for o in renc + rdec:
-        o.close()
+    for p in range(T):
+        bits, nb = eb.encode(x[p], cap=cap)
+        tb, tnb, tf = rr.step(x[p], bits, nb, flags[:, p])
+        pcm, ret = db.decode(tb, tnb, tf)
+        assert (ret == 0).all()
+        rr.check_pcm(pcm)
+    rr.close()
     eb.close(); db.close()
 
 
@@ -121,7 +46,6 @@ def test_signal_classes_at_other_rates(sb, ref, rate):
 def test_full_batch_sample_of_1024_streams_25_packets(sb, ref):
     """BASELINE configs 3 + 5 at full size (65 536 streams, per-stream loss process, trimming on the device): 1 024 streams
     spread over the batch x 25 packets against the reference (SURVEY.md 8(d) config 4 wording)."""
-    import torch
     N, T, cap = 65536, 25, 128
     clip = load_clip()
     sample = sorted(set(list(range(0, N, 64))))[:1024]
@@ -132,40 +56,14 @@ def test_full_batch_sample_of_1024_streams_25_packets(sb, ref):
     other = rng.integers(1, 5, size=(N, T)).astype(np.int32)
     mask = np.ones(N, bool); mask[sample] = False
     flags[mask] = other[mask]
-    dev = torch.device("cuda", 0)
     eb, db = sb.EncoderBatch(N), sb.DecoderBatch(N)
-    renc = {s: ref.RefEncoder("fix", rate=13600) for s in sample}
-    rdec = {s: ref.RefDecoder("flp") for s in sample}
-    d_bits, d_nb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
-    d_tb, d_tnb = torch.zeros_like(d_bits), torch.zeros_like(d_nb)
-    d_pcm, d_ret = torch.zeros((N, 640), dtype=torch.int16, device=dev), torch.zeros(N, dtype=torch.int32, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
-    idx = torch.tensor(sample, device=dev)
-
-    def ref_row(args):
-        s, p, xs = args
-        b, rnb, n = renc[s].encode(xs)
-        f = int(flags[s, p])
-        pb, pnb = trim_payload(b, rnb, f)
-        y, r = rdec[s].decode(pb, pnb, f)
-        return b, rnb, n, y, r
-
-    with ThreadPoolExecutor(32) as pool:
-        for p in range(T):
-            xh = speech_replay(clip, N, 1, first_packet=p)[0]
-            x = torch.from_numpy(xh).to(dev)
-            f = torch.from_numpy(flags[:, p].copy()).to(dev)
-            eb.encode_device(x.data_ptr(), d_bits.data_ptr(), cap, d_nb.data_ptr(), st)
-            sb.apply_loss_device(d_bits.data_ptr(), d_nb.data_ptr(), f.data_ptr(), d_tb.data_ptr(), d_tnb.data_ptr(), cap, N, st)
-            db.decode_device(d_pcm.data_ptr(), d_tb.data_ptr(), cap, d_tnb.data_ptr(), f.data_ptr(), d_ret.data_ptr(), st)
-            rows = list(pool.map(ref_row, [(s, p, xh[s]) for s in sample]))
-            torch.cuda.synchronize()
-            assert int((d_ret != 0).sum().item()) == 0
-            bits, nb, pcm = d_bits[idx].cpu().numpy(), d_nb[idx].cpu().numpy(), d_pcm[idx].cpu().numpy()
-            for i, s in enumerate(sample):
-                b, rnb, n, y, r = rows[i]
-                assert r == 0 and tuple(nb[i]) == rnb and bytes(bits[i, :n]) == b, (p, s)
-                assert np.abs(pcm[i].astype(np.int32) - y.astype(np.int32)).max() <= PCM_TOL, (p, s, int(flags[s, p]))
-    for o in list(renc.values()) + list(rdec.values()):
-        o.close()
+    dp, rr = DevicePath(sb, eb, db, cap=cap), RefRows(ref, sample, decode="ref", rate=13600)
+    for p in range(T):
+        xh = speech_replay(clip, N, 1, first_packet=p)[0]
+        dp.encode(xh)
+        dp.decode(flags[:, p])
+        bits, nb, pcm = dp.rows(sample)
+        rr.step(xh[sample], bits, nb, flags[sample, p])
+        rr.check_pcm(pcm)
+    rr.close()
     eb.close(); db.close()

@@ -3,48 +3,20 @@
 Bar: encoder payloads + length fields byte-identical to the reference FIX build; decoded PCM identical (tolerance
 stated by the north star is +-1 LSB; we require 0) to the reference FLP build."""
 import hashlib
-import struct
 
 import numpy as np
 import pytest
 
-from tests.util import load_clip, load_golden, loss_flags, speech_replay, synth_inputs, trim_payload
+from tests.parity import PCM_TOL, RefRows, ref, sb  # noqa: F401  (fixtures)
+from tests.util import bitfile, encode_signal, load_clip, load_golden, loss_flags, speech_replay, synth_inputs, trim_payload
 
 pytestmark = pytest.mark.gpu
-
-PCM_TOL = 0  # LSB; north star allows 1
-
-
-@pytest.fixture(scope="module")
-def sb():
-    import solo_b200
-    solo_b200.lib()
-    return solo_b200
-
-
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built")
-    return r
-
-
-def bitfile(pk):
-    return b"".join(struct.pack("<hh", *nb) + (b if nb[0] else b"") for b, nb, n in pk)
-
-
-def encode_single(sb, pcm, **kw):
-    e = sb.SoloEncoder(**kw)
-    pk = [e.encode(pcm[i * 640:(i + 1) * 640]) for i in range(len(pcm) // 640)]
-    e.close()
-    return pk
 
 
 def test_single_stream_golden_bitstream(sb):
     """Config 1/2 plumbing: the six-function ABI reproduces the reference FIX bit file of the shipped clip."""
     g = load_golden()
-    pk = encode_single(sb, load_clip(), rate=13600)
+    pk = encode_signal(sb.SoloEncoder(rate=13600), load_clip())
     assert hashlib.md5(bitfile(pk)).hexdigest() == str(g["fix_bitfile_md5"])
     for i, (b, nb, n) in enumerate(pk):
         assert n == len(b) == g["fix_nbytes"][i, 0]
@@ -74,10 +46,7 @@ def test_single_stream_golden_decode(sb, mode):
 def test_synthetic_inputs_golden(sb):
     g = load_golden()
     for name, x, kw in synth_inputs(load_clip()):
-        kw2 = dict(kw)
-        if "mdi" in kw2:
-            kw2["use_md_index"] = kw2.pop("mdi")
-        pk = encode_single(sb, x, **kw2)
+        pk = encode_signal(sb.SoloEncoder(**kw), x)
         assert hashlib.md5(bitfile(pk)).hexdigest() == str(g["synth_" + name]), name
 
 
@@ -86,44 +55,30 @@ def test_batch_encode_matches_reference(sb, ref):
     length fields equal to libjc1_fix.so run per stream."""
     N, T, cap = 256, 12, 256
     x = speech_replay(load_clip(), N, T)
-    eb = sb.EncoderBatch(N, rate=13600)
-    refs = [ref.RefEncoder("fix", rate=13600) for _ in range(N)]
+    eb, rr = sb.EncoderBatch(N, rate=13600), RefRows(ref, range(N), rate=13600)
     for p in range(T):
         bits, nb = eb.encode(x[p], cap=cap)
-        for s in range(N):
-            b, rnb, n = refs[s].encode(x[p, s])
-            assert tuple(nb[s]) == rnb, (p, s)
-            assert bytes(bits[s, :n]) == b, (p, s)
+        rr.step(x[p], bits, nb)
+    rr.close()
     eb.close()
 
 
 def test_batch_roundtrip_with_loss_matches_reference(sb, ref):
-    """Config 3 + 5 (reduced): encode -> decode with a per-stream loss process (seed 1 + stream id, 50 %), PCM against
-    libjc1_flp.so driven with identical flags."""
+    """Config 3 + 5 (reduced): encode -> decode with a per-stream loss process (seed 1 + stream id, 50 %), payloads against
+    libjc1_fix.so and PCM against libjc1_flp.so driven with identical payloads and flags."""
     N, T, cap = 96, 14, 256
     x = speech_replay(load_clip(), N, T)
-    eb = sb.EncoderBatch(N)
-    db = sb.DecoderBatch(N)
-    rdec = [ref.RefDecoder("flp") for _ in range(N)]
+    eb, db = sb.EncoderBatch(N), sb.DecoderBatch(N)
+    rr = RefRows(ref, range(N), decode="gpu")
     flags = np.array([loss_flags(T, 50, seed=1 + s) for s in range(N)], np.int32)  # [N, T]
     flags[:N // 4] = 4  # a quarter of the streams loss-free
     for p in range(T):
         bits, nb = eb.encode(x[p], cap=cap)
-        dbits = np.zeros((N, cap), np.uint8)
-        dnb = np.zeros((N, 2), np.int16)
-        want = np.zeros((N, 640), np.int16)
-        for s in range(N):
-            b = bytes(bits[s, :nb[s, 0]])
-            pb, pnb = trim_payload(b, nb[s], flags[s, p])
-            dbits[s, :len(pb)] = np.frombuffer(pb, np.uint8)
-            dnb[s] = pnb
-            want[s], r = rdec[s].decode(pb, pnb, flags[s, p])
-            assert r == 0
-        pcm, ret = db.decode(dbits, dnb, flags[:, p].copy())
+        pcm, ret = db.decode(*rr.step(x[p], bits, nb, flags[:, p]))
         assert (ret == 0).all()
-        assert np.abs(pcm.astype(np.int32) - want.astype(np.int32)).max() <= PCM_TOL, p
-    eb.close()
-    db.close()
+        rr.check_pcm(pcm)
+    rr.close()
+    eb.close(); db.close()
 
 
 def test_full_size_properties(sb):

@@ -10,37 +10,17 @@ packet drivers (sb_coop.cuh, sb_nsq_warp.cuh) on 32 emulated lanes in the last t
 Bar: payloads and length fields byte-identical to the FIX build, PCM identical to the FLP build (north star allows
 +-1 LSB)."""
 import hashlib
-import struct
 
 import numpy as np
 import pytest
 
-from tests.util import load_clip, load_golden, loss_flags, speech_replay, synth_inputs, trim_payload
-
-PCM_TOL = 0
-
-
-@pytest.fixture(scope="module")
-def sim():
-    from tests.hostsim import sim as s
-    s.lib()
-    return s
-
-
-def bitfile(pk):
-    return b"".join(struct.pack("<hh", *nb) + (b if nb[0] else b"") for b, nb, n in pk)
-
-
-def encode(mod_enc, pcm, **kw):
-    e = mod_enc(**kw)
-    pk = [e.encode(pcm[i * 640:(i + 1) * 640]) for i in range(len(pcm) // 640)]
-    e.close()
-    return pk
+from tests.parity import PCM_TOL, lockstep, ref, ref_and_model, sim  # noqa: F401  (fixtures)
+from tests.util import bitfile, encode_signal, load_clip, load_golden, loss_flags, speech_replay, synth_inputs, trim_payload
 
 
 def test_encoder_matches_golden_bitstream(sim):
     g = load_golden()
-    pk = encode(sim.SimEncoder, load_clip(), rate=13600)
+    pk = encode_signal(sim.SimEncoder(rate=13600), load_clip())
     assert hashlib.md5(bitfile(pk)).hexdigest() == str(g["fix_bitfile_md5"])
     for i, (b, nb, n) in enumerate(pk):
         assert nb == tuple(g["fix_nbytes"][i]) and n == nb[0]
@@ -70,10 +50,7 @@ def test_encoder_matches_synthetic_hashes(sim):
     """Other rates, scaled / clipped speech, noise, silence, DC, full-scale square, sine, DTX, MD index flag."""
     g = load_golden()
     for name, x, kw in synth_inputs(load_clip()):
-        kw = dict(kw)
-        if "mdi" in kw:
-            kw["use_md_index"] = kw.pop("mdi")
-        assert hashlib.md5(bitfile(encode(sim.SimEncoder, x, **kw))).hexdigest() == str(g["synth_" + name]), name
+        assert hashlib.md5(bitfile(encode_signal(sim.SimEncoder(**kw), x))).hexdigest() == str(g["synth_" + name]), name
 
 
 def test_empty_and_error_inputs(sim):
@@ -89,34 +66,13 @@ def test_empty_and_error_inputs(sim):
     d.close()
 
 
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built")
-    return r
-
-
 def test_speech_replay_streams_match_reference(sim, ref):
     """SURVEY.md 8(d) batch (i), 12 streams x 30 packets, each stream with its own loss pattern (seed 1 + s, 50 %):
     encoder bytes vs FIX, decoder PCM vs FLP fed the same payloads and flags."""
     S, P = 12, 30
     x = speech_replay(load_clip(), S, P)
     for s in range(S):
-        e_ref, e_sim = ref.RefEncoder("fix", rate=13600), sim.SimEncoder(rate=13600)
-        d_ref, d_sim = ref.RefDecoder("flp"), sim.SimDecoder()
-        flags = loss_flags(P, 50, seed=1 + s)
-        for p in range(P):
-            b0, nb0, n0 = e_ref.encode(x[p, s])
-            b1, nb1, n1 = e_sim.encode(x[p, s])
-            assert (b0[:n0], nb0, n0) == (b1[:n1], nb1, n1), (s, p)
-            pb, pnb = trim_payload(b0, nb0, flags[p])
-            y0, r0 = d_ref.decode(pb, pnb, flags[p])
-            y1, r1 = d_sim.decode(pb, pnb, flags[p])
-            assert r0 == r1 == 0
-            assert np.abs(y0.astype(np.int32) - y1.astype(np.int32)).max() <= PCM_TOL, (s, p, flags[p])
-        for o in (e_ref, e_sim, d_ref, d_sim):
-            o.close()
+        lockstep(*ref_and_model(ref, sim, rate=13600), x[:, s], loss_flags(P, 50, seed=1 + s), tag=(s,))
 
 
 def test_random_rates_and_signals_match_reference(sim, ref):
@@ -131,19 +87,7 @@ def test_random_rates_and_signals_match_reference(sim, ref):
                 (6000 * np.sin(2 * np.pi * (80 + 3e-3 * t) * t / 16000)).astype(np.int16),
                 np.clip(rng.normal(0, 500, 640 * 25), -32768, 32767).astype(np.int16)]
         for x in sigs:
-            a = encode(lambda **kw: ref.RefEncoder("fix", **kw), x, rate=rate, dtx=dtx, use_md_index=mdi)
-            b = encode(sim.SimEncoder, x, rate=rate, dtx=dtx, use_md_index=mdi)
-            assert [(p[0][:max(p[2], 0)], p[1], p[2]) for p in a] == [(p[0][:max(p[2], 0)], p[1], p[2]) for p in b], (rate, mdi, dtx)
-            d0, d1 = ref.RefDecoder("flp", use_md_index=mdi), sim.SimDecoder(use_md_index=mdi)
-            for (pb, nb, n) in a:
-                if nb[0] <= 0:        # DTX: nothing was sent, the receiver conceals
-                    y0, _ = d0.decode(bytes(16), (16, 8), 1)
-                    y1, _ = d1.decode(bytes(16), (16, 8), 1)
-                else:
-                    y0, _ = d0.decode(pb[:n], nb, 4)
-                    y1, _ = d1.decode(pb[:n], nb, 4)
-                assert np.abs(y0.astype(np.int32) - y1.astype(np.int32)).max() <= PCM_TOL
-            d0.close(); d1.close()
+            lockstep(*ref_and_model(ref, sim, rate=rate, dtx=dtx, use_md_index=mdi), x.reshape(25, 640), [4] * 25, tag=(rate, mdi, dtx))
 
 
 def test_small_output_buffer_matches_reference(sim, ref):
@@ -171,26 +115,9 @@ def test_20ms_packets_match_reference(sim, ref):
     bytes, AGR_BWE_SDK_API.c:78-81,106-110): payloads vs FIX, PCM vs FLP, with loss, DTX and the MD index flag."""
     clip = load_clip()
     for rate, dtx, mdi in ((13600, 0, 0), (8000, 0, 1), (24000, 1, 0)):
-        e0 = ref.RefEncoder("fix", rate=rate, dtx=dtx, use_md_index=mdi, framesize_ms=20)
-        e1 = sim.SimEncoder(rate=rate, dtx=dtx, use_md_index=mdi, framesize_ms=20)
-        d0, d1 = ref.RefDecoder("flp", use_md_index=mdi, framesize_ms=20), sim.SimDecoder(use_md_index=mdi, framesize_ms=20)
-        flags = loss_flags(240, 30, seed=5)
-        for p in range(240):
-            x = clip[p * 320:(p + 1) * 320]
-            b0, nb0, n0 = e0.encode(x)
-            b1, nb1, n1 = e1.encode(x)
-            assert (b0[:max(n0, 0)], nb0, n0) == (b1[:max(n1, 0)], nb1, n1), (rate, p)
-            if nb0[0] > 0:
-                assert nb0[1] >= 4 and n0 == nb0[0]
-                pb, pnb, f = trim_payload(b0, nb0, flags[p]) + (flags[p],)
-            else:                                   # DTX: nothing was sent
-                pb, pnb, f = bytes(16), (16, 8), 1
-            y0, r0 = d0.decode(pb, pnb, f)
-            y1, r1 = d1.decode(pb, pnb, f)
-            assert r0 == r1 == 0 and y0.size == y1.size == 320
-            assert np.abs(y0.astype(np.int32) - y1.astype(np.int32)).max() <= PCM_TOL, (rate, p, f)
-        for o in (e0, e1, d0, d1):
-            o.close()
+        pk = lockstep(*ref_and_model(ref, sim, rate=rate, dtx=dtx, use_md_index=mdi, framesize_ms=20), clip[:320 * 240].reshape(240, 320),
+                      loss_flags(240, 30, seed=5), tag=(rate,))
+        assert all(nb[1] >= 4 and n == nb[0] for _, nb, n in pk if nb[0] > 0), rate
 
 
 def test_joint_mode1_matches_reference(sim, ref):
@@ -198,25 +125,8 @@ def test_joint_mode1_matches_reference(sim, ref):
     sub-frames) per packet, core rate = target - 800."""
     clip = load_clip()
     for rate, dtx, mdi in ((13600, 0, 0), (8000, 0, 1), (24000, 1, 0)):
-        e0 = ref.RefEncoder("fix", rate=rate, dtx=dtx, use_md_index=mdi, joint_hb=1)
-        e1 = sim.SimEncoder(rate=rate, dtx=dtx, use_md_index=mdi, joint_hb=1)
-        d0, d1 = ref.RefDecoder("flp", use_md_index=mdi, joint_hb=1), sim.SimDecoder(use_md_index=mdi, joint_hb=1)
-        flags = loss_flags(120, 30, seed=9)
-        for p in range(120):
-            x = clip[p * 640:(p + 1) * 640]
-            b0, nb0, n0 = e0.encode(x)
-            b1, nb1, n1 = e1.encode(x)
-            assert (b0[:max(n0, 0)], nb0, n0) == (b1[:max(n1, 0)], nb1, n1), (rate, p)
-            if nb0[0] > 0:
-                pb, pnb, f = trim_payload(b0, nb0, flags[p]) + (flags[p],)
-            else:
-                pb, pnb, f = bytes(16), (16, 8), 1
-            y0, r0 = d0.decode(pb, pnb, f)
-            y1, r1 = d1.decode(pb, pnb, f)
-            assert r0 == r1 == 0
-            assert np.abs(y0.astype(np.int32) - y1.astype(np.int32)).max() <= PCM_TOL, (rate, p, f)
-        for o in (e0, e1, d0, d1):
-            o.close()
+        lockstep(*ref_and_model(ref, sim, rate=rate, dtx=dtx, use_md_index=mdi, joint_hb=1), clip[:640 * 120].reshape(120, 640),
+                 loss_flags(120, 30, seed=9), tag=(rate,))
 
 
 def test_long_run_with_level_changes_dtx_and_loss_bursts(sim, ref):
@@ -226,33 +136,17 @@ def test_long_run_with_level_changes_dtx_and_loss_bursts(sim, ref):
     clip = load_clip()
     rng = np.random.Generator(np.random.PCG64(5))
     for rate, dtx, mdi, fs, j in ((13600, 1, 0, 40, 0), (9000, 0, 1, 20, 0), (20000, 1, 0, 40, 1)):
-        spp = 16 * fs
-        kw = dict(rate=rate, dtx=dtx, use_md_index=mdi, framesize_ms=fs, joint_hb=j)
-        e0, e1 = ref.RefEncoder("fix", **kw), sim.SimEncoder(**kw)
-        d0 = ref.RefDecoder("flp", use_md_index=mdi, framesize_ms=fs, joint_hb=j)
-        d1 = sim.SimDecoder(use_md_index=mdi, framesize_ms=fs, joint_hb=j)
-        P = 1000
-        flags = loss_flags(P, 25, seed=77)
+        spp, P = 16 * fs, 1000
+        x, flags = np.zeros((P, spp), np.int16), loss_flags(P, 25, seed=77)
         pos, gain = 0, 1.0
         for p in range(P):
             if p % 97 == 0:
                 gain = [1.0, 0.5, 0.1, 2.5, 0.0][int(rng.integers(0, 5))]
-            seg = clip[pos:pos + spp]
+            x[p] = np.clip(clip[pos:pos + spp].astype(np.float64) * gain, -32768, 32767).astype(np.int16)
             pos = (pos + spp) % (len(clip) - spp)
-            x = np.clip(seg.astype(np.float64) * gain, -32768, 32767).astype(np.int16)
-            b0, nb0, n0 = e0.encode(x)
-            b1, nb1, n1 = e1.encode(x)
-            assert (b0[:max(n0, 0)], nb0, n0) == (b1[:max(n1, 0)], nb1, n1), (rate, p)
-            f = flags[p] if (p // 200) % 2 == 0 else (1 if rng.random() < 0.6 else 4)
-            if nb0[0] <= 0:
-                pb, pnb, f = bytes(16), (16, 8), 1
-            else:
-                pb, pnb = trim_payload(b0, nb0, f)
-            y0, r0 = d0.decode(pb, pnb, f)
-            y1, r1 = d1.decode(pb, pnb, f)
-            assert r0 == r1 == 0 and np.abs(y0.astype(np.int32) - y1.astype(np.int32)).max() <= PCM_TOL, (rate, p, f)
-        for o in (e0, e1, d0, d1):
-            o.close()
+            if (p // 200) % 2:                      # every other 200 packets: bursts of loss
+                flags[p] = 1 if rng.random() < 0.6 else 4
+        lockstep(*ref_and_model(ref, sim, rate=rate, dtx=dtx, use_md_index=mdi, framesize_ms=fs, joint_hb=j), x, flags, tag=(rate,))
 
 
 def test_cooperative_analysis_under_32_lane_emulation(sim):
@@ -267,12 +161,9 @@ def test_cooperative_analysis_under_32_lane_emulation(sim):
         b, nb, n = e.encode(clip[p * 640:(p + 1) * 640])
         assert nb == tuple(g["fix_nbytes"][p]) and b[:n] == bytes(g["fix_bits"][p, :n]), p
     e.close()
-    cases = [(name, x, dict(kw)) for name, x, kw in synth_inputs(clip)]
-    cases += [("20ms", clip[:320 * 80], dict(framesize_ms=20)), ("joint1", clip[:640 * 60], dict(joint_hb=1)),
-              ("20ms_rate8000", clip[:320 * 60], dict(framesize_ms=20, rate=8000))]
+    cases = synth_inputs(clip) + [("20ms", clip[:320 * 80], dict(framesize_ms=20)), ("joint1", clip[:640 * 60], dict(joint_hb=1)),
+                                  ("20ms_rate8000", clip[:320 * 60], dict(framesize_ms=20, rate=8000))]
     for name, x, kw in cases:
-        if "mdi" in kw:
-            kw["use_md_index"] = kw.pop("mdi")
         e0, e1 = sim.SimEncoder(emu=False, **kw), sim.SimEncoder(emu=True, **kw)
         spp = e0.samples
         for p in range(min(len(x) // spp, 50)):
@@ -294,11 +185,9 @@ def test_quantiser_kernel_code_under_32_lane_emulation(sim):
         b, nb, n = e.encode(clip[p * 640:(p + 1) * 640])
         assert nb == tuple(g["fix_nbytes"][p]) and b[:n] == bytes(g["fix_bits"][p, :n]), p
     e.close()
-    cases = [(name, x, dict(kw)) for name, x, kw in synth_inputs(clip) if name not in ("rate15600", "rate_default", "shift2", "dtx")]
+    cases = [c for c in synth_inputs(clip) if c[0] not in ("rate15600", "rate_default", "shift2", "dtx")]
     cases += [("20ms", clip[320 * 30:], dict(framesize_ms=20)), ("joint1", clip[640 * 15:], dict(joint_hb=1))]
     for name, x, kw in cases:
-        if "mdi" in kw:
-            kw["use_md_index"] = kw.pop("mdi")
         e0, e1 = sim.SimEncoder(emu=False, **kw), sim.SimEncoder(emu=True, emu_nsq=True, **kw)
         spp = e0.samples
         first = 12 if name.startswith("rate") or name in ("clip4x", "mdi") else 0     # start inside the speech

@@ -4,36 +4,17 @@ libraries, and the md5 values recorded in SURVEY.md 7.2 for the reference CLI ag
 oracle ever disagree (different compiler, different flags) every other parity statement is void, so check it first.
 Skipped where oracle/_ref is not built (it needs /root/reference; the GPU box receives the prebuilt libraries)."""
 import hashlib
-import struct
 
 import numpy as np
 import pytest
 
-from tests.util import load_clip, load_golden, synth_inputs, trim_payload
-
-
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import ref as r
-    if not r.available():
-        pytest.skip("oracle/_ref not built (run `make -C oracle` where /root/reference exists)")
-    return r
-
-
-def bitfile(pk):
-    return b"".join(struct.pack("<hh", *nb) + (b if nb[0] else b"") for b, nb, n in pk)
-
-
-def encode(ref, pcm, **kw):
-    e = ref.RefEncoder("fix", **kw)
-    pk = [e.encode(pcm[i * 640:(i + 1) * 640]) for i in range(len(pcm) // 640)]
-    e.close()
-    return pk
+from tests.parity import ref  # noqa: F401  (fixture)
+from tests.util import bitfile, encode_signal, load_clip, load_golden, synth_inputs, trim_payload
 
 
 @pytest.fixture(scope="module")
 def clip_packets(ref):
-    return encode(ref, load_clip(), rate=13600)
+    return encode_signal(ref.RefEncoder("fix", rate=13600), load_clip())
 
 
 def test_fix_encoder_reproduces_golden_bitstream(clip_packets):
@@ -66,10 +47,7 @@ def test_flp_decoder_reproduces_golden_pcm(ref, clip_packets, mode):
 def test_fix_encoder_reproduces_synthetic_hashes(ref):
     g = load_golden()
     for name, x, kw in synth_inputs(load_clip()):
-        kw = dict(kw)
-        if "mdi" in kw:
-            kw["use_md_index"] = kw.pop("mdi")
-        assert hashlib.md5(bitfile(encode(ref, x, **kw))).hexdigest() == str(g["synth_" + name]), name
+        assert hashlib.md5(bitfile(encode_signal(ref.RefEncoder("fix", **kw), x))).hexdigest() == str(g["synth_" + name]), name
 
 
 def test_loss_process_matches_fixture():
@@ -85,10 +63,7 @@ def test_flp_encoder_leg_of_config0(ref):
     bitstream target is the FIX encoder, but the oracle build is pinned on this leg too: the FLP encoder's .bit file has the
     md5 SURVEY.md 7.2 recorded for the reference CLI (it moves under FMA contraction, which is why oracle/Makefile builds with
     -ffp-contract=off), and the FLP decoder decodes it without error."""
-    clip = load_clip()
-    e = ref.RefEncoder("flp", rate=13600)
-    pk = [e.encode(clip[i * 640:(i + 1) * 640]) for i in range(len(clip) // 640)]
-    e.close()
+    pk = encode_signal(ref.RefEncoder("flp", rate=13600), load_clip())
     bf = bitfile(pk)
     assert len(bf) == 16545 and hashlib.md5(bf).hexdigest() == "26da320f33e8d8f9f0043df37765533c"
     d = ref.RefDecoder("flp")

@@ -1,5 +1,6 @@
-"""Shared helpers of the test-suite (input synthesis, the reference driver's loss process, payload trimming)."""
+"""Shared helpers of the test-suite (input synthesis, the reference driver's loss process, what the receiver decodes)."""
 import os
+import struct
 
 import numpy as np
 
@@ -50,6 +51,27 @@ def trim_payload(b, nb, flag):
     return b[:n0], (n0, n1)
 
 
+def receive(bits, nb, flag):
+    """(payload, nbytes, lostflag) the receiver hands to the decoder for one encoded packet: a DTX packet (nb[0] <= 0,
+    nothing was sent) is concealed as a lost one, any other packet is trimmed for its lostflag."""
+    if nb[0] <= 0:
+        return bytes(16), (16, 8), 1
+    return trim_payload(bits, nb, flag) + (int(flag),)
+
+
+def bitfile(pk):
+    """The reference CLI's .bit file of a list of (payload, (n0, n1), n) packets."""
+    return b"".join(struct.pack("<hh", *nb) + (b if nb[0] else b"") for b, nb, n in pk)
+
+
+def encode_signal(enc, pcm):
+    """The packets of a whole signal through one encoder (enc.samples per packet); closes the encoder."""
+    k = enc.samples
+    pk = [enc.encode(pcm[i * k:(i + 1) * k]) for i in range(len(pcm) // k)]
+    enc.close()
+    return pk
+
+
 def speech_replay(clip, n_streams, n_packets, first_packet=0):
     """SURVEY.md 8(d) synthetic batch (i): stream s reads the clip circularly from sample offset
     (s*7919*640) mod len(clip), scaled by 2^-(s mod 4).  Returns int16 [n_packets, n_streams, 640]."""
@@ -84,6 +106,82 @@ def synth_inputs(clip):
         ("square100", np.where((t // 80) % 2 == 0, 32767, -32767).astype(np.int16), {}),
         ("sine200", (8000 * np.sin(2 * np.pi * 200 * t / 16000)).astype(np.int16), {}),
         ("dtx", np.concatenate([clip[:640 * 60], np.zeros(640 * 60, np.int16), clip[:640 * 40]]), dict(dtx=1)),
-        ("mdi", clip[:640 * 80], dict(mdi=1)),
+        ("mdi", clip[:640 * 80], dict(use_md_index=1)),
     ]
     return cases
+
+
+def signal_classes(clip, n_rows, n_packets, seed=5):
+    """int16 [n_packets, n_rows, 640]; row s belongs to class s % 8:
+    0 speech, 1 noise sigma 2000, 2 noise sigma 20000, 3 zeros, 4 DC 1000, 5 +-32767 square, 6 200 Hz sine, 7 4x clipped speech."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    L = n_packets * 640
+    t = np.arange(L)
+    out = np.zeros((n_rows, L), np.int16)
+    for s in range(n_rows):
+        k = s % 8
+        off = (s * 7919 * 640) % (len(clip) - 1)
+        sp = np.take(clip, (off + t) % len(clip))
+        if k == 0:
+            out[s] = sp
+        elif k == 1:
+            out[s] = np.clip(rng.normal(0, 2000, L), -32768, 32767).astype(np.int16)
+        elif k == 2:
+            out[s] = np.clip(rng.normal(0, 20000, L), -32768, 32767).astype(np.int16)
+        elif k == 3:
+            out[s] = 0
+        elif k == 4:
+            out[s] = 1000
+        elif k == 5:
+            out[s] = np.where(((t + 13 * s) // 80) % 2 == 0, 32767, -32767).astype(np.int16)
+        elif k == 6:
+            out[s] = (8000 * np.sin(2 * np.pi * 200 * (t + 7 * s) / 16000)).astype(np.int16)
+        else:
+            out[s] = np.clip(sp.astype(np.int32) * 4, -32768, 32767).astype(np.int16)
+    return np.ascontiguousarray(out.reshape(n_rows, n_packets, 640).transpose(1, 0, 2))
+
+
+def near_silent_classes(clip, n_rows, n_packets, samples=640, seed=9):
+    """int16 [n_packets, n_rows, samples]; row s belongs to class s % 8:
+    0 speech, 1-3 white noise sigma 1, 3, 8, 4 DC +1 / -1 (alternating between rows of the class), 5 isolated one-sample
+    clicks in zeros, 6 speech at 2^-10, 7 speech fading into silence and back out (period 30 packets)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    L = n_packets * samples
+    t = np.arange(L)
+    out = np.zeros((n_rows, L), np.int16)
+    for s in range(n_rows):
+        k = s % 8
+        off = (s * 7919 * 640) % (len(clip) - 1)
+        sp = np.take(clip, (off + t) % len(clip)).astype(np.float64)
+        if k == 0:
+            v = sp
+        elif k in (1, 2, 3):
+            v = rng.normal(0, (1, 3, 8)[k - 1], L)
+        elif k == 4:
+            v = np.full(L, 1 if (s // 8) % 2 == 0 else -1)
+        elif k == 5:
+            v = np.zeros(L)
+            pos = np.cumsum(rng.integers(200, 3000, L // 200 + 1))
+            pos = pos[pos < L]
+            v[pos] = rng.choice([-1, 1], pos.size) * rng.integers(1, 2000, pos.size)
+        elif k == 6:
+            v = sp / 1024.0
+        else:
+            ph = (t % (30 * samples)) / (30.0 * samples)
+            env = np.clip(np.abs(2.0 * ph - 1.0) * 3.0 - 1.0, 0.0, 1.0)     # loud - fade - silent - fade - loud
+            v = sp * env
+        out[s] = np.clip(np.round(v), -32768, 32767).astype(np.int16)
+    return np.ascontiguousarray(out.reshape(n_rows, n_packets, samples).transpose(1, 0, 2))
+
+
+def loss_with_bursts(T, n_rows, seed=3):
+    """Per-stream lostflags: the reference driver's 20 % process, one burst of 10-14 lost packets per stream at a random
+    place, every fifth row loss-free."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    flags = np.array([loss_flags(T, 20, seed=1 + s) for s in range(n_rows)], np.int32)
+    for s in range(n_rows):
+        n = int(rng.integers(10, 15))
+        a = int(rng.integers(1, T - n))
+        flags[s, a:a + n] = 1
+    flags[::5] = 4
+    return flags
