@@ -32,8 +32,10 @@ namespace sb {
 // Row paddings keep the three quantisers' rows in different shared-memory banks (the 12 lanes address
 // [qz][same index][state]); the pad words are never read.
 // The long buffers (sLTP_Q16, sLTP_shp_Q10 here, xq in NsqState) are 160-entry rings: logical index j of the reference's
-// 2*frame_length arrays (old frame [0,160), frame being written [160,320)) lives at j mod 160.  Nothing older than
-// lag + 2 <= 146 samples behind the write position is ever read, so the ring holds exactly the persistent state on entry and on exit.
+// 2*frame_length arrays (old frame [0,160), frame being written [160,320)) lives at j mod 160.  Pitch lags run from 15 to
+// 146 (lag 16..144 plus a contour offset of -1..+2), and nothing older than lag + 2 <= 148 samples behind the write position
+// is ever read (the rewhitening starts at FRAME - lag - LPC_ORDER - LTP_ORDER / 2 >= 2), so the ring holds exactly the
+// persistent state on entry and on exit.
 struct NsqSmem {
     i32 sLTP_Q16[3][FRAME + 1];
     i32 sLTP_shp_Q10[3][FRAME + 2];

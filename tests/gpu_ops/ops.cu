@@ -2,12 +2,18 @@
 // (sb_common.cuh), compiled for sm_90a exactly as sb_analysis.cu compiles them, one warp per case.  Each kernel reads its
 // case from global memory, stages the routine's scratch struct and arrays in shared memory as the analysis kernel does,
 // calls the routine and writes every output back.  tests/test_gpu_ops.py compares the results with the reference.
+// The quantiser kernel's device code runs here too, whole packets in the production kernel's layout (sb_ops_nsq,
+// tests/test_gpu_nsq.py).
 // Every launcher takes host arrays, copies them to the device and back, and returns a CUDA error code (0 = success).
 #define SB_COOP 1
 #define SB_DIV_OUTLINE 1
 #define SB_BLOCK_STREAMS 8
 #include <cuda_runtime.h>
+#include <string.h>
+#include <vector>
 #include "sb_coop.cuh"
+#include "sb_nsq_warp.cuh"
+#include "../../oracle/nsq_io.h"
 
 using namespace sb;
 
@@ -217,6 +223,18 @@ __global__ void __launch_bounds__(SB_BLOCK_STREAMS * 32) msvq_kernel(const MsvqC
     if (live && lane < LPC_ORDER) nlsf_out[s * LPC_ORDER + lane] = Q->NLSF_Q15[lane];
 }
 
+// ---- the quantiser kernel's device code (nsq_packet_warp) in sb_enc_nsq_kernel's layout: one-warp blocks, a stream per
+//      16-lane group, a group without a case of its own shadowing the last one, the same dynamic shared memory and bounds ----
+constexpr int kNsqSpb = 32 / SB_NSQ_GW;
+__global__ void __launch_bounds__(32, 12) nsq_kernel(NsqState* ns, EncScratch* scratch, int nf, int n) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int g = threadIdx.x / SB_NSQ_GW;
+    NsqSmem* S = reinterpret_cast<NsqSmem*>(smem_raw) + g;
+    int s = blockIdx.x * kNsqSpb + g;
+    if (s >= n) s = n - 1;
+    nsq_packet_warp(*S, &ns[3 * s], &scratch[s], nf);
+}
+
 template <class T> struct Dev {
     T* p = nullptr;
     size_t n = 0;
@@ -347,4 +365,50 @@ extern "C" int sb_ops_msvq(const int32_t* cases, const int32_t* nlsf, const int3
     SB_CHECK(finish());
     SB_CHECK(di.back(idx));
     return (int)dq.back(nlsf_q);
+}
+
+extern "C" void nsq_io_sizes(int* s) { NSQ_IO_SIZES(s); }
+
+// n cases of npk packets of nf frames (oracle/nsq_io.h): st0 [n][3], fr [n][npk * nf] -> out [n][npk * nf] after every
+// frame, st_after [n][npk][3] after every packet.  One launch per packet; the states stay on the device between packets and
+// the scratch outputs (pulses, centre excitation, random-generator history) are poisoned with 0xA5 before every launch.
+extern "C" int sb_ops_nsq(int n, int npk, int nf, const NsqStateIO* st0, const NsqFrameIn* fr, NsqFrameOut* out, NsqStateIO* st_after) {
+    if (n <= 0 || npk <= 0 || (nf != 1 && nf != 2)) return -1;
+    const int nfr = npk * nf;
+    const int smem = kNsqSpb * (int)sizeof(NsqSmem);
+    SB_CHECK(cudaFuncSetAttribute(nsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    std::vector<NsqState> ns((size_t)n * 3);
+    std::vector<EncScratch> scr(n);
+    for (int i = 0; i < n * 3; i++) nsqio_state_to(&ns[i], &st0[i]);
+    Dev<NsqState> dns(ns.data(), ns.size());
+    Dev<EncScratch> dscr(nullptr, scr.size());
+    SB_CHECK(dns.err); SB_CHECK(dscr.err);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) {
+            memset(&scr[s], 0, sizeof(EncScratch));
+            memset(scr[s].q_md, 0xA5, sizeof(scr[s].q_md));
+            memset(scr[s].r16, 0xA5, sizeof(scr[s].r16));
+            memset(scr[s].nsq_rand, 0xA5, sizeof(scr[s].nsq_rand));
+            for (int f = 0; f < nf; f++) {
+                const NsqFrameIn* x = &fr[(size_t)s * nfr + p * nf + f];
+                nsqio_ctrl(&scr[s].c[f], x);
+                memcpy(scr[s].xfw[f], x->x, sizeof(scr[s].xfw[f]));
+            }
+        }
+        SB_CHECK(cudaMemcpy(dscr.p, scr.data(), sizeof(EncScratch) * scr.size(), cudaMemcpyHostToDevice));
+        nsq_kernel<<<(n + kNsqSpb - 1) / kNsqSpb, 32, smem>>>(dns.p, dscr.p, nf, n);
+        SB_CHECK(finish());
+        SB_CHECK(dscr.back(scr.data()));
+        SB_CHECK(dns.back(ns.data()));
+        for (int s = 0; s < n; s++) {
+            for (int f = 0; f < nf; f++) {
+                NsqFrameOut* o = &out[(size_t)s * nfr + p * nf + f];
+                memcpy(o->q_md, scr[s].q_md[f], sizeof(o->q_md));
+                memcpy(o->r16, scr[s].r16[f], sizeof(o->r16));
+                o->Seed = scr[s].c[f].Seed;
+            }
+            for (int qz = 0; qz < 3; qz++) nsqio_state_from(&st_after[((size_t)s * npk + p) * 3 + qz], &ns[s * 3 + qz]);
+        }
+    }
+    return 0;
 }

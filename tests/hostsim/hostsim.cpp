@@ -106,6 +106,7 @@ static void run32m(const std::function<void()>& f) {
 #endif
 #include "../../solo_b200/csrc/sb_enc.cuh"
 #include "../../solo_b200/csrc/sb_dec.cuh"
+#include "../../oracle/nsq_io.h"
 #ifdef SB_EMU
 #include "../../solo_b200/csrc/sb_coop.cuh"
 // ---- the quantiser kernel's device code (sb_nsq_warp.cuh) under the same 32-fibre emulation: one stream per "warp"
@@ -218,6 +219,83 @@ int hs_enc_encode_pair(void* pa, void* pb, const short* pcm_a, const short* pcm_
     emu_nsq(hh);
     ret[0] = sb::enc_packet_finish(&hh[0]->st, &hh[0]->w.scr, hh[0]->w.rcbuf, out_a, cap, nb_a);
     ret[1] = sb::enc_packet_finish(&hh[1]->st, &hh[1]->w.scr, hh[1]->w.rcbuf, out_b, cap, nb_b);
+    return 0;
+#else
+    return -1;
+#endif
+}
+// ---- the quantiser stage on its own (tests/test_gpu_nsq.py), frames and states in the layout of oracle/nsq_io.h ----
+void nsq_io_sizes(int* s) { NSQ_IO_SIZES(s); }
+// one packet: what the quantiser stage receives -- fr[f] (frame control and prefiltered input of every frame) and st[3]
+// (the three quantiser states before it runs) -- then the rest of the packet as hs_enc_encode runs it
+int hs_enc_capture(void* p, const short* pcm, NsqFrameIn* fr, NsqStateIO* st, unsigned char* out, int cap, short* nb) {
+    HsEnc* h = (HsEnc*)p;
+    enc_front(h, pcm);
+    for (int f = 0; f < h->st.frames_per_packet; f++) sb::nsqio_frame_from(&fr[f], &h->w.scr.c[f], h->w.scr.xfw[f]);
+    for (int qz = 0; qz < 3; qz++) sb::nsqio_state_from(&st[qz], &h->st.nsq[qz]);
+    return sb::enc_packet_quantise_and_code(&h->st, &h->w, out, cap, nb);
+}
+// n cases of npk packets of nf frames each, from the states st0[n][3]: out[n][npk * nf] after every frame, st_after[n][npk][3]
+// after every packet.  kernel_code = 0: the scalar model (sb_nsq.cuh, one frame at a time); 1 (emulated builds): the device
+// code, nsq_packet_warp, on emulated warps with the kernel's packing -- lane group g of warp w takes case w * G + g (G = 32 /
+// SB_NSQ_GW), a group without a case of its own shadows the last one -- and its scratch outputs poisoned before every packet.
+int hs_nsq_run(int kernel_code, int n, int npk, int nf, const NsqStateIO* st0, const NsqFrameIn* fr, NsqFrameOut* out, NsqStateIO* st_after) {
+    if (n <= 0 || npk <= 0 || (nf != 1 && nf != 2)) return -1;
+    const int nfr = npk * nf;
+    if (kernel_code == 0) {
+        sb::EncState* st = (sb::EncState*)calloc(1, sizeof(sb::EncState));
+        sb::NsqWork* W = (sb::NsqWork*)calloc(1, sizeof(sb::NsqWork));
+        static sb::EncCtrl c;
+        sb::i32 r[sb::FRAME];
+        for (int s = 0; s < n; s++) {
+            for (int qz = 0; qz < 3; qz++) sb::nsqio_state_to(&st->nsq[qz], &st0[s * 3 + qz]);
+            for (int f = 0; f < nfr; f++) {
+                const NsqFrameIn* x = &fr[(size_t)s * nfr + f];
+                NsqFrameOut* o = &out[(size_t)s * nfr + f];
+                sb::nsqio_ctrl(&c, x);
+                sb::nsq_del_dec(st, &c, W, x->x, (sb::i8*)0, o->q_md[0], o->q_md[1], r);
+                for (int i = 0; i < sb::FRAME; i++) o->r16[i] = (sb::i16)(r[i] >> 10);
+                o->Seed = c.Seed;
+                if (f % nf == nf - 1)
+                    for (int qz = 0; qz < 3; qz++) sb::nsqio_state_from(&st_after[((size_t)s * npk + f / nf) * 3 + qz], &st->nsq[qz]);
+            }
+        }
+        free(st); free(W);
+        return 0;
+    }
+#ifdef SB_EMU
+    const int G = 32 / SB_NSQ_GW;
+    sb::NsqState* ns = (sb::NsqState*)calloc((size_t)n * 3, sizeof(sb::NsqState));
+    sb::EncScratch* scr = (sb::EncScratch*)calloc(n, sizeof(sb::EncScratch));
+    static sb::NsqSmem S[2];
+    for (int s = 0; s < n; s++) for (int qz = 0; qz < 3; qz++) sb::nsqio_state_to(&ns[s * 3 + qz], &st0[s * 3 + qz]);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) {
+            memset(scr[s].q_md, 0xA5, sizeof(scr[s].q_md)); memset(scr[s].r16, 0xA5, sizeof(scr[s].r16));
+            memset(scr[s].nsq_rand, 0xA5, sizeof(scr[s].nsq_rand));
+            for (int f = 0; f < nf; f++) {
+                const NsqFrameIn* x = &fr[(size_t)s * nfr + p * nf + f];
+                sb::nsqio_ctrl(&scr[s].c[f], x);
+                for (int i = 0; i < sb::FRAME; i++) scr[s].xfw[f][i] = x->x[i];
+            }
+        }
+        for (int w = 0; w * G < n; w++)
+            sb::emu::run32m([=]() {
+                const int g = sb::emu::lane / SB_NSQ_GW;
+                const int s = w * G + g < n ? w * G + g : n - 1;
+                sb::nsq_packet_warp(S[g], &ns[s * 3], &scr[s], nf);
+            });
+        for (int s = 0; s < n; s++) {
+            for (int f = 0; f < nf; f++) {
+                NsqFrameOut* o = &out[(size_t)s * nfr + p * nf + f];
+                memcpy(o->q_md, scr[s].q_md[f], sizeof(o->q_md));
+                memcpy(o->r16, scr[s].r16[f], sizeof(o->r16));
+                o->Seed = scr[s].c[f].Seed;
+            }
+            for (int qz = 0; qz < 3; qz++) sb::nsqio_state_from(&st_after[((size_t)s * npk + p) * 3 + qz], &ns[s * 3 + qz]);
+        }
+    }
+    free(ns); free(scr);
     return 0;
 #else
     return -1;

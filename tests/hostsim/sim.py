@@ -25,6 +25,9 @@ def lib(emu=None):
         L.hs_enc_set_control.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.hs_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.hs_dec_destroy.argtypes = [C.c_void_p]
+        L.nsq_io_sizes.argtypes = [C.c_void_p]
+        L.hs_enc_capture.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_void_p]
+        L.hs_nsq_run.argtypes = [C.c_int] * 4 + [C.c_void_p] * 4
         if emu:
             L.hs_set_emu_nsq.argtypes = [C.c_int]
             L.hs_enc_encode_pair.argtypes = [C.c_void_p] * 6 + [C.c_int] + [C.c_void_p] * 3
@@ -52,6 +55,21 @@ class SimEncoder:
         n = self.L.hs_enc_encode(self.h, x.ctypes.data, self.out.ctypes.data, self.cap, self.nb.ctypes.data)
         return bytes(self.out[:max(n, 0)]), (int(self.nb[0]), int(self.nb[1])), n
 
+    def capture(self, pcm640):
+        """Encode one packet and return what its quantiser stage received: the frames (oracle.nsq_ref.FRAME_IN, one per
+        frame of the packet) and the three quantiser states before it ran (oracle.nsq_ref.STATE, centre first)."""
+        from oracle import nsq_ref
+        x = np.ascontiguousarray(pcm640, np.int16)
+        assert x.size == self.samples
+        fr = np.zeros(self.samples // 320, nsq_ref.FRAME_IN)
+        st = np.zeros(3, nsq_ref.STATE)
+        if self.L.hs_is_emu() == 1:
+            self.L.hs_set_emu_nsq(0)
+        n = self.L.hs_enc_capture(self.h, x.ctypes.data, fr.ctypes.data, st.ctypes.data, self.out.ctypes.data, self.cap,
+                                  self.nb.ctypes.data)
+        assert n >= 0
+        return fr, st
+
     def set_control(self, rate=None, dtx=None, loss=None):
         """Rate (b/s), DTX and expected loss (%) from the next packet on, through enc_set_control; None = unchanged."""
         self.L.hs_enc_set_control(self.h, *(-1 if v is None else int(v) for v in (rate, dtx, loss)))
@@ -71,6 +89,24 @@ def encode_pair(ea, eb, pcm_a, pcm_b):
                                 ea.nb.ctypes.data, eb.nb.ctypes.data, ret.ctypes.data)
     assert r == 0
     return tuple((bytes(e.out[:max(int(n), 0)]), (int(e.nb[0]), int(e.nb[1])), int(n)) for e, n in ((ea, ret[0]), (eb, ret[1])))
+
+
+def nsq_run(st0, frames, nf, emu=None):
+    """The quantiser stage alone over n cases: st0 [n, 3] (oracle.nsq_ref.STATE), frames [n, npk * nf] (FRAME_IN).
+    emu=None: the scalar model; emu="gw16" (or True): the kernel's device code on emulated warps of that build.
+    Returns (out [n, npk * nf] FRAME_OUT, states after every packet [n, npk, 3] STATE)."""
+    from oracle import nsq_ref
+    L = lib(emu if emu else False)
+    nsq_ref.check_sizes(L)
+    st0 = np.ascontiguousarray(st0, nsq_ref.STATE)
+    frames = np.ascontiguousarray(frames, nsq_ref.FRAME_IN)
+    n, nfr = frames.shape
+    assert st0.shape == (n, 3) and nfr % nf == 0
+    out = np.zeros((n, nfr), nsq_ref.FRAME_OUT)
+    st = np.zeros((n, nfr // nf, 3), nsq_ref.STATE)
+    r = L.hs_nsq_run(1 if emu else 0, n, nfr // nf, nf, st0.ctypes.data, frames.ctypes.data, out.ctypes.data, st.ctypes.data)
+    assert r == 0, r
+    return out, st
 
 
 class SimDecoder:
