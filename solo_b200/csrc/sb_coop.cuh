@@ -13,12 +13,12 @@
 // side by side on consecutive threads (c_instances, sb_par.cuh).  Pure recurrences that depend on nothing else in the frame
 // are not here at all: the voice-activity detector runs before this kernel, the shaping-filter finishing and the prefilter
 // after it, as thread-per-instance kernels (solo_b200.cu).
-// The scalar routines of sb_enc_*.cuh / sb_sigproc.cuh remain the executable specification: tests/hostsim compiles both and
-// checks this file (32 fibres per stream, sb_par.cuh SB_EMU) against the golden bitstream on a machine without a GPU.
+// The per-frame control arithmetic between the lane-parallel cores (thresholds, scores, gains, shaping parameters, the
+// per-window shaping filter) is not restated here: it is the SB_HD helpers next to the scalar routines of sb_enc_*.cuh /
+// sb_sigproc.cuh, which both forms call.  tests/hostsim compiles both forms and checks this file (32 fibres per stream,
+// sb_par.cuh SB_EMU) against the golden bitstream and the scalar model on a machine without a GPU.
 #pragma once
-#include "sb_enc_front.cuh"
-#include "sb_enc_pred.cuh"
-#include "sb_enc_shape.cuh"
+#include "sb_enc.cuh"
 #include "sb_par.cuh"
 
 #if SB_COOP_ACTIVE
@@ -171,18 +171,7 @@ SB_CFN int c_pitch_analysis_core(PitchScr* P, const i16* signal, i32* pitch_out,
 #pragma unroll
     for (int j = 0; j < 5; j++) { const int i = lane + 32 * j; v[j] = i > 0 ? add_sat16(sig4[i], sig4[i - 1]) : (i32)sig4[0]; }
     SB_SYNC();
-    i32 mx = 0;
-#pragma unroll
-    for (int j = 0; j < 5; j++) mx = imax(mx, v[j] * v[j]);
-    mx = wmax(mx);
-    i32 shift;
-    // pitch_find_scaling(signal_4kHz, 160, 80): the reference takes |x| at the largest x^2 (-32768 counts as 32767)
-    const i32 x_max4 = mx >= 1073676289 ? 32767 : wmax(imax(imax(imax(iabs(v[0]), iabs(v[1])), imax(iabs(v[2]), iabs(v[3]))), iabs(v[4])));
-    {
-        i32 nbits = x_max4 < 32767 ? 32 - clz32(smulbb(x_max4, x_max4)) : 30;
-        nbits += 17 - (clz32(imax(SF8, FL4 >> 1)) - 16);
-        shift = nbits < 31 ? 0 : nbits - 30;
-    }
+    i32 shift = pitch_find_scaling(wmax(imax(imax(imax(iabs(v[0]), iabs(v[1])), imax(iabs(v[2]), iabs(v[3]))), iabs(v[4]))), imax(SF8, FL4 >> 1));
 #pragma unroll
     for (int j = 0; j < 5; j++) sig4[lane + 32 * j] = (i16)((i16)v[j] >> shift);
     SB_SYNC();
@@ -298,10 +287,7 @@ SB_CFN int c_pitch_analysis_core(PitchScr* P, const i16* signal, i32* pitch_out,
     {
         i32 m8 = 0;
         SB_PARFOR(i, 0, FL8) m8 = imax(m8, iabs((i32)sig8[i]));
-        const i32 x_max = imin(wmax(m8), 32767);
-        i32 nbits = x_max < 32767 ? 32 - clz32(smulbb(x_max, x_max)) : 30;
-        nbits += 17 - (clz32(SF8) - 16);
-        shift = nbits < 31 ? 0 : nbits - 30;
+        shift = pitch_find_scaling(wmax(m8), SF8);
     }
     if (shift > 0) SB_PARFOR(i, 0, FL8) sig8[i] = (i16)(sig8[i] >> shift);
     SB_SYNC();
@@ -317,26 +303,11 @@ SB_CFN int c_pitch_analysis_core(PitchScr* P, const i16* signal, i32* pitch_out,
 #pragma unroll 8
         for (int i = 0; i < SF8; i++) { const i32 bv = basis[i]; cross_corr = addw(cross_corr, (i32)target[i] * bv); energy_basis = addw(energy_basis, bv * bv); }
         const i32 energy_target = k == 0 ? et0 : (k == 1 ? et1 : (k == 2 ? et2 : et3));
-        i32 cv = 0;
-        if (cross_corr > 0) {
-            i32 en = imax(energy_target, energy_basis);
-            int lz = clz32(cross_corr);
-            int lshift = limit(lz - 1, 0, 15);
-            i32 temp32 = shl(cross_corr, lshift) / ((en >> (15 - lshift)) + 1);
-            temp32 = smulwb(cross_corr, temp32);
-            temp32 = add_sat32(temp32, temp32);
-            lz = clz32(temp32);
-            lshift = limit(lz - 1, 0, 15);
-            en = imin(energy_target, energy_basis);
-            cv = (i16)(shl(temp32, lshift) / ((en >> (15 - lshift)) + 1));
-        }
-        P->C2[k][j] = (i16)cv;
+        P->C2[k][j] = (i16)pitch_stage2_corr(cross_corr, energy_target, energy_basis);
     }
     SB_SYNC();
     // ---- search over the short list (one candidate lag per lane) ----
     const i16* cbl = SB_T(pitch_cb_lags_stage2);   // [4][11]
-    const i32 prevLag_log2_Q7 = prevLag > 0 ? lin2log(prevLag) : 0;
-    const i32 corr_thres_Q15 = smulbb(search_thres2_Q15, search_thres2_Q15) >> 13;
     const i32 ltpcorr_prev = *LTPCorr_Q15;
     i32 key = SB_I32_MIN, my_cc = SB_I32_MIN, my_cb = 0, my_d = 0;
     if (lane < length_d_srch) {
@@ -348,16 +319,7 @@ SB_CFN int c_pitch_analysis_core(PitchScr* P, const i16* signal, i32* pitch_out,
             for (int i = 0; i < 4; i++) { const int sl = P->slot[d + cbl[i * NCB + j]]; cc += sl ? (i32)P->C2[i][sl - 1] : 0; }
             if (cc > CCmax_new) { CCmax_new = cc; CBimax_new = j; }
         }
-        const i32 lag_log2_Q7 = lin2log(d);
-        i32 CCmax_new_b = CCmax_new - (smulbb(4 * 6554, lag_log2_Q7) >> 7);
-        if (prevLag > 0) {
-            i32 dl = lag_log2_Q7 - prevLag_log2_Q7;
-            dl = smulbb(dl, dl) >> 7;
-            i32 prev_lag_bias_Q15 = smulbb(4 * 6554, ltpcorr_prev) >> 15;
-            prev_lag_bias_Q15 = mulw(prev_lag_bias_Q15, dl) / (dl + (1 << 6));
-            CCmax_new_b -= prev_lag_bias_Q15;
-        }
-        if (CCmax_new > corr_thres_Q15 && cbl[0 * NCB + CBimax_new] <= MINL8) key = CCmax_new_b;
+        key = pitch_lag_score(CCmax_new, CBimax_new, d, prevLag, ltpcorr_prev, search_thres2_Q15);
         my_cc = CCmax_new; my_cb = CBimax_new; my_d = d;
     }
     i32 best = key, who = lane;
@@ -413,7 +375,7 @@ SB_CFN void c_find_pitch_lags(EncSilk* st, EncCtrl* c, PitchScr* P, i16* res, co
     SB_SYNC();
     const i32 ac0 = P->acorr[0];
     const i32 res_nrg = c_schur(P->rc_Q15, P->acorr, ORD);
-    const i32 predGain = div32_varq(ac0, imax(res_nrg, 1), 16);
+    const i32 predGain = pitch_pred_gain_q16(ac0, res_nrg);
     SB_SYNC();
     const i32 A_Q24 = c_k2a(P->rc_Q15, ORD);
     {
@@ -424,17 +386,12 @@ SB_CFN void c_find_pitch_lags(EncSilk* st, EncCtrl* c, PitchScr* P, i16* res, co
     c_fir_zero_state<ORD, false>(x_buf, P->A_Q12, res, BUF_LEN);
     SB_SYNC();
     if (lane < ORD) res[lane] = 0;
-    i32 thrhld_Q15 = SB_FIXC(0.45, 15);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.004, 15), ORD);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.1, 7), st->speech_activity_Q8);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(0.15, 15), st->prev_sigtype);
-    thrhld_Q15 = smlawb(thrhld_Q15, SB_FIXC(-0.1, 16), c->input_tilt_Q15);
-    thrhld_Q15 = sat16(thrhld_Q15);
+    const i32 thrhld_Q15 = pitch_thrhld_q15(st->speech_activity_Q8, st->prev_sigtype, c->input_tilt_Q15);
     const i32 prevLag = st->prevLag;
     SB_SYNC();
     SB_PHASE();
     const int sigtype = c_pitch_analysis_core(P, res, c->pitchL, &c->lagIndex, &c->contourIndex, &st->LTPCorr_Q15, prevLag,
-                                              SB_FIXC(0.7f, 16), (i16)thrhld_Q15);
+                                              SB_FIXC(0.7f, 16), thrhld_Q15);
     if (lane == 0) { c->sigtype = sigtype; c->predGain_Q16 = predGain; }
     SB_SYNC();
 }
@@ -490,73 +447,14 @@ SB_CFN void c_warped_autocorr4(ShapeScr* S, i32 warping_Q16) {
     if (g == 0) S->scale[win] = -(QC + lsh);
 }
 
-// ---- the per-window recursions with every array in registers (fixed order, fully unrolled): on the device these run as
-// one scalar instance per window, where a local-memory array would put a ~30-cycle load into every step of a long
-// dependent chain.  Same arithmetic as schur64 / k2a_q16 / bwexpander_32 (sb_sigproc.cuh), which remain the reference
-// statements.
-template <int ORD> SB_CFN i32 schur64_r(i32 (&rc_Q16)[ORD], const i32 (&c)[ORD + 1]) {
-    i32 C0[ORD + 1], C1[ORD + 1];
-    if (c[0] <= 0) {
-#pragma unroll
-        for (int k = 0; k < ORD; k++) rc_Q16[k] = 0;
-        return 0;
-    }
-#pragma unroll
-    for (int k = 0; k < ORD + 1; k++) C0[k] = C1[k] = c[k];
-#pragma unroll
-    for (int k = 0; k < ORD; k++) {
-        const i32 rc_Q31 = div32_varq(negw(C0[k + 1]), C1[0], 31);
-        rc_Q16[k] = rshift_round(rc_Q31, 15);
-#pragma unroll
-        for (int n = 0; n < ORD - k; n++) {
-            const i32 t1 = C0[n + k + 1], t2 = C1[n];
-            C0[n + k + 1] = addw(t1, smmul(shl(t2, 1), rc_Q31));
-            C1[n] = addw(t2, smmul(shl(t1, 1), rc_Q31));
-        }
-    }
-    return C1[0];
-}
-template <int ORD> SB_CFN void k2a_q16_r(i32 (&A_Q24)[ORD], const i32 (&rc_Q16)[ORD]) {
-#pragma unroll
-    for (int k = 0; k < ORD; k++) {
-        i32 Atmp[ORD];
-#pragma unroll
-        for (int n = 0; n < k; n++) Atmp[n] = A_Q24[n];
-#pragma unroll
-        for (int n = 0; n < k; n++) A_Q24[n] = smlaww(A_Q24[n], Atmp[k - n - 1], rc_Q16[k]);
-        A_Q24[k] = negw(shl(rc_Q16[k], 8));
-    }
-}
-template <int ORD> SB_CFN void bwexpander_32_r(i32 (&ar)[ORD], i32 chirp_Q16) {
-    i32 t = chirp_Q16;
-#pragma unroll
-    for (int i = 0; i < ORD - 1; i++) { ar[i] = smulww(ar[i], t); t = smulww(chirp_Q16, t); }
-    ar[ORD - 1] = smulww(ar[ORD - 1], t);
-}
-
 // pitch_res points at res_pitch + FRAME, x at x_buf + FRAME.
 SB_CFN void c_noise_shape_analysis(EncSilk* st, EncCtrl* c, ShapeScr* S, const i16* pitch_res, const i16* x) {
     const int lane = SB_LANE;
     // ---- scalars, computed by every lane from shared data; lane 0 stores ----
     const i32 sigtype = c->sigtype;
     const i32 speech_activity_Q8 = st->speech_activity_Q8, LTPCorr_Q15 = st->LTPCorr_Q15;
-    const i32 current_SNR_dB_Q7 = st->SNR_dB_Q7, current_SNRPerMD_dB_Q7 = st->SNRPerMD_dB_Q7;
-    const i32 input_quality_Q14 = (c->input_quality_bands_Q15[0] + c->input_quality_bands_Q15[1]) >> 2;
-    const i32 coding_quality_Q14 = sigm_q15(rshift_round(current_SNR_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
-    i32 b_Q8 = SB_FIXC(1.0, 8) - speech_activity_Q8;
-    b_Q8 = smulwb(shl(b_Q8, 8), b_Q8);
-    i32 SNR_adj_dB_Q7 = smlawb(current_SNR_dB_Q7, smulbb(SB_FIXC(-4.0f, 7) >> (4 + 1), b_Q8),
-                               smulwb(SB_FIXC(1.0, 14) + input_quality_Q14, coding_quality_Q14));
-    if (sigtype == 0) SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, SB_FIXC(2.0f, 8), LTPCorr_Q15);
-    else SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, smlawb(SB_FIXC(6.0, 9), -SB_FIXC(0.4, 18), current_SNR_dB_Q7), SB_FIXC(1.0, 14) - input_quality_Q14);
-    const i32 md_input_quality_Q14 = sigm_q15(rshift_round(current_SNRPerMD_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
-    i32 md_SNR_adj_dB_Q7 = smlawb(current_SNRPerMD_dB_Q7, smulbb(SB_FIXC(-4.0f, 7) >> (4 + 1), b_Q8),
-                                  smulwb(SB_FIXC(1.0, 14) + md_input_quality_Q14, coding_quality_Q14));
-    if (sigtype == 0) md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, SB_FIXC(2.0f, 8), LTPCorr_Q15);
-    else md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, smlawb(SB_FIXC(6.0, 9), -SB_FIXC(0.4, 18), current_SNRPerMD_dB_Q7), SB_FIXC(1.0, 14) - input_quality_Q14);
-
     // sparseness of the residual (unvoiced): ten 2 ms energies, one per lane
-    i32 sparseness_Q8 = 0, QuantOffsetType = 0;
+    i32 energy_variation_Q7 = 0;
     if (sigtype != 0) {      // uniform
         i32 log_energy_Q7 = 0;
         if (lane < 10) {
@@ -566,22 +464,11 @@ SB_CFN void c_noise_shape_analysis(EncSilk* st, EncCtrl* c, ShapeScr* S, const i
             log_energy_Q7 = lin2log(nrg);
         }
         const i32 prev = wshfl_up(log_energy_Q7, 1);
-        const i32 energy_variation_Q7 = wsum((lane >= 1 && lane < 10) ? iabs(log_energy_Q7 - prev) : 0);
-        sparseness_Q8 = sigm_q15(smulwb(energy_variation_Q7 - SB_FIXC(5.0, 7), SB_FIXC(0.1, 16))) >> 7;
-        QuantOffsetType = sparseness_Q8 > SB_FIXC(0.75f, 8) ? 0 : 1;
-        SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), sparseness_Q8 - SB_FIXC(0.5, 8));
-        md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), sparseness_Q8 - SB_FIXC(0.5, 8));
+        energy_variation_Q7 = wsum((lane >= 1 && lane < 10) ? iabs(log_energy_Q7 - prev) : 0);
     }
-    // bandwidth expansion control
-    const i32 predGain_Q16 = c->predGain_Q16;
-    i32 strength_Q16 = smulwb(predGain_Q16, SB_FIXC(1e-3f, 16));
-    i32 BWExp1_Q16, BWExp2_Q16;
-    BWExp1_Q16 = BWExp2_Q16 = div32_varq(SB_FIXC(0.95f, 16), smlaww(SB_FIXC(1.0, 16), strength_Q16, strength_Q16), 16);
-    const i32 delta_Q16 = smulwb(SB_FIXC(1.0, 16) - smulbb(3, coding_quality_Q14), SB_FIXC(0.01f, 16));
-    BWExp1_Q16 = subw(BWExp1_Q16, delta_Q16);
-    BWExp2_Q16 = addw(BWExp2_Q16, delta_Q16);
-    BWExp1_Q16 = shl(BWExp1_Q16, 14) / (BWExp2_Q16 >> 2);
-    const i32 warping_Q16 = smlawb(WARPING_Q16, coding_quality_Q14, SB_FIXC(0.01, 18));
+    const ShapeCtl s = shape_control(sigtype, st->SNR_dB_Q7, st->SNRPerMD_dB_Q7, c->input_quality_bands_Q15, speech_activity_Q8,
+                                     LTPCorr_Q15, energy_variation_Q7, c->predGain_Q16);
+    const i32 warping_Q16 = s.warping_Q16;
 
     // ---- the four 15 ms windows: slopes on eight lanes, flat parts copied by all ----
     {
@@ -602,96 +489,33 @@ SB_CFN void c_noise_shape_analysis(EncSilk* st, EncCtrl* c, ShapeScr* S, const i
     SB_SYNC();
     SB_PHASE();
     // ---- per window: reflection coefficients, shaping filters, gains -- one scalar instance per window ----
-    if (lane == 0) { S->par3[0] = warping_Q16; S->par3[1] = BWExp1_Q16; S->par3[2] = BWExp2_Q16; }
+    if (lane == 0) { S->par3[0] = warping_Q16; S->par3[1] = s.BWExp1_Q16; S->par3[2] = s.BWExp2_Q16; }
     c_instances<NB_SUBFR>([&](int d, int k) {
         ShapeScr* Sj = xoff(S, d);
-        EncCtrl* cj = xoff(c, d);
-        const i32 warp_Q16 = Sj->par3[0], bw1 = Sj->par3[1], bw2 = Sj->par3[2];
-        i32 auto_corr[SHAPE_ORDER + 1], refl_coef_Q16[SHAPE_ORDER], AR1_Q24[SHAPE_ORDER], AR2_Q24[SHAPE_ORDER];
+        i32 auto_corr[SHAPE_ORDER + 1], AR1_Q24[SHAPE_ORDER], AR2_Q24[SHAPE_ORDER];
 #pragma unroll
         for (int i = 0; i <= SHAPE_ORDER; i++) auto_corr[i] = Sj->acorr[k][i];
-        auto_corr[0] = addw(auto_corr[0], imax(smulwb(auto_corr[0] >> 4, SB_FIXC(1e-5f, 20)), 1));
-        i32 nrg = schur64_r<SHAPE_ORDER>(refl_coef_Q16, auto_corr);
-        k2a_q16_r<SHAPE_ORDER>(AR2_Q24, refl_coef_Q16);
-        int Qnrg = -Sj->scale[k];
-        if (Qnrg & 1) { Qnrg -= 1; nrg >>= 1; }
-        const i32 tmp32 = sqrt_approx(nrg);
-        Qnrg >>= 1;
-        i32 gk = lshift_sat32(tmp32, 16 - Qnrg);
-        i32 gain_mult_Q16;
-        {   // warped_gain (noise_shape_analysis_FIX.c:33-50)
-            const i32 lam = -warp_Q16;
-            i32 g24 = AR2_Q24[SHAPE_ORDER - 1];
-#pragma unroll
-            for (int i = SHAPE_ORDER - 2; i >= 0; i--) g24 = smlawb(AR2_Q24[i], g24, lam);
-            g24 = smlawb(SB_FIXC(1.0, 24), g24, -lam);
-            gain_mult_Q16 = inverse32_varq(g24, 40);
-        }
-        gk = smulww(gk, gain_mult_Q16);
-        if (gk < 0) gk = SB_I32_MAX;
-        bwexpander_32_r<SHAPE_ORDER>(AR2_Q24, bw2);
-#pragma unroll
-        for (int i = 0; i < SHAPE_ORDER; i++) AR1_Q24[i] = AR2_Q24[i];
-        bwexpander_32_r<SHAPE_ORDER>(AR1_Q24, bw1);
-        Sj->gains[k][0] = gk;
+        Sj->gains[k][0] = shape_window(AR2_Q24, AR1_Q24, auto_corr, Sj->scale[k], Sj->par3[0], Sj->par3[1], Sj->par3[2]);
 #pragma unroll
         for (int i = 0; i < SHAPE_ORDER; i++) { Sj->ar[k][0][i] = AR2_Q24[i]; Sj->ar[k][1][i] = AR1_Q24[i]; }
     });
     // (inverse prediction gains, pre-gains, coefficient limiting and the Q13 coefficients of the windows are finished by the
     //  shaping-filter kernel that runs after this one: nothing in the rest of the analysis reads them)
-    i32 gain_k = S->gains[lane & 3][0];
-    // ---- gain tweaking ----
-    const i32 md_gain_mult_Q16 = log2lin(negw(smlawb(-SB_FIXC(16.0, 7), md_SNR_adj_dB_Q7, SB_FIXC(0.16, 16))));
-    i32 gain_mult_Q16 = log2lin(negw(smlawb(-SB_FIXC(16.0, 7), SNR_adj_dB_Q7, SB_FIXC(0.16, 16))));
+    // ---- gain tweaking: lane k owns sub-frame k ----
+    const i32 md_gain_mult_Q16 = shape_gain_mult_q16(s.md_SNR_adj_dB_Q7);
+    const i32 gain_mult_Q16 = shape_gain_mult_q16(s.SNR_adj_dB_Q7);
     const float md_delta_gain_par = (float)gain_mult_Q16 / (float)md_gain_mult_Q16;
-    i32 gain_add_Q16 = log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(4.0f, 7), SB_FIXC(0.16, 16)));
     i32 avgGain_Q16 = st->avgGain_Q16;
-    {
-        i32 t32 = log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(-50.0f, 7), SB_FIXC(0.16, 16)));
-        t32 = smulww(avgGain_Q16, t32);
-        gain_add_Q16 = add_sat32(gain_add_Q16, t32);
-    }
-    gain_k = smulww(gain_k, gain_mult_Q16);
-    if (gain_k < 0) gain_k = SB_I32_MAX;
-    gain_k = add_pos_sat32(gain_k, gain_add_Q16);
-    {   // the running average chains through the four sub-frames
-        const i32 coef = rshift_round(smulbb(speech_activity_Q8, SB_FIXC(1e-3f, 10)), 2);
-        for (int k = 0; k < NB_SUBFR; k++) {
-            const i32 gk = wshfl(gain_k, k);
-            avgGain_Q16 = add_sat32(avgGain_Q16, smulwb(gk - avgGain_Q16, coef));
-        }
-    }
-    gain_mult_Q16 = SB_FIXC(1.0, 16) + rshift_round(mlaw(SB_FIXC(0.05f, 26), coding_quality_Q14, SB_FIXC(0.1f, 12)), 10);   // pre-gain multiplier
+    const i32 gain_k = shape_gain_tweak(S->gains[lane & 3][0], gain_mult_Q16, shape_gain_add_q16(avgGain_Q16));
+    for (int k = 0; k < NB_SUBFR; k++) avgGain_Q16 = shape_avg_gain_q16(avgGain_Q16, wshfl(gain_k, k), speech_activity_Q8);
     // ---- low-frequency shaping, tilt, harmonic shaping ----
-    strength_Q16 = mulw(SB_FIXC(3.0f, 0), SB_FIXC(1.0, 16) + smulbb(SB_FIXC(0.5f, 1), c->input_quality_bands_Q15[0] - SB_FIXC(1.0, 15)));
-    i32 Tilt_Q16, LF_shp_k;
-    if (sigtype == 0) {
-        const i32 fs_kHz_inv = SB_FIXC(0.2, 14) / 8;
-        const i32 b_Q14 = fs_kHz_inv + SB_FIXC(3.0, 14) / imax(c->pitchL[lane & 3], 1);
-        LF_shp_k = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, b_Q14), 16);
-        LF_shp_k |= (u16)(b_Q14 - SB_FIXC(1.0, 14));
-        Tilt_Q16 = -SB_FIXC(0.3f, 16) - smulwb(SB_FIXC(1.0, 16) - SB_FIXC(0.3f, 16), smulwb(SB_FIXC(0.35f, 24), speech_activity_Q8));
-    } else {
-        const i32 b_Q14 = 21299 / 8;
-        LF_shp_k = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, smulwb(SB_FIXC(0.6, 16), b_Q14)), 16);
-        LF_shp_k |= (u16)(b_Q14 - SB_FIXC(1.0, 14));
-        Tilt_Q16 = -SB_FIXC(0.3f, 16);
-    }
-    i32 HarmBoost_Q16 = smulwb(smulwb(SB_FIXC(1.0, 17) - shl(coding_quality_Q14, 3), LTPCorr_Q15), SB_FIXC(0.1f, 16));
-    HarmBoost_Q16 = smlawb(HarmBoost_Q16, SB_FIXC(1.0, 16) - shl(input_quality_Q14, 2), SB_FIXC(0.1f, 16));
-    i32 HarmShapeGain_Q16 = 0;
-    if (sigtype == 0) {
-        HarmShapeGain_Q16 = smlawb(SB_FIXC(0.3f, 16),
-            SB_FIXC(1.0, 16) - smulwb(SB_FIXC(1.0, 18) - shl(coding_quality_Q14, 4), input_quality_Q14), SB_FIXC(0.2f, 16));
-        HarmShapeGain_Q16 = smulwb(shl(HarmShapeGain_Q16, 1), sqrt_approx(shl(LTPCorr_Q15, 15)));
-    }
+    const i32 LF_shp_k = shape_lf_shp_q14(sigtype, c->pitchL[lane & 3], c->input_quality_bands_Q15[0]);
+    const HarmTilt h = shape_harm_tilt(sigtype, speech_activity_Q8, s.input_quality_Q14, s.coding_quality_Q14, LTPCorr_Q15);
     i32 hb = st->HarmBoost_smth_Q16, hs = st->HarmShapeGain_smth_Q16, ti = st->Tilt_smth_Q16;
     i32 hb_k = 0, hs_k = 0, ti_k = 0;
     for (int k = 0; k < NB_SUBFR; k++) {
-        hb = smlawb(hb, HarmBoost_Q16 - hb, SB_FIXC(0.4f, 16));
-        hs = smlawb(hs, HarmShapeGain_Q16 - hs, SB_FIXC(0.4f, 16));
-        ti = smlawb(ti, Tilt_Q16 - ti, SB_FIXC(0.4f, 16));
-        if (lane == k) { hb_k = rshift_round(hb, 2); hs_k = rshift_round(hs, 2); ti_k = rshift_round(ti, 2); }
+        const i32 hb_q = shape_smooth_q14(hb, h.HarmBoost_Q16), hs_q = shape_smooth_q14(hs, h.HarmShapeGain_Q16), ti_q = shape_smooth_q14(ti, h.Tilt_Q16);
+        if (lane == k) { hb_k = hb_q; hs_k = hs_q; ti_k = ti_q; }
     }
     SB_SYNC();     // every lane has read what it needs from c / st
     if (lane < NB_SUBFR) {
@@ -702,16 +526,16 @@ SB_CFN void c_noise_shape_analysis(EncSilk* st, EncCtrl* c, ShapeScr* S, const i
         c->Tilt_Q14[lane] = ti_k;
     }
     if (lane == 0) {
-        c->current_SNR_dB_Q7 = current_SNR_dB_Q7;
-        c->current_SNRPerMD_dB_Q7 = current_SNRPerMD_dB_Q7;
-        c->input_quality_Q14 = input_quality_Q14;
-        c->coding_quality_Q14 = coding_quality_Q14;
-        c->sparseness_Q8 = sparseness_Q8;
-        c->QuantOffsetType = QuantOffsetType;
+        c->current_SNR_dB_Q7 = st->SNR_dB_Q7;
+        c->current_SNRPerMD_dB_Q7 = st->SNRPerMD_dB_Q7;
+        c->input_quality_Q14 = s.input_quality_Q14;
+        c->coding_quality_Q14 = s.coding_quality_Q14;
+        c->sparseness_Q8 = s.sparseness_Q8;
+        c->QuantOffsetType = s.QuantOffsetType;
         c->md_delta_gain_par = md_delta_gain_par;
         st->avgGain_Q16 = avgGain_Q16;
         st->HarmBoost_smth_Q16 = hb; st->HarmShapeGain_smth_Q16 = hs; st->Tilt_smth_Q16 = ti;
-        S->par3[1] = gain_mult_Q16;
+        S->par3[1] = shape_pregain_mult_q16(s.coding_quality_Q14);
     }
     SB_SYNC();
 }
@@ -1077,13 +901,7 @@ SB_CFN void c_find_lpc(i32* NLSF_Q15, i32* interpIndex, const i32* prev_NLSFq_Q1
     const bool interpOn = useInterp == 1;      // per stream: the instance sections below are entered by every warp of the block
     if (lane == 0) Q->flag_interp = interpOn ? 1 : 0;
     if (interpOn) {
-        int shift = res_tmp_nrg_Q - res_nrg_Q;
-        if (shift >= 0) {
-            if (shift < 32) res_nrg = subw(res_nrg, res_tmp_nrg >> shift);
-        } else {
-            res_nrg = subw(res_nrg >> (-shift), res_tmp_nrg);
-            res_nrg_Q = res_tmp_nrg_Q;
-        }
+        lpc_first_half_nrg(res_nrg, res_nrg_Q, res_tmp_nrg, res_tmp_nrg_Q);
         c_a2nlsf<ORD>(NLSF_Q15, Q->A_Q16[1], &Q->u.lpc.a2n);
     }
     // the four interpolation candidates: NLSF -> LPC as four scalar instances, analysis filters over all lanes
@@ -1119,21 +937,8 @@ SB_CFN void c_find_lpc(i32* NLSF_Q15, i32* interpIndex, const i32* prev_NLSFq_Q1
         Qj->ie[k][0] = e; Qj->ie[k][1] = sft;
     });
     if (interpOn) {
-        for (int kq = 3; kq >= 0; kq--) {
-            i32 res_nrg0 = Q->ie[2 * kq][0], res_nrg1 = Q->ie[2 * kq + 1][0];
-            const i32 rshift0 = Q->ie[2 * kq][1], rshift1 = Q->ie[2 * kq + 1][1];
-            i32 res_nrg_interp_Q;
-            int shift = rshift0 - rshift1;
-            if (shift >= 0) { res_nrg1 = res_nrg1 >> shift; res_nrg_interp_Q = -rshift0; }
-            else { res_nrg0 = res_nrg0 >> (-shift); res_nrg_interp_Q = -rshift1; }
-            const i32 res_nrg_interp = addw(res_nrg0, res_nrg1);
-            shift = res_nrg_interp_Q - res_nrg_Q;
-            int lower;
-            if (shift >= 0) lower = (res_nrg_interp >> shift) < res_nrg;
-            else if (-shift < 32) lower = res_nrg_interp < (res_nrg >> (-shift));
-            else lower = 0;
-            if (lower) { res_nrg = res_nrg_interp; res_nrg_Q = res_nrg_interp_Q; interp = kq; }
-        }
+        for (int kq = 3; kq >= 0; kq--)
+            if (lpc_interp_lower(res_nrg, res_nrg_Q, Q->ie[2 * kq][0], Q->ie[2 * kq][1], Q->ie[2 * kq + 1][0], Q->ie[2 * kq + 1][1])) interp = kq;
         SB_SYNC();
     }
     if (interp == 4) c_a2nlsf<ORD>(NLSF_Q15, Q->A_Q16[0], &Q->u.lpc.a2n);
@@ -1314,14 +1119,7 @@ SB_CFN void c_process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, PredScr* Q,
     const int lane = SB_LANE;
     const int sigtype = c->sigtype, interpQ2 = c->NLSFInterpCoef_Q2;
     i32 NLSF_mu_Q15, NLSF_mu_fluc_red_Q16;
-    if (sigtype == 0) {
-        NLSF_mu_Q15 = smlawb(66, -8388, st->speech_activity_Q8);
-        NLSF_mu_fluc_red_Q16 = smlawb(6554, -838848, st->speech_activity_Q8);
-    } else {
-        NLSF_mu_Q15 = smlawb(164, -33554, st->speech_activity_Q8);
-        NLSF_mu_fluc_red_Q16 = smlawb(13107, -1677696, st->speech_activity_Q8 + c->sparseness_Q8);
-    }
-    NLSF_mu_Q15 = imax(NLSF_mu_Q15, 1);
+    nlsf_mu(NLSF_mu_Q15, NLSF_mu_fluc_red_Q16, sigtype, st->speech_activity_Q8, c->sparseness_Q8);
     const int doInterpolate = interpQ2 < (1 << 2);
     // Laroia weights: one scalar instance for the target vector, one for the interpolated one (eleven divisions each)
     c_instances<2>([&](int d, int k) {
@@ -1339,12 +1137,8 @@ SB_CFN void c_process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, PredScr* Q,
         for (int i = 0; i < LPC_ORDER; i++) Qj->u.vq.nlsf_s[k][i] = w[i];
     });
     if (lane < LPC_ORDER) {
-        i32 w = Q->u.vq.nlsf_s[0][lane];
-        if (doInterpolate) {
-            const i32 i_sqr_Q15 = shl(smulbb(interpQ2, interpQ2), 11);
-            w = smlawb(w >> 1, Q->u.vq.nlsf_s[1][lane], i_sqr_Q15);
-        }
-        Q->NLSFW_Q6[lane] = w;
+        const i32 w = Q->u.vq.nlsf_s[0][lane];
+        Q->NLSFW_Q6[lane] = doInterpolate ? nlsf_interp_weight_q6(w, Q->u.vq.nlsf_s[1][lane], interpQ2) : w;
     }
     SB_SYNC();
     NlsfCb cb = nlsf_cb(sigtype);
@@ -1358,7 +1152,7 @@ SB_CFN void c_process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, PredScr* Q,
     if (lane < LPC_ORDER) {
         const i32 q = pNLSF_Q15[lane];
         Q->nlsf_out[1][lane] = q;
-        Q->nlsf_out[0][lane] = doInterpolate ? st->prev_NLSFq_Q15[lane] + (mulw(q - st->prev_NLSFq_Q15[lane], interpQ2) >> 2) : q;
+        Q->nlsf_out[0][lane] = nlsf_first_half_q15(st->prev_NLSFq_Q15[lane], q, interpQ2);
     }
     SB_SYNC();
 }
@@ -1367,7 +1161,7 @@ SB_CFN void c_process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, PredScr* Q,
 SB_CFN void c_find_pred_coefs(EncSilk* st, EncCtrl* c, PredScr* Q, const i16* res_pitch, int frame_in_packet, const NlsfFastTabs* fast) {
     const int lane = SB_LANE;
     const int sigtype = c->sigtype;
-    {
+    {   // (find_pred_coefs states this step too: as a shared helper it grows this kernel's spill traffic)
         const i32 g = c->Gains_Q16[lane & 3];
         i32 min_gain_Q16 = SB_I32_MAX >> 6;
         for (int i = 0; i < NB_SUBFR; i++) min_gain_Q16 = imin(min_gain_Q16, c->Gains_Q16[i]);
@@ -1402,15 +1196,7 @@ SB_CFN void c_find_pred_coefs(EncSilk* st, EncCtrl* c, PredScr* Q, const i16* re
         // SKP_Silk_LTP_analysis_filter_FIX (LTP_analysis_filter_FIX.c:30-80): lanes over outputs
         for (int t = lane; t < NB_SUBFR * (SUBFR + LPC_ORDER); t += 32) {
             const int k = t / (SUBFR + LPC_ORDER), i = t - k * (SUBFR + LPC_ORDER);
-            const i16* x_ptr = xb + k * SUBFR;
-            const i16* x_lag_ptr = x_ptr - c->pitchL[k] + i;
-            const i16* Bq = &c->LTPCoef_Q14[k * LTP_ORDER];
-            i32 est = smulbb(x_lag_ptr[LTP_ORDER / 2], Bq[0]);
-#pragma unroll
-            for (int j = 1; j < LTP_ORDER; j++) est = smlabb(est, x_lag_ptr[LTP_ORDER / 2 - j], Bq[j]);
-            est = rshift_round(est, 14);
-            const i32 r = sat16((i32)x_ptr[i] - est);
-            Q->LPC_in_pre[t] = (i16)smulwb(Q->invGains_Q16[k], r);
+            Q->LPC_in_pre[t] = ltp_analysis_sample(xb, c->LTPCoef_Q14, c->pitchL, Q->invGains_Q16, k, i);
         }
     } else {
         for (int t = lane; t < NB_SUBFR * (SUBFR + LPC_ORDER); t += 32) {
@@ -1470,21 +1256,14 @@ template <int F> SB_CFN void c_hb_analyse_frame(EncBands* hb, HbScr* H, const i1
     const i16* cb2 = SB_T(hb_lsp_cb2_fix);
     i32 best = SB_I32_MAX, idx1 = 0;
     for (int e = lane; e < 256; e += 32) {
-        i32 dist = 0;
-#pragma unroll
-        for (int j = 0; j < HB_ORDER; j++) { const i32 t = lsp[j] - cb1[e * HB_ORDER + j]; dist = smlabb(dist, t, t); }
+        const i32 dist = hb_lsp_dist1(lsp, e);
         if (dist < best) { best = dist; idx1 = e; }
     }
     wargmin(best, idx1);
 #pragma unroll
     for (int j = 0; j < HB_ORDER; j++) lsp[j] -= cb1[idx1 * HB_ORDER + j];
     i32 best2 = SB_I32_MAX, idx2 = lane;
-    if (lane < 16) {
-        i32 dist = 0;
-#pragma unroll
-        for (int j = 0; j < HB_ORDER; j++) { const i32 t = subw(lsp[j], cb2[lane * HB_ORDER + j]); dist = smlawb(dist, smulbb(t, t), H->weight[j]); }
-        best2 = dist;
-    }
+    if (lane < 16) best2 = hb_lsp_dist2(lsp, H->weight, lane);
     wargmin(best2, idx2);
     if (best2 == SB_I32_MAX) idx2 = 0;      // the reference's strict comparison never accepts INT_MAX
     SB_SYNC();
@@ -1563,17 +1342,9 @@ SB_CFN void c_encode_frame_analysis(EncSilk* st, CoopWork* W, const i16* pIn, in
     EncCtrl* c = &W->c;
     i16* x_frame = st->x_buf + FRAME;
     c_instances<1>([&](int d, int) {
-        EncSilk* sj = xoff(st, d);
         CoopWork* Wj = xoff(W, d);
-        EncCtrl* cj = &Wj->c;
-        const i16* pj = xoff(pIn, d);
-        cj->Seed = sj->frameCounter++ & 3;
-        // voice activity of this frame: computed ahead of time by the VAD kernel (it depends on nothing but the band signal
-        // and its own state), handed over in W->vad
-        sj->speech_activity_Q8 = Wj->vad[frame_in_packet][0];
-        for (int b = 0; b < 4; b++) cj->input_quality_bands_Q15[b] = Wj->vad[frame_in_packet][1 + b];
-        cj->input_tilt_Q15 = Wj->vad[frame_in_packet][5];
-        hp_variable_cutoff(sj, cj, Wj->pIn_HP, pj);
+        const i32* vad = Wj->vad[frame_in_packet];
+        frame_analysis_begin(xoff(st, d), &Wj->c, Wj->pIn_HP, xoff(pIn, d), vad[0], vad + 1, vad[5]);
     });
     SB_PARFOR(i, 0, FRAME) x_frame[LA_SHAPE + i] = W->pIn_HP[i];   // LP_variable_cutoff is a copy (transition_frame_no == 0)
     SB_SYNC();
@@ -1586,11 +1357,7 @@ SB_CFN void c_encode_frame_analysis(EncSilk* st, CoopWork* W, const i16* pIn, in
     SB_SYNC();
     SB_PHASE();
     c_find_pred_coefs(st, c, &W->u.pred, W->res_pitch, frame_in_packet, fast);
-    if (SB_LANE0) {
-        st->prev_sigtype = c->sigtype;
-        st->prevLag = c->pitchL[NB_SUBFR - 1];
-        st->first_frame_after_reset = 0;
-    }
+    if (SB_LANE0) frame_analysis_end(st, c);
     SB_SYNC();
     {   // x_buf slides by one frame: [0,160) <- [160,320), then [160,200) <- [320,360) (each step reads only unwritten words)
         i32* xb = reinterpret_cast<i32*>(st->x_buf);

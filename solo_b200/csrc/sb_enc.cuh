@@ -109,6 +109,22 @@ SB_FN void qmf_decomp(const i16* xx, i16* y1, i16* y2, i16* mem, int N) {
 }
 
 // ---- AGR_Sate_lsp_quant_highband (AGR_BWE_quant_highband.c:23-104) ----------------------------------------------
+// Distances of lsp to first-stage code vector i (squared error) and of the first stage's residual to second-stage code
+// vector i (Laroia-weighted); the high-band kernel evaluates one code vector per lane (c_hb_analyse_frame, sb_coop.cuh).
+SB_HD i32 hb_lsp_dist1(const i32* lsp, int i) {
+    const i16* cb1 = SB_T(hb_lsp_cb1_fix);
+    i32 dist = 0;
+#pragma unroll
+    for (int j = 0; j < HB_ORDER; j++) { const i32 t = lsp[j] - cb1[i * HB_ORDER + j]; dist = smlabb(dist, t, t); }
+    return dist;
+}
+SB_HD i32 hb_lsp_dist2(const i32* res, const i32* weight, int i) {
+    const i16* cb2 = SB_T(hb_lsp_cb2_fix);
+    i32 dist = 0;
+#pragma unroll
+    for (int j = 0; j < HB_ORDER; j++) { const i32 t = subw(res[j], cb2[i * HB_ORDER + j]); dist = smlawb(dist, smulbb(t, t), weight[j]); }
+    return dist;
+}
 SB_FN i32 hb_lsp_quant(i32* lsp) {
     i32 weight[HB_ORDER];
     nlsf_vq_weights_laroia(weight, lsp, HB_ORDER);
@@ -116,15 +132,13 @@ SB_FN i32 hb_lsp_quant(i32* lsp) {
     const i16* cb2 = SB_T(hb_lsp_cb2_fix);
     i32 min_dist = SB_I32_MAX; int idx1 = 0;
     for (int i = 0; i < 256; i++) {
-        i32 dist = 0;
-        for (int j = 0; j < HB_ORDER; j++) { i32 t = lsp[j] - cb1[i * HB_ORDER + j]; dist = smlabb(dist, t, t); }
+        const i32 dist = hb_lsp_dist1(lsp, i);
         if (dist < min_dist) { min_dist = dist; idx1 = i; }
     }
     for (int i = 0; i < HB_ORDER; i++) lsp[i] -= cb1[idx1 * HB_ORDER + i];
     i32 best = SB_I32_MAX; int idx2 = 0;
     for (int i = 0; i < 16; i++) {
-        i32 dist = 0;
-        for (int j = 0; j < HB_ORDER; j++) { i32 t = subw(lsp[j], cb2[i * HB_ORDER + j]); dist = smlawb(dist, smulbb(t, t), weight[j]); }
+        const i32 dist = hb_lsp_dist2(lsp, weight, i);
         if (dist < best) { best = dist; idx2 = i; }
     }
     for (int i = 0; i < HB_ORDER; i++) lsp[i] = (i32)cb1[idx1 * HB_ORDER + i] + (i32)cb2[idx2 * HB_ORDER + i];
@@ -197,26 +211,38 @@ struct EncAnalysisWork {
     i16 res_pitch[2 * FRAME + LA_PITCH];
 };
 
+// Start of a frame's analysis (encode_frame_FIX.c:34-75), shared with the core-analysis kernel (c_encode_frame_analysis,
+// sb_coop.cuh): seed, the frame's voice activity (computed ahead by the VAD kernel: speech activity, four band qualities,
+// tilt), high-pass filter of pIn into pIn_HP.
+SB_HD void frame_analysis_begin(EncSilk* st, EncCtrl* c, i16* pIn_HP, const i16* pIn, i32 speech_activity_Q8, const i32* quality_Q15,
+                                i32 tilt_Q15) {
+    c->Seed = st->frameCounter++ & 3;
+    st->speech_activity_Q8 = speech_activity_Q8;
+    for (int b = 0; b < 4; b++) c->input_quality_bands_Q15[b] = quality_Q15[b];
+    c->input_tilt_Q15 = tilt_Q15;
+    hp_variable_cutoff(st, c, pIn_HP, pIn);
+}
+// what the next frame's analysis reads of this one (encode_frame_FIX.c:199-208)
+SB_HD void frame_analysis_end(EncSilk* st, const EncCtrl* c) {
+    st->prev_sigtype = c->sigtype;
+    st->prevLag = c->pitchL[NB_SUBFR - 1];
+    st->first_frame_after_reset = 0;
+}
+
 // SKP_Silk_encode_frame_FIX (encode_frame_FIX.c:34-131) up to the quantised NLSFs, for frame f of the packet: the scalar
 // model of the core-analysis kernel (c_encode_frame_analysis).  Reads the frame's voice activity from scr and writes what
 // the kernel writes there: c[f], x_hp[f], ar_Q24[f], shape_par[f], nlsf_Q15[f], lpc_in_pre[f], local_gains[f].
 SB_FN void encode_frame_analysis(EncSilk* st, EncAnalysisWork* W, EncScratch* scr, int f) {
     EncCtrl* c = &scr->c[f];
     i16* x_frame = st->x_buf + FRAME;
-    c->Seed = st->frameCounter++ & 3;
-    st->speech_activity_Q8 = scr->vad_sa_Q8[f];
-    for (int b = 0; b < 4; b++) c->input_quality_bands_Q15[b] = scr->vad_quality_Q15[f][b];
-    c->input_tilt_Q15 = scr->vad_tilt_Q15[f];
-    hp_variable_cutoff(st, c, W->pIn_HP, W->low + f * FRAME);
+    frame_analysis_begin(st, c, W->pIn_HP, W->low + f * FRAME, scr->vad_sa_Q8[f], scr->vad_quality_Q15[f], scr->vad_tilt_Q15[f]);
     for (int i = 0; i < FRAME; i++) x_frame[LA_SHAPE + i] = W->pIn_HP[i];  // LP_variable_cutoff is a copy (transition_frame_no == 0)
     find_pitch_lags(st, c, W->res_pitch, x_frame);
     noise_shape_analysis(st, c, W->res_pitch + FRAME, x_frame, scr->ar_Q24[f], scr->shape_par[f]);
     find_pred_coefs(st, c, W->res_pitch, scr, f);
     for (int i = 0; i < FRAME; i++) scr->x_hp[f][i] = x_frame[i];    // the prefilter's input: the frame as the analysis saw it
     for (int i = 0; i < FRAME + LA_SHAPE; i++) st->x_buf[i] = st->x_buf[FRAME + i];
-    st->prev_sigtype = c->sigtype;
-    st->prevLag = c->pitchL[NB_SUBFR - 1];
-    st->first_frame_after_reset = 0;
+    frame_analysis_end(st, c);
 }
 
 // scalar model of the core-analysis kernel (c_enc_packet_analysis): every frame of the packet

@@ -162,23 +162,52 @@ SB_FN void vad_flag_and_dtx(EncSilk* st, i32* vadFlag) {
     *vadFlag = st->vadFlag;
 }
 
-// ---- SKP_Silk_pitch_analysis_core.c:680-706 ---------------------------------------------------------
-SB_FN i32 pitch_find_scaling(const i16* signal, int signal_length, int sum_sqr_len) {
-    // int16_array_maxabs (SKP_Silk_array_maxabs.c:40-66)
-    i32 mx = 0; int ind = signal_length - 1;
-    mx = (i32)signal[ind] * (i32)signal[ind];
-    for (int i = signal_length - 2; i >= 0; i--) {
-        i32 lvl = (i32)signal[i] * (i32)signal[i];
-        if (lvl > mx) { mx = lvl; ind = i; }
-    }
-    i32 x_max;
-    if (mx >= 1073676289) x_max = 32767;
-    else x_max = signal[ind] < 0 ? -signal[ind] : signal[ind];
+// The pitch-search arithmetic below is written once for the scalar model and the analysis kernel (c_pitch_analysis_core,
+// c_find_pitch_lags in sb_coop.cuh), which calls it on every lane or on the lane that owns a candidate.
+
+// ---- SKP_Silk_pitch_analysis_core.c:680-706: down-shift of a signal whose largest |x| is x_maxabs ---------------
+SB_HD i32 pitch_find_scaling(i32 x_maxabs, int sum_sqr_len) {
+    // int16_array_maxabs (SKP_Silk_array_maxabs.c:40-66) takes |x| at the largest x^2 and reports 32767 from 1073676289 on
+    const i32 x_max = x_maxabs * x_maxabs >= 1073676289 ? 32767 : x_maxabs;
     i32 nbits;
     if (x_max < 32767) nbits = 32 - clz32(smulbb(x_max, x_max));
     else nbits = 30;
     nbits += 17 - (clz32(sum_sqr_len) - 16);
     return nbits < 31 ? 0 : nbits - 30;
+}
+SB_FN i32 maxabs16(const i16* x, int n) {
+    i32 m = 0;
+    for (int i = 0; i < n; i++) m = imax(m, iabs((i32)x[i]));
+    return m;
+}
+// stage-2 normalised correlation of a target sub-frame and one lag's basis vector (:399-420)
+SB_HD i32 pitch_stage2_corr(i32 cross_corr, i32 energy_target, i32 energy_basis) {
+    if (cross_corr <= 0) return 0;
+    i32 energy = imax(energy_target, energy_basis);
+    int lshift = limit(clz32(cross_corr) - 1, 0, 15);
+    i32 temp32 = shl(cross_corr, lshift) / ((energy >> (15 - lshift)) + 1);
+    temp32 = smulwb(cross_corr, temp32);
+    temp32 = add_sat32(temp32, temp32);
+    lshift = limit(clz32(temp32) - 1, 0, 15);
+    energy = imin(energy_target, energy_basis);
+    return (i16)(shl(temp32, lshift) / ((energy >> (15 - lshift)) + 1));
+}
+// Score of stage-2 candidate lag d, whose best contour CBimax sums to CCmax: the sum less the short-lag bias and the
+// previous-lag bias (:427-455).  SB_I32_MIN if the candidate may not win: its sum is not above the threshold, or the
+// contour's first lag is above the minimum lag.
+SB_HD i32 pitch_lag_score(i32 CCmax, int CBimax, int d, i32 prevLag, i32 LTPCorr_Q15, i32 search_thres2_Q15) {
+    const i32 corr_thres_Q15 = smulbb(search_thres2_Q15, search_thres2_Q15) >> 13;
+    if (CCmax <= corr_thres_Q15 || SB_T(pitch_cb_lags_stage2)[CBimax] > 16) return SB_I32_MIN;
+    const i32 lag_log2_Q7 = lin2log(d);
+    i32 score = CCmax - (smulbb(4 * 6554, lag_log2_Q7) >> 7);
+    if (prevLag > 0) {
+        i32 dl = lag_log2_Q7 - lin2log(prevLag);
+        dl = smulbb(dl, dl) >> 7;
+        i32 prev_lag_bias_Q15 = smulbb(4 * 6554, LTPCorr_Q15) >> 15;
+        prev_lag_bias_Q15 = mulw(prev_lag_bias_Q15, dl) / (dl + (1 << 6));
+        score -= prev_lag_bias_Q15;
+    }
+    return score;
 }
 
 // ---- SKP_Silk_pitch_analysis_core.c:65-560 specialised to Fs = 8 kHz, complexity 2 (stage 3 is skipped
@@ -195,7 +224,7 @@ SB_FN int pitch_analysis_core(const i16* signal, i32* pitch_out, i32* lagIndex, 
     for (int i = 0; i < FL8; i++) signal_8kHz[i] = signal[i];
     resampler_down2(filt_state, signal_4kHz, signal_8kHz, FL8);
     for (int i = FL4 - 1; i > 0; i--) signal_4kHz[i] = (i16)add_sat16(signal_4kHz[i], signal_4kHz[i - 1]);
-    i32 shift = pitch_find_scaling(signal_4kHz, FL4, imax(SF8, FL4 >> 1));
+    i32 shift = pitch_find_scaling(maxabs16(signal_4kHz, FL4), imax(SF8, FL4 >> 1));
     if (shift > 0) for (int i = 0; i < FL4; i++) signal_4kHz[i] = (i16)(signal_4kHz[i] >> shift);
 
     // ---- first stage at 4 kHz ----
@@ -254,7 +283,7 @@ SB_FN int pitch_analysis_core(const i16* signal, i32* pitch_out, i32* lagIndex, 
     }
 
     // ---- second stage at 8 kHz ----
-    shift = pitch_find_scaling(signal_8kHz, FL8, SF8);
+    shift = pitch_find_scaling(maxabs16(signal_8kHz, FL8), SF8);
     if (shift > 0) for (int i = 0; i < FL8; i++) signal_8kHz[i] = (i16)(signal_8kHz[i] >> shift);
     for (int k = 0; k < 4; k++) for (int i = 0; i < CW; i++) C[k][i] = 0;
     target_ptr = &signal_8kHz[FL4];
@@ -263,29 +292,12 @@ SB_FN int pitch_analysis_core(const i16* signal, i32* pitch_out, i32* lagIndex, 
         for (int j = 0; j < length_d_comp; j++) {
             int d = d_comp[j];
             const i16* basis_ptr = target_ptr - d;
-            i32 cross_corr = inner_prod16(target_ptr, basis_ptr, SF8);
-            i32 energy_basis = inner_prod16(basis_ptr, basis_ptr, SF8);
-            if (cross_corr > 0) {
-                energy = imax(energy_target, energy_basis);
-                int lz = clz32(cross_corr);
-                int lshift = limit(lz - 1, 0, 15);
-                i32 temp32 = shl(cross_corr, lshift) / ((energy >> (15 - lshift)) + 1);
-                temp32 = smulwb(cross_corr, temp32);
-                temp32 = add_sat32(temp32, temp32);
-                lz = clz32(temp32);
-                lshift = limit(lz - 1, 0, 15);
-                energy = imin(energy_target, energy_basis);
-                C[k][d] = (i16)(shl(temp32, lshift) / ((energy >> (15 - lshift)) + 1));
-            } else {
-                C[k][d] = 0;
-            }
+            C[k][d] = (i16)pitch_stage2_corr(inner_prod16(target_ptr, basis_ptr, SF8), energy_target, inner_prod16(basis_ptr, basis_ptr, SF8));
         }
         target_ptr += SF8;
     }
     i32 CCmax = SB_I32_MIN, CCmax_b = SB_I32_MIN;
     int CBimax = 0, lag = -1;
-    i32 prevLag_log2_Q7 = prevLag > 0 ? lin2log(prevLag) : 0;
-    i32 corr_thres_Q15 = smulbb(search_thres2_Q15, search_thres2_Q15) >> 13;
     const i16* cbl = SB_T(pitch_cb_lags_stage2);  // [4][11]
     for (int k = 0; k < length_d_srch; k++) {
         int d = d_srch[k];
@@ -296,18 +308,8 @@ SB_FN int pitch_analysis_core(const i16* signal, i32* pitch_out, i32* lagIndex, 
         }
         i32 CCmax_new = SB_I32_MIN; int CBimax_new = 0;
         for (int i = 0; i < NCB; i++) if (CC[i] > CCmax_new) { CCmax_new = CC[i]; CBimax_new = i; }
-        i32 lag_log2_Q7 = lin2log(d);
-        i32 CCmax_new_b = CCmax_new - (smulbb(4 * 6554, lag_log2_Q7) >> 7);
-        if (prevLag > 0) {
-            i32 dl = lag_log2_Q7 - prevLag_log2_Q7;
-            dl = smulbb(dl, dl) >> 7;
-            i32 prev_lag_bias_Q15 = smulbb(4 * 6554, *LTPCorr_Q15) >> 15;
-            prev_lag_bias_Q15 = mulw(prev_lag_bias_Q15, dl) / (dl + (1 << 6));
-            CCmax_new_b -= prev_lag_bias_Q15;
-        }
-        if (CCmax_new_b > CCmax_b && CCmax_new > corr_thres_Q15 && cbl[0 * NCB + CBimax_new] <= MINL8) {
-            CCmax_b = CCmax_new_b; CCmax = CCmax_new; lag = d; CBimax = CBimax_new;
-        }
+        const i32 CCmax_new_b = pitch_lag_score(CCmax_new, CBimax_new, d, prevLag, *LTPCorr_Q15, search_thres2_Q15);
+        if (CCmax_new_b > CCmax_b) { CCmax_b = CCmax_new_b; CCmax = CCmax_new; lag = d; CBimax = CBimax_new; }
     }
     if (lag == -1) {
         for (int k = 0; k < 4; k++) pitch_out[k] = 0;
@@ -323,6 +325,17 @@ SB_FN int pitch_analysis_core(const i16* signal, i32* pitch_out, i32* lagIndex, 
 }
 
 // ---- SKP_Silk_find_pitch_lags_FIX.c:32-125 -----------------------------------------------------------
+// prediction gain of the order-10 whitening filter from the regularised energy and Schur's residual energy (:86-88)
+SB_HD i32 pitch_pred_gain_q16(i32 auto_corr0, i32 res_nrg) { return div32_varq(auto_corr0, imax(res_nrg, 1), 16); }
+// voicing threshold of the pitch search, order 10 (:108-115)
+SB_HD i32 pitch_thrhld_q15(i32 speech_activity_Q8, i32 prev_sigtype, i32 input_tilt_Q15) {
+    i32 thrhld_Q15 = SB_FIXC(0.45, 15);
+    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.004, 15), 10);
+    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.1, 7), speech_activity_Q8);
+    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(0.15, 15), prev_sigtype);
+    thrhld_Q15 = smlawb(thrhld_Q15, SB_FIXC(-0.1, 16), input_tilt_Q15);
+    return (i16)sat16(thrhld_Q15);
+}
 // x points at x_buf + FRAME (start of the frame to encode); res receives 336 samples of LPC residual.
 SB_FN void find_pitch_lags(EncSilk* st, EncCtrl* c, i16* res, const i16* x) {
     enum { BUF_LEN = LA_PITCH + 2 * FRAME, ORD = 10 };
@@ -340,20 +353,14 @@ SB_FN void find_pitch_lags(EncSilk* st, EncCtrl* c, i16* res, const i16* x) {
     autocorr(auto_corr, &scale, Wsig, PITCH_LPC_WIN, ORD + 1);
     auto_corr[0] = smlawb(auto_corr[0], auto_corr[0], SB_FIXC(1e-3f, 16));
     i32 res_nrg = schur(rc_Q15, auto_corr, ORD);
-    c->predGain_Q16 = div32_varq(auto_corr[0], imax(res_nrg, 1), 16);
+    c->predGain_Q16 = pitch_pred_gain_q16(auto_corr[0], res_nrg);
     k2a(A_Q24, rc_Q15, ORD);
     for (int i = 0; i < ORD; i++) A_Q12[i] = (i16)sat16(A_Q24[i] >> 12);
     bwexpander(A_Q12, ORD, SB_FIXC(0.99f, 16));
     ma_prediction_zero_state(x_buf, A_Q12, res, BUF_LEN, ORD);
     for (int i = 0; i < ORD; i++) res[i] = 0;
-    i32 thrhld_Q15 = SB_FIXC(0.45, 15);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.004, 15), ORD);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(-0.1, 7), st->speech_activity_Q8);
-    thrhld_Q15 = smlabb(thrhld_Q15, SB_FIXC(0.15, 15), st->prev_sigtype);
-    thrhld_Q15 = smlawb(thrhld_Q15, SB_FIXC(-0.1, 16), c->input_tilt_Q15);
-    thrhld_Q15 = sat16(thrhld_Q15);
-    c->sigtype = pitch_analysis_core(res, c->pitchL, &c->lagIndex, &c->contourIndex, &st->LTPCorr_Q15, st->prevLag,
-                                     SB_FIXC(0.7f, 16), (i16)thrhld_Q15);
+    c->sigtype = pitch_analysis_core(res, c->pitchL, &c->lagIndex, &c->contourIndex, &st->LTPCorr_Q15, st->prevLag, SB_FIXC(0.7f, 16),
+                                     pitch_thrhld_q15(st->speech_activity_Q8, st->prev_sigtype, c->input_tilt_Q15));
 }
 
 }  // namespace sb

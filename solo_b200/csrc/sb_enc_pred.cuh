@@ -348,27 +348,48 @@ SB_FN void ltp_scale_ctrl(EncSilk* st, EncCtrl* c, int frame_in_packet) {
 }
 
 // ---- SKP_Silk_LTP_analysis_filter_FIX.c:30-80 --------------------------------------------------------------
-SB_FN void ltp_analysis_filter(i16* LTP_res, const i16* x, const i16* LTPCoef_Q14, const i32* pitchL, const i32* invGains_Q16) {
-    const int pre = LPC_ORDER;
-    const i16* x_ptr = x;
-    i16* out = LTP_res;
-    for (int k = 0; k < NB_SUBFR; k++) {
-        const i16* x_lag_ptr = x_ptr - pitchL[k];
-        const i16* B = &LTPCoef_Q14[k * LTP_ORDER];
-        for (int i = 0; i < SUBFR + pre; i++) {
-            i32 est = smulbb(x_lag_ptr[LTP_ORDER / 2], B[0]);
-            for (int j = 1; j < LTP_ORDER; j++) est = smlabb(est, x_lag_ptr[LTP_ORDER / 2 - j], B[j]);
-            est = rshift_round(est, 14);
-            i32 r = sat16((i32)x_ptr[i] - est);
-            out[i] = (i16)smulwb(invGains_Q16[k], r);
-            x_lag_ptr++;
-        }
-        out += SUBFR + pre;
-        x_ptr += SUBFR;
-    }
+// Output i of sub-frame k's block of SUBFR + LPC_ORDER samples, x pointing at the first block's start: the LTP residual
+// scaled by the sub-frame's inverse gain.  The analysis kernel computes one output per lane (c_find_pred_coefs).
+SB_HD i16 ltp_analysis_sample(const i16* x, const i16* LTPCoef_Q14, const i32* pitchL, const i32* invGains_Q16, int k, int i) {
+    const i16* x_ptr = x + k * SUBFR;
+    const i16* x_lag_ptr = x_ptr - pitchL[k] + i;
+    const i16* B = &LTPCoef_Q14[k * LTP_ORDER];
+    i32 est = smulbb(x_lag_ptr[LTP_ORDER / 2], B[0]);
+#pragma unroll
+    for (int j = 1; j < LTP_ORDER; j++) est = smlabb(est, x_lag_ptr[LTP_ORDER / 2 - j], B[j]);
+    est = rshift_round(est, 14);
+    const i32 r = sat16((i32)x_ptr[i] - est);
+    return (i16)smulwb(invGains_Q16[k], r);
 }
 
 // ---- SKP_Silk_find_LPC_FIX.c:32-148 --------------------------------------------------------------------
+// The energy comparisons are written once for this scalar model and the analysis kernel (c_find_lpc, sb_coop.cuh).
+// Residual energy of the first half: the whole frame's less the second half's, in the coarser of the two Q-domains (:83-93).
+SB_HD void lpc_first_half_nrg(i32& res_nrg, i32& res_nrg_Q, i32 res_tmp_nrg, i32 res_tmp_nrg_Q) {
+    const int shift = res_tmp_nrg_Q - res_nrg_Q;
+    if (shift >= 0) {
+        if (shift < 32) res_nrg = subw(res_nrg, res_tmp_nrg >> shift);
+    } else {
+        res_nrg = subw(res_nrg >> (-shift), res_tmp_nrg);
+        res_nrg_Q = res_tmp_nrg_Q;
+    }
+}
+// Interpolation candidate with half-frame residual energies res_nrg0 / res_nrg1 (right shifts rshift0 / rshift1): true,
+// and its energy becomes the best, if it is lower than the best so far (:119-140).
+SB_HD bool lpc_interp_lower(i32& res_nrg, i32& res_nrg_Q, i32 res_nrg0, i32 rshift0, i32 res_nrg1, i32 rshift1) {
+    i32 res_nrg_interp_Q;
+    int shift = rshift0 - rshift1;
+    if (shift >= 0) { res_nrg1 = res_nrg1 >> shift; res_nrg_interp_Q = -rshift0; }
+    else { res_nrg0 = res_nrg0 >> (-shift); res_nrg_interp_Q = -rshift1; }
+    const i32 res_nrg_interp = addw(res_nrg0, res_nrg1);
+    shift = res_nrg_interp_Q - res_nrg_Q;
+    bool lower;
+    if (shift >= 0) lower = (res_nrg_interp >> shift) < res_nrg;
+    else if (-shift < 32) lower = res_nrg_interp < (res_nrg >> (-shift));
+    else lower = false;
+    if (lower) { res_nrg = res_nrg_interp; res_nrg_Q = res_nrg_interp_Q; }
+    return lower;
+}
 // x: nb_subfr blocks of subfr_length samples (each with `order` preceding samples); x is 4-byte aligned.
 SB_FN void find_lpc(i32* NLSF_Q15, i32* interpIndex, const i32* prev_NLSFq_Q15, int useInterp, int order, const i16* x,
                     int subfr_length) {
@@ -384,13 +405,7 @@ SB_FN void find_lpc(i32* NLSF_Q15, i32* interpIndex, const i32* prev_NLSFq_Q15, 
         burg_modified(&res_tmp_nrg, &res_tmp_nrg_Q, a_tmp_Q16, x + (NB_SUBFR >> 1) * subfr_length, subfr_length, NB_SUBFR >> 1,
                       SB_FIXC(2.5e-5f, 32), order);
         bwexpander_32(a_tmp_Q16, order, SB_FIXC(0.99995f, 16));
-        int shift = res_tmp_nrg_Q - res_nrg_Q;
-        if (shift >= 0) {
-            if (shift < 32) res_nrg = subw(res_nrg, res_tmp_nrg >> shift);
-        } else {
-            res_nrg = subw(res_nrg >> (-shift), res_tmp_nrg);
-            res_nrg_Q = res_tmp_nrg_Q;
-        }
+        lpc_first_half_nrg(res_nrg, res_nrg_Q, res_tmp_nrg, res_tmp_nrg_Q);
         a2nlsf(NLSF_Q15, a_tmp_Q16, order);
         for (int k = 3; k >= 0; k--) {
             interpolate(NLSF0_Q15, prev_NLSFq_Q15, NLSF_Q15, k, order);
@@ -399,17 +414,7 @@ SB_FN void find_lpc(i32* NLSF_Q15, i32* interpIndex, const i32* prev_NLSFq_Q15, 
             i32 res_nrg0, res_nrg1, rshift0, rshift1;
             sum_sqr_shift(&res_nrg0, &rshift0, LPC_res + order, subfr_length - order, order & 1);
             sum_sqr_shift(&res_nrg1, &rshift1, LPC_res + order + subfr_length, subfr_length - order, (order + subfr_length) & 1);
-            i32 res_nrg_interp_Q;
-            shift = rshift0 - rshift1;
-            if (shift >= 0) { res_nrg1 = res_nrg1 >> shift; res_nrg_interp_Q = -rshift0; }
-            else { res_nrg0 = res_nrg0 >> (-shift); res_nrg_interp_Q = -rshift1; }
-            i32 res_nrg_interp = addw(res_nrg0, res_nrg1);
-            shift = res_nrg_interp_Q - res_nrg_Q;
-            int lower;
-            if (shift >= 0) lower = (res_nrg_interp >> shift) < res_nrg;
-            else if (-shift < 32) lower = res_nrg_interp < (res_nrg >> (-shift));
-            else lower = 0;
-            if (lower) { res_nrg = res_nrg_interp; res_nrg_Q = res_nrg_interp_Q; *interpIndex = k; }
+            if (lpc_interp_lower(res_nrg, res_nrg_Q, res_nrg0, rshift0, res_nrg1, rshift1)) *interpIndex = k;
         }
     }
     if (*interpIndex == 4) a2nlsf(NLSF_Q15, a_Q16, order);
@@ -564,31 +569,45 @@ SB_FN void nlsf_fast_tabs_fill(NlsfFastTabs* T, int tid, int nthreads) {
     for (int i = tid; i < 720; i += nthreads) T->cb1[i] = SB_T(nlsf_cb1_q15)[i];
     for (int i = tid; i < 72; i += nthreads) T->rates1[i] = SB_T(nlsf_cb1_rates_q5)[i];
 }
+// The rules below are written once for this scalar model and the analysis kernel (c_process_nlsfs, sb_coop.cuh).
+// rate weight and fluctuation-reduction weight of the NLSF quantiser (:52-63)
+SB_HD void nlsf_mu(i32& NLSF_mu_Q15, i32& NLSF_mu_fluc_red_Q16, int sigtype, i32 speech_activity_Q8, i32 sparseness_Q8) {
+    if (sigtype == 0) {
+        NLSF_mu_Q15 = smlawb(66, -8388, speech_activity_Q8);
+        NLSF_mu_fluc_red_Q16 = smlawb(6554, -838848, speech_activity_Q8);
+    } else {
+        NLSF_mu_Q15 = smlawb(164, -33554, speech_activity_Q8);
+        NLSF_mu_fluc_red_Q16 = smlawb(13107, -1677696, speech_activity_Q8 + sparseness_Q8);
+    }
+    NLSF_mu_Q15 = imax(NLSF_mu_Q15, 1);
+}
+// one Laroia weight of the target NLSFs, w_Q6, merged with that of the first half's interpolated NLSFs, w0_Q6 (:71-82)
+SB_HD i32 nlsf_interp_weight_q6(i32 w_Q6, i32 w0_Q6, int interpQ2) {
+    return smlawb(w_Q6 >> 1, w0_Q6, shl(smulbb(interpQ2, interpQ2), 11));
+}
+// one quantised NLSF of the first half-frame: interpolated from the previous frame's unless interpQ2 == 4 (:108-118)
+SB_HD i32 nlsf_first_half_q15(i32 prev_Q15, i32 q_Q15, int interpQ2) {
+    return interpQ2 < (1 << 2) ? prev_Q15 + (mulw(q_Q15 - prev_Q15, interpQ2) >> 2) : q_Q15;
+}
 // Up to the quantised NLSFs of the two half-frames, nlsf_out = {interpolated first half, second half}; gains_packet turns
 // them into the prediction filters (:108-127).
 SB_FN void process_nlsfs(EncSilk* st, EncCtrl* c, i32* pNLSF_Q15, i32 (*nlsf_out)[LPC_ORDER]) {
     i32 pNLSFW_Q6[LPC_ORDER], pNLSF0_temp_Q15[LPC_ORDER], pNLSFW0_temp_Q6[LPC_ORDER];
     i32 NLSF_mu_Q15, NLSF_mu_fluc_red_Q16;
-    if (c->sigtype == 0) {
-        NLSF_mu_Q15 = smlawb(66, -8388, st->speech_activity_Q8);
-        NLSF_mu_fluc_red_Q16 = smlawb(6554, -838848, st->speech_activity_Q8);
-    } else {
-        NLSF_mu_Q15 = smlawb(164, -33554, st->speech_activity_Q8);
-        NLSF_mu_fluc_red_Q16 = smlawb(13107, -1677696, st->speech_activity_Q8 + c->sparseness_Q8);
-    }
-    NLSF_mu_Q15 = imax(NLSF_mu_Q15, 1);
+    nlsf_mu(NLSF_mu_Q15, NLSF_mu_fluc_red_Q16, c->sigtype, st->speech_activity_Q8, c->sparseness_Q8);
     nlsf_vq_weights_laroia(pNLSFW_Q6, pNLSF_Q15, LPC_ORDER);
-    int doInterpolate = c->NLSFInterpCoef_Q2 < (1 << 2);
-    if (doInterpolate) {
-        interpolate(pNLSF0_temp_Q15, st->prev_NLSFq_Q15, pNLSF_Q15, c->NLSFInterpCoef_Q2, LPC_ORDER);
+    const int interpQ2 = c->NLSFInterpCoef_Q2;
+    if (interpQ2 < (1 << 2)) {
+        interpolate(pNLSF0_temp_Q15, st->prev_NLSFq_Q15, pNLSF_Q15, interpQ2, LPC_ORDER);
         nlsf_vq_weights_laroia(pNLSFW0_temp_Q6, pNLSF0_temp_Q15, LPC_ORDER);
-        i32 i_sqr_Q15 = shl(smulbb(c->NLSFInterpCoef_Q2, c->NLSFInterpCoef_Q2), 11);
-        for (int i = 0; i < LPC_ORDER; i++) pNLSFW_Q6[i] = smlawb(pNLSFW_Q6[i] >> 1, pNLSFW0_temp_Q6[i], i_sqr_Q15);
+        for (int i = 0; i < LPC_ORDER; i++) pNLSFW_Q6[i] = nlsf_interp_weight_q6(pNLSFW_Q6[i], pNLSFW0_temp_Q6[i], interpQ2);
     }
     nlsf_msvq_encode(c->NLSFIndices, pNLSF_Q15, nlsf_cb(c->sigtype), st->prev_NLSFq_Q15, pNLSFW_Q6, NLSF_mu_Q15, NLSF_mu_fluc_red_Q16,
                      st->first_frame_after_reset);
-    for (int i = 0; i < LPC_ORDER; i++) nlsf_out[0][i] = nlsf_out[1][i] = pNLSF_Q15[i];
-    if (doInterpolate) interpolate(nlsf_out[0], st->prev_NLSFq_Q15, pNLSF_Q15, c->NLSFInterpCoef_Q2, LPC_ORDER);
+    for (int i = 0; i < LPC_ORDER; i++) {
+        nlsf_out[1][i] = pNLSF_Q15[i];
+        nlsf_out[0][i] = nlsf_first_half_q15(st->prev_NLSFq_Q15[i], pNLSF_Q15[i], interpQ2);
+    }
 }
 
 // ---- SKP_Silk_residual_energy_FIX.c:32-92 ------------------------------------------------------------------
@@ -625,6 +644,7 @@ SB_FN void find_pred_coefs(EncSilk* st, EncCtrl* c, const i16* res_pitch, EncScr
     i32 NLSF_Q15[LPC_ORDER];
     i32* local_gains = scr->local_gains[frame_in_packet];
     i16* LPC_in_pre = scr->lpc_in_pre[frame_in_packet];
+    // (the analysis kernel states this step separately: as a shared helper it grows the kernel's spill traffic)
     i32 min_gain_Q16 = SB_I32_MAX >> 6;
     for (int i = 0; i < NB_SUBFR; i++) min_gain_Q16 = imin(min_gain_Q16, c->Gains_Q16[i]);
     for (int i = 0; i < NB_SUBFR; i++) {
@@ -638,7 +658,9 @@ SB_FN void find_pred_coefs(EncSilk* st, EncCtrl* c, const i16* res_pitch, EncScr
         find_ltp(c->LTPCoef_Q14, WLTP, &c->LTPredCodGain_Q7, res_pitch, res_pitch + (FRAME >> 1), c->pitchL, Wght_Q15, LTP_corrs_rshift);
         quant_ltp_gains(c->LTPCoef_Q14, c->LTPIndex, &c->PERIndex, WLTP, SB_FIXC(0.03f, 8));
         ltp_scale_ctrl(st, c, frame_in_packet);
-        ltp_analysis_filter(LPC_in_pre, st->x_buf + FRAME - LPC_ORDER, c->LTPCoef_Q14, c->pitchL, invGains_Q16);
+        for (int k = 0; k < NB_SUBFR; k++)
+            for (int i = 0; i < SUBFR + LPC_ORDER; i++)
+                LPC_in_pre[k * (SUBFR + LPC_ORDER) + i] = ltp_analysis_sample(st->x_buf + FRAME - LPC_ORDER, c->LTPCoef_Q14, c->pitchL, invGains_Q16, k, i);
     } else {
         const i16* x_ptr = st->x_buf + FRAME - LPC_ORDER;
         i16* x_pre_ptr = LPC_in_pre;

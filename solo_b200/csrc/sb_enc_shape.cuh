@@ -33,15 +33,6 @@ SB_FN void warped_autocorrelation(i32* corr, i32* scale, const i16* input, i32 w
     else for (int i = 0; i < order + 1; i++) corr[i] = (i32)(corr_QC[i] >> (-lsh));
 }
 
-// ---- SKP_Silk_noise_shape_analysis_FIX.c:33-50 ----------------------------------------------------------
-SB_FN i32 warped_gain(const i32* coefs_Q24, i32 lambda_Q16, int order) {
-    lambda_Q16 = -lambda_Q16;
-    i32 gain_Q24 = coefs_Q24[order - 1];
-    for (int i = order - 2; i >= 0; i--) gain_Q24 = smlawb(coefs_Q24[i], gain_Q24, lambda_Q16);
-    gain_Q24 = smlawb(SB_FIXC(1.0, 24), gain_Q24, -lambda_Q16);
-    return inverse32_varq(gain_Q24, 40);
-}
-
 // ---- SKP_Silk_noise_shape_analysis_FIX.c:52-132 -----------------------------------------------------------
 SB_FN void limit_warped_coefs(i32* syn_Q24, i32* ana_Q24, i32 lambda_Q16, i32 limit_Q24, int order) {
     int ind = 0;
@@ -105,47 +96,147 @@ SB_FN void limit_warped_coefs(i32* syn_Q24, i32* ana_Q24, i32 lambda_Q16, i32 li
 }
 
 // ---- SKP_Silk_noise_shape_analysis_FIX.c:137-531 ---------------------------------------------------------
+// The per-frame control arithmetic below is written once for the scalar model and the analysis kernel
+// (c_noise_shape_analysis, sb_coop.cuh), which calls it on every lane or on the lane that owns sub-frame / window k.
+
+// Frame-level control: SNR adjustment, sparseness (unvoiced: energy_variation_Q7 of the residual's ten 2 ms energies),
+// bandwidth expansion and warping (:155-268).
+struct ShapeCtl {
+    i32 input_quality_Q14, coding_quality_Q14, SNR_adj_dB_Q7, md_SNR_adj_dB_Q7, sparseness_Q8, QuantOffsetType;
+    i32 BWExp1_Q16, BWExp2_Q16, warping_Q16;
+};
+SB_HD ShapeCtl shape_control(int sigtype, i32 SNR_dB_Q7, i32 SNRPerMD_dB_Q7, const i32* input_quality_bands_Q15,
+                             i32 speech_activity_Q8, i32 LTPCorr_Q15, i32 energy_variation_Q7, i32 predGain_Q16) {
+    ShapeCtl s;
+    // inBandFEC_SNR_comp_Q8 == 0 (LBRR off)
+    s.input_quality_Q14 = (input_quality_bands_Q15[0] + input_quality_bands_Q15[1]) >> 2;
+    s.coding_quality_Q14 = sigm_q15(rshift_round(SNR_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
+    const i32 md_input_quality_Q14 = sigm_q15(rshift_round(SNRPerMD_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
+    i32 b_Q8 = SB_FIXC(1.0, 8) - speech_activity_Q8;
+    b_Q8 = smulwb(shl(b_Q8, 8), b_Q8);
+    auto snr_adj = [&](i32 snr_Q7, i32 quality_Q14) {
+        const i32 a = smlawb(snr_Q7, smulbb(SB_FIXC(-4.0f, 7) >> (4 + 1), b_Q8), smulwb(SB_FIXC(1.0, 14) + quality_Q14, s.coding_quality_Q14));
+        if (sigtype == 0) return smlawb(a, SB_FIXC(2.0f, 8), LTPCorr_Q15);
+        return smlawb(a, smlawb(SB_FIXC(6.0, 9), -SB_FIXC(0.4, 18), snr_Q7), SB_FIXC(1.0, 14) - s.input_quality_Q14);
+    };
+    s.SNR_adj_dB_Q7 = snr_adj(SNR_dB_Q7, s.input_quality_Q14);
+    s.md_SNR_adj_dB_Q7 = snr_adj(SNRPerMD_dB_Q7, md_input_quality_Q14);
+    s.sparseness_Q8 = 0;
+    s.QuantOffsetType = 0;
+    if (sigtype != 0) {
+        s.sparseness_Q8 = sigm_q15(smulwb(energy_variation_Q7 - SB_FIXC(5.0, 7), SB_FIXC(0.1, 16))) >> 7;
+        s.QuantOffsetType = s.sparseness_Q8 > SB_FIXC(0.75f, 8) ? 0 : 1;
+        s.SNR_adj_dB_Q7 = smlawb(s.SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), s.sparseness_Q8 - SB_FIXC(0.5, 8));
+        s.md_SNR_adj_dB_Q7 = smlawb(s.md_SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), s.sparseness_Q8 - SB_FIXC(0.5, 8));
+    }
+    const i32 strength_Q16 = smulwb(predGain_Q16, SB_FIXC(1e-3f, 16));
+    s.BWExp1_Q16 = s.BWExp2_Q16 = div32_varq(SB_FIXC(0.95f, 16), smlaww(SB_FIXC(1.0, 16), strength_Q16, strength_Q16), 16);
+    const i32 delta_Q16 = smulwb(SB_FIXC(1.0, 16) - smulbb(3, s.coding_quality_Q14), SB_FIXC(0.01f, 16));
+    s.BWExp1_Q16 = subw(s.BWExp1_Q16, delta_Q16);
+    s.BWExp2_Q16 = addw(s.BWExp2_Q16, delta_Q16);
+    s.BWExp1_Q16 = shl(s.BWExp1_Q16, 14) / (s.BWExp2_Q16 >> 2);
+    s.warping_Q16 = smlawb(WARPING_Q16, s.coding_quality_Q14, SB_FIXC(0.01, 18));
+    return s;
+}
+
+// One window's shaping filters from its warped autocorrelation (Q-domain exponent `scale`; auto_corr is overwritten):
+// regularisation, Schur, step-up, warped gain, AR2 = bandwidth expansion BWExp2, AR1 = AR2 expanded by BWExp1 (:300-344).
+// Returns the window's gain before the frame-level tweaks.
+SB_HD i32 shape_window(i32 (&AR2_Q24)[SHAPE_ORDER], i32 (&AR1_Q24)[SHAPE_ORDER], i32 (&auto_corr)[SHAPE_ORDER + 1], i32 scale,
+                       i32 warping_Q16, i32 BWExp1_Q16, i32 BWExp2_Q16) {
+    i32 refl_coef_Q16[SHAPE_ORDER];
+    auto_corr[0] = addw(auto_corr[0], imax(smulwb(auto_corr[0] >> 4, SB_FIXC(1e-5f, 20)), 1));
+    i32 nrg = schur64_r<SHAPE_ORDER>(refl_coef_Q16, auto_corr);
+    k2a_q16_r<SHAPE_ORDER>(AR2_Q24, refl_coef_Q16);
+    int Qnrg = -scale;
+    if (Qnrg & 1) { Qnrg -= 1; nrg >>= 1; }
+    const i32 tmp32 = sqrt_approx(nrg);
+    Qnrg >>= 1;
+    i32 gain_Q16 = lshift_sat32(tmp32, 16 - Qnrg);
+    {   // warped_gain (:33-50)
+        const i32 lambda_Q16 = -warping_Q16;
+        i32 gain_Q24 = AR2_Q24[SHAPE_ORDER - 1];
+#pragma unroll
+        for (int i = SHAPE_ORDER - 2; i >= 0; i--) gain_Q24 = smlawb(AR2_Q24[i], gain_Q24, lambda_Q16);
+        gain_Q24 = smlawb(SB_FIXC(1.0, 24), gain_Q24, -lambda_Q16);
+        gain_Q16 = smulww(gain_Q16, inverse32_varq(gain_Q24, 40));
+    }
+    if (gain_Q16 < 0) gain_Q16 = SB_I32_MAX;
+    bwexpander_32_r<SHAPE_ORDER>(AR2_Q24, BWExp2_Q16);
+#pragma unroll
+    for (int i = 0; i < SHAPE_ORDER; i++) AR1_Q24[i] = AR2_Q24[i];
+    bwexpander_32_r<SHAPE_ORDER>(AR1_Q24, BWExp1_Q16);
+    return gain_Q16;
+}
+
+// gain tweaking (:346-384): the SNR-dependent multiplier, the offset that follows the running average, one gain
+SB_HD i32 shape_gain_mult_q16(i32 SNR_adj_dB_Q7) { return log2lin(negw(smlawb(-SB_FIXC(16.0, 7), SNR_adj_dB_Q7, SB_FIXC(0.16, 16)))); }
+SB_HD i32 shape_gain_add_q16(i32 avgGain_Q16) {
+    const i32 gain_add_Q16 = log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(4.0f, 7), SB_FIXC(0.16, 16)));
+    return add_sat32(gain_add_Q16, smulww(avgGain_Q16, log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(-50.0f, 7), SB_FIXC(0.16, 16)))));
+}
+SB_HD i32 shape_gain_tweak(i32 gain_Q16, i32 gain_mult_Q16, i32 gain_add_Q16) {
+    gain_Q16 = smulww(gain_Q16, gain_mult_Q16);
+    if (gain_Q16 < 0) gain_Q16 = SB_I32_MAX;
+    return add_pos_sat32(gain_Q16, gain_add_Q16);
+}
+// the running average after one sub-frame's tweaked gain
+SB_HD i32 shape_avg_gain_q16(i32 avgGain_Q16, i32 gain_Q16, i32 speech_activity_Q8) {
+    return add_sat32(avgGain_Q16, smulwb(gain_Q16 - avgGain_Q16, rshift_round(smulbb(speech_activity_Q8, SB_FIXC(1e-3f, 10)), 2)));
+}
+// de-essing factor: fs == 8 kHz takes no branch (:438-457), so it is the pre-gain multiplier alone
+SB_HD i32 shape_pregain_mult_q16(i32 coding_quality_Q14) {
+    return SB_FIXC(1.0, 16) + rshift_round(mlaw(SB_FIXC(0.05f, 26), coding_quality_Q14, SB_FIXC(0.1f, 12)), 10);
+}
+// low-frequency shaping of a sub-frame with pitch lag pitchL (voiced; the same for every sub-frame when unvoiced) (:459-477)
+SB_HD i32 shape_lf_shp_q14(int sigtype, i32 pitchL, i32 input_quality_band0_Q15) {
+    const i32 strength_Q16 = mulw(SB_FIXC(3.0f, 0), SB_FIXC(1.0, 16) + smulbb(SB_FIXC(0.5f, 1), input_quality_band0_Q15 - SB_FIXC(1.0, 15)));
+    i32 b_Q14, LF_shp_Q14;
+    if (sigtype == 0) {
+        b_Q14 = SB_FIXC(0.2, 14) / 8 + SB_FIXC(3.0, 14) / imax(pitchL, 1);
+        LF_shp_Q14 = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, b_Q14), 16);
+    } else {
+        b_Q14 = 21299 / 8;
+        LF_shp_Q14 = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, smulwb(SB_FIXC(0.6, 16), b_Q14)), 16);
+    }
+    return LF_shp_Q14 | (u16)(b_Q14 - SB_FIXC(1.0, 14));
+}
+// targets of the three smoothed shaping parameters (:470-505)
+struct HarmTilt { i32 HarmBoost_Q16, HarmShapeGain_Q16, Tilt_Q16; };
+SB_HD HarmTilt shape_harm_tilt(int sigtype, i32 speech_activity_Q8, i32 input_quality_Q14, i32 coding_quality_Q14, i32 LTPCorr_Q15) {
+    HarmTilt h;
+    h.HarmBoost_Q16 = smulwb(smulwb(SB_FIXC(1.0, 17) - shl(coding_quality_Q14, 3), LTPCorr_Q15), SB_FIXC(0.1f, 16));
+    h.HarmBoost_Q16 = smlawb(h.HarmBoost_Q16, SB_FIXC(1.0, 16) - shl(input_quality_Q14, 2), SB_FIXC(0.1f, 16));
+    h.HarmShapeGain_Q16 = 0;
+    h.Tilt_Q16 = -SB_FIXC(0.3f, 16);
+    if (sigtype == 0) {
+        h.Tilt_Q16 -= smulwb(SB_FIXC(1.0, 16) - SB_FIXC(0.3f, 16), smulwb(SB_FIXC(0.35f, 24), speech_activity_Q8));
+        h.HarmShapeGain_Q16 = smlawb(SB_FIXC(0.3f, 16),
+            SB_FIXC(1.0, 16) - smulwb(SB_FIXC(1.0, 18) - shl(coding_quality_Q14, 4), input_quality_Q14), SB_FIXC(0.2f, 16));
+        h.HarmShapeGain_Q16 = smulwb(shl(h.HarmShapeGain_Q16, 1), sqrt_approx(shl(LTPCorr_Q15, 15)));
+    }
+    return h;
+}
+// one sub-frame step of a smoothed parameter (state Q16) towards its target; returns the sub-frame's Q14 value
+SB_HD i32 shape_smooth_q14(i32& smth_Q16, i32 target_Q16) {
+    smth_Q16 = smlawb(smth_Q16, target_Q16 - smth_Q16, SB_FIXC(0.4f, 16));
+    return rshift_round(smth_Q16, 2);
+}
+
 // pitch_res points at res_pitch + FRAME, x at x_buf + FRAME.  Stops, as the analysis kernel does, after the bandwidth
 // expansion of each window: ar_Q24[k] = {AR2, AR1} and shape_par = {warping_Q16, de-essing multiplier Q16} go to
 // shape_post_window, which finishes the filters and the pre-gains.
 SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, const i16* x, i32 (*ar_Q24)[2][SHAPE_ORDER], i32* shape_par) {
-    i32 auto_corr[SHAPE_ORDER + 1], refl_coef_Q16[SHAPE_ORDER], AR1_Q24[SHAPE_ORDER], AR2_Q24[SHAPE_ORDER];
+    i32 auto_corr[SHAPE_ORDER + 1], AR1_Q24[SHAPE_ORDER], AR2_Q24[SHAPE_ORDER];
     i16 x_windowed[SHAPE_WIN];
     i32 scale = 0, nrg;
     const i16* x_ptr = x - LA_SHAPE;
 
-    c->current_SNR_dB_Q7 = st->SNR_dB_Q7;
-    c->current_SNRPerMD_dB_Q7 = st->SNRPerMD_dB_Q7;
-    // inBandFEC_SNR_comp_Q8 == 0 (LBRR off)
-    c->input_quality_Q14 = (c->input_quality_bands_Q15[0] + c->input_quality_bands_Q15[1]) >> 2;
-    c->coding_quality_Q14 = sigm_q15(rshift_round(c->current_SNR_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
-    i32 b_Q8 = SB_FIXC(1.0, 8) - st->speech_activity_Q8;
-    b_Q8 = smulwb(shl(b_Q8, 8), b_Q8);
-    i32 SNR_adj_dB_Q7 = smlawb(c->current_SNR_dB_Q7, smulbb(SB_FIXC(-4.0f, 7) >> (4 + 1), b_Q8),
-                               smulwb(SB_FIXC(1.0, 14) + c->input_quality_Q14, c->coding_quality_Q14));
-    if (c->sigtype == 0) {
-        SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, SB_FIXC(2.0f, 8), st->LTPCorr_Q15);
-    } else {
-        SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, smlawb(SB_FIXC(6.0, 9), -SB_FIXC(0.4, 18), c->current_SNR_dB_Q7),
-                               SB_FIXC(1.0, 14) - c->input_quality_Q14);
-    }
-    i32 md_input_quality_Q14 = sigm_q15(rshift_round(c->current_SNRPerMD_dB_Q7 - SB_FIXC(18.0, 7), 4)) >> 1;
-    i32 md_SNR_adj_dB_Q7 = smlawb(c->current_SNRPerMD_dB_Q7, smulbb(SB_FIXC(-4.0f, 7) >> (4 + 1), b_Q8),
-                                  smulwb(SB_FIXC(1.0, 14) + md_input_quality_Q14, c->coding_quality_Q14));
-    if (c->sigtype == 0) {
-        md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, SB_FIXC(2.0f, 8), st->LTPCorr_Q15);
-    } else {
-        md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, smlawb(SB_FIXC(6.0, 9), -SB_FIXC(0.4, 18), c->current_SNRPerMD_dB_Q7),
-                                  SB_FIXC(1.0, 14) - c->input_quality_Q14);
-    }
-
-    // sparseness
-    if (c->sigtype == 0) {
-        c->QuantOffsetType = 0;
-        c->sparseness_Q8 = 0;
-    } else {
+    // sparseness of the unvoiced residual
+    i32 energy_variation_Q7 = 0;
+    if (c->sigtype != 0) {
         const int nSamples = 16;
-        i32 energy_variation_Q7 = 0, log_energy_prev_Q7 = 0;
+        i32 log_energy_prev_Q7 = 0;
         const i16* pr = pitch_res;
         for (int k = 0; k < 10; k++) {
             sum_sqr_shift(&nrg, &scale, pr, nSamples, 0);
@@ -155,21 +246,15 @@ SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, c
             log_energy_prev_Q7 = log_energy_Q7;
             pr += nSamples;
         }
-        c->sparseness_Q8 = sigm_q15(smulwb(energy_variation_Q7 - SB_FIXC(5.0, 7), SB_FIXC(0.1, 16))) >> 7;
-        c->QuantOffsetType = c->sparseness_Q8 > SB_FIXC(0.75f, 8) ? 0 : 1;
-        SNR_adj_dB_Q7 = smlawb(SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), c->sparseness_Q8 - SB_FIXC(0.5, 8));
-        md_SNR_adj_dB_Q7 = smlawb(md_SNR_adj_dB_Q7, SB_FIXC(2.0f, 15), c->sparseness_Q8 - SB_FIXC(0.5, 8));
     }
-
-    // bandwidth expansion control
-    i32 strength_Q16 = smulwb(c->predGain_Q16, SB_FIXC(1e-3f, 16));
-    i32 BWExp1_Q16, BWExp2_Q16;
-    BWExp1_Q16 = BWExp2_Q16 = div32_varq(SB_FIXC(0.95f, 16), smlaww(SB_FIXC(1.0, 16), strength_Q16, strength_Q16), 16);
-    i32 delta_Q16 = smulwb(SB_FIXC(1.0, 16) - smulbb(3, c->coding_quality_Q14), SB_FIXC(0.01f, 16));
-    BWExp1_Q16 = subw(BWExp1_Q16, delta_Q16);
-    BWExp2_Q16 = addw(BWExp2_Q16, delta_Q16);
-    BWExp1_Q16 = shl(BWExp1_Q16, 14) / (BWExp2_Q16 >> 2);
-    i32 warping_Q16 = smlawb(WARPING_Q16, c->coding_quality_Q14, SB_FIXC(0.01, 18));
+    const ShapeCtl s = shape_control(c->sigtype, st->SNR_dB_Q7, st->SNRPerMD_dB_Q7, c->input_quality_bands_Q15, st->speech_activity_Q8,
+                                     st->LTPCorr_Q15, energy_variation_Q7, c->predGain_Q16);
+    c->current_SNR_dB_Q7 = st->SNR_dB_Q7;
+    c->current_SNRPerMD_dB_Q7 = st->SNRPerMD_dB_Q7;
+    c->input_quality_Q14 = s.input_quality_Q14;
+    c->coding_quality_Q14 = s.coding_quality_Q14;
+    c->sparseness_Q8 = s.sparseness_Q8;
+    c->QuantOffsetType = s.QuantOffsetType;
 
     for (int k = 0; k < NB_SUBFR; k++) {
         const int flat_part = 40, slope_part = (SHAPE_WIN - 40) >> 1;
@@ -177,83 +262,28 @@ SB_FN void noise_shape_analysis(EncSilk* st, EncCtrl* c, const i16* pitch_res, c
         for (int i = 0; i < flat_part; i++) x_windowed[slope_part + i] = x_ptr[slope_part + i];
         apply_sine_window(x_windowed + slope_part + flat_part, x_ptr + slope_part + flat_part, 2, slope_part);
         x_ptr += SUBFR;
-        warped_autocorrelation(auto_corr, &scale, x_windowed, warping_Q16, SHAPE_WIN, SHAPE_ORDER);
-        auto_corr[0] = addw(auto_corr[0], imax(smulwb(auto_corr[0] >> 4, SB_FIXC(1e-5f, 20)), 1));
-        nrg = schur64(refl_coef_Q16, auto_corr, SHAPE_ORDER);
-        k2a_q16(AR2_Q24, refl_coef_Q16, SHAPE_ORDER);
-        int Qnrg = -scale;
-        if (Qnrg & 1) { Qnrg -= 1; nrg >>= 1; }
-        i32 tmp32 = sqrt_approx(nrg);
-        Qnrg >>= 1;
-        c->Gains_Q16[k] = lshift_sat32(tmp32, 16 - Qnrg);
-        i32 gain_mult_Q16 = warped_gain(AR2_Q24, warping_Q16, SHAPE_ORDER);
-        c->Gains_Q16[k] = smulww(c->Gains_Q16[k], gain_mult_Q16);
-        if (c->Gains_Q16[k] < 0) c->Gains_Q16[k] = SB_I32_MAX;
-        bwexpander_32(AR2_Q24, SHAPE_ORDER, BWExp2_Q16);
-        for (int i = 0; i < SHAPE_ORDER; i++) AR1_Q24[i] = AR2_Q24[i];
-        bwexpander_32(AR1_Q24, SHAPE_ORDER, BWExp1_Q16);
+        warped_autocorrelation(auto_corr, &scale, x_windowed, s.warping_Q16, SHAPE_WIN, SHAPE_ORDER);
+        c->Gains_Q16[k] = shape_window(AR2_Q24, AR1_Q24, auto_corr, scale, s.warping_Q16, s.BWExp1_Q16, s.BWExp2_Q16);
         for (int i = 0; i < SHAPE_ORDER; i++) { ar_Q24[k][0][i] = AR2_Q24[i]; ar_Q24[k][1][i] = AR1_Q24[i]; }
     }
 
-    // gain tweaking
-    i32 md_gain_mult_Q16 = log2lin(negw(smlawb(-SB_FIXC(16.0, 7), md_SNR_adj_dB_Q7, SB_FIXC(0.16, 16))));
-    i32 gain_mult_Q16 = log2lin(negw(smlawb(-SB_FIXC(16.0, 7), SNR_adj_dB_Q7, SB_FIXC(0.16, 16))));
+    const i32 md_gain_mult_Q16 = shape_gain_mult_q16(s.md_SNR_adj_dB_Q7);
+    const i32 gain_mult_Q16 = shape_gain_mult_q16(s.SNR_adj_dB_Q7);
     c->md_delta_gain_par = (float)gain_mult_Q16 / (float)md_gain_mult_Q16;
-    i32 gain_add_Q16 = log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(4.0f, 7), SB_FIXC(0.16, 16)));
-    i32 tmp32 = log2lin(smlawb(SB_FIXC(16.0, 7), SB_FIXC(-50.0f, 7), SB_FIXC(0.16, 16)));
-    tmp32 = smulww(st->avgGain_Q16, tmp32);
-    gain_add_Q16 = add_sat32(gain_add_Q16, tmp32);
+    const i32 gain_add_Q16 = shape_gain_add_q16(st->avgGain_Q16);
     for (int k = 0; k < NB_SUBFR; k++) {
-        c->Gains_Q16[k] = smulww(c->Gains_Q16[k], gain_mult_Q16);
-        if (c->Gains_Q16[k] < 0) c->Gains_Q16[k] = SB_I32_MAX;
+        c->Gains_Q16[k] = shape_gain_tweak(c->Gains_Q16[k], gain_mult_Q16, gain_add_Q16);
+        st->avgGain_Q16 = shape_avg_gain_q16(st->avgGain_Q16, c->Gains_Q16[k], st->speech_activity_Q8);
     }
+    shape_par[0] = s.warping_Q16;
+    shape_par[1] = shape_pregain_mult_q16(s.coding_quality_Q14);
+
+    const HarmTilt h = shape_harm_tilt(c->sigtype, st->speech_activity_Q8, s.input_quality_Q14, s.coding_quality_Q14, st->LTPCorr_Q15);
     for (int k = 0; k < NB_SUBFR; k++) {
-        c->Gains_Q16[k] = add_pos_sat32(c->Gains_Q16[k], gain_add_Q16);
-        st->avgGain_Q16 = add_sat32(st->avgGain_Q16,
-            smulwb(c->Gains_Q16[k] - st->avgGain_Q16, rshift_round(smulbb(st->speech_activity_Q8, SB_FIXC(1e-3f, 10)), 2)));
-    }
-
-    // de-essing factor: fs == 8 kHz takes no branch (noise_shape_analysis_FIX.c:438-457)
-    shape_par[0] = warping_Q16;
-    shape_par[1] = SB_FIXC(1.0, 16) + rshift_round(mlaw(SB_FIXC(0.05f, 26), c->coding_quality_Q14, SB_FIXC(0.1f, 12)), 10);
-
-    // low-frequency shaping and noise tilt
-    strength_Q16 = mulw(SB_FIXC(3.0f, 0), SB_FIXC(1.0, 16) + smulbb(SB_FIXC(0.5f, 1), c->input_quality_bands_Q15[0] - SB_FIXC(1.0, 15)));
-    i32 Tilt_Q16;
-    if (c->sigtype == 0) {
-        i32 fs_kHz_inv = SB_FIXC(0.2, 14) / 8;
-        for (int k = 0; k < NB_SUBFR; k++) {
-            i32 b_Q14 = fs_kHz_inv + SB_FIXC(3.0, 14) / c->pitchL[k];
-            c->LF_shp_Q14[k] = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, b_Q14), 16);
-            c->LF_shp_Q14[k] |= (u16)(b_Q14 - SB_FIXC(1.0, 14));
-        }
-        Tilt_Q16 = -SB_FIXC(0.3f, 16) - smulwb(SB_FIXC(1.0, 16) - SB_FIXC(0.3f, 16), smulwb(SB_FIXC(0.35f, 24), st->speech_activity_Q8));
-    } else {
-        i32 b_Q14 = 21299 / 8;
-        c->LF_shp_Q14[0] = shl(SB_FIXC(1.0, 14) - b_Q14 - smulwb(strength_Q16, smulwb(SB_FIXC(0.6, 16), b_Q14)), 16);
-        c->LF_shp_Q14[0] |= (u16)(b_Q14 - SB_FIXC(1.0, 14));
-        for (int k = 1; k < NB_SUBFR; k++) c->LF_shp_Q14[k] = c->LF_shp_Q14[0];
-        Tilt_Q16 = -SB_FIXC(0.3f, 16);
-    }
-
-    // harmonic shaping control
-    i32 HarmBoost_Q16 = smulwb(smulwb(SB_FIXC(1.0, 17) - shl(c->coding_quality_Q14, 3), st->LTPCorr_Q15), SB_FIXC(0.1f, 16));
-    HarmBoost_Q16 = smlawb(HarmBoost_Q16, SB_FIXC(1.0, 16) - shl(c->input_quality_Q14, 2), SB_FIXC(0.1f, 16));
-    i32 HarmShapeGain_Q16;
-    if (c->sigtype == 0) {
-        HarmShapeGain_Q16 = smlawb(SB_FIXC(0.3f, 16),
-            SB_FIXC(1.0, 16) - smulwb(SB_FIXC(1.0, 18) - shl(c->coding_quality_Q14, 4), c->input_quality_Q14), SB_FIXC(0.2f, 16));
-        HarmShapeGain_Q16 = smulwb(shl(HarmShapeGain_Q16, 1), sqrt_approx(shl(st->LTPCorr_Q15, 15)));
-    } else {
-        HarmShapeGain_Q16 = 0;
-    }
-    for (int k = 0; k < NB_SUBFR; k++) {
-        st->HarmBoost_smth_Q16 = smlawb(st->HarmBoost_smth_Q16, HarmBoost_Q16 - st->HarmBoost_smth_Q16, SB_FIXC(0.4f, 16));
-        st->HarmShapeGain_smth_Q16 = smlawb(st->HarmShapeGain_smth_Q16, HarmShapeGain_Q16 - st->HarmShapeGain_smth_Q16, SB_FIXC(0.4f, 16));
-        st->Tilt_smth_Q16 = smlawb(st->Tilt_smth_Q16, Tilt_Q16 - st->Tilt_smth_Q16, SB_FIXC(0.4f, 16));
-        c->HarmBoost_Q14[k] = rshift_round(st->HarmBoost_smth_Q16, 2);
-        c->HarmShapeGain_Q14[k] = rshift_round(st->HarmShapeGain_smth_Q16, 2);
-        c->Tilt_Q14[k] = rshift_round(st->Tilt_smth_Q16, 2);
+        c->LF_shp_Q14[k] = shape_lf_shp_q14(c->sigtype, c->pitchL[k], c->input_quality_bands_Q15[0]);
+        c->HarmBoost_Q14[k] = shape_smooth_q14(st->HarmBoost_smth_Q16, h.HarmBoost_Q16);
+        c->HarmShapeGain_Q14[k] = shape_smooth_q14(st->HarmShapeGain_smth_Q16, h.HarmShapeGain_Q16);
+        c->Tilt_Q14[k] = shape_smooth_q14(st->Tilt_smth_Q16, h.Tilt_Q16);
     }
 }
 

@@ -95,31 +95,47 @@ SB_FN void k2a(i32* A_Q24, const i16* rc_Q15, int order) {
     }
 }
 
-// ---- SKP_Silk_schur64.c:42-91 ---------------------------------------------------------------------
-SB_FN i32 schur64(i32* rc_Q16, const i32* c, int order) {
-    i32 C[17][2];
-    if (c[0] <= 0) { for (int k = 0; k < order; k++) rc_Q16[k] = 0; return 0; }
-    for (int k = 0; k < order + 1; k++) C[k][0] = C[k][1] = c[k];
-    for (int k = 0; k < order; k++) {
-        i32 rc_Q31 = div32_varq(negw(C[k + 1][0]), C[0][1], 31);
+// ---- SKP_Silk_schur64.c:42-91, SKP_Silk_k2a_Q16.c:40-60, SKP_Silk_bwexpander_32.c:31-47 at a fixed order -------------
+// Every array in registers (fully unrolled): in the analysis kernel these run as one scalar instance per shaping window,
+// where a local-memory array would put a ~30-cycle load into every step of a long dependent chain.
+template <int ORD> SB_HD i32 schur64_r(i32 (&rc_Q16)[ORD], const i32 (&c)[ORD + 1]) {
+    i32 C0[ORD + 1], C1[ORD + 1];
+    if (c[0] <= 0) {
+#pragma unroll
+        for (int k = 0; k < ORD; k++) rc_Q16[k] = 0;
+        return 0;
+    }
+#pragma unroll
+    for (int k = 0; k < ORD + 1; k++) C0[k] = C1[k] = c[k];
+#pragma unroll
+    for (int k = 0; k < ORD; k++) {
+        const i32 rc_Q31 = div32_varq(negw(C0[k + 1]), C1[0], 31);
         rc_Q16[k] = rshift_round(rc_Q31, 15);
-        for (int n = 0; n < order - k; n++) {
-            i32 t1 = C[n + k + 1][0], t2 = C[n][1];
-            C[n + k + 1][0] = addw(t1, smmul(shl(t2, 1), rc_Q31));
-            C[n][1] = addw(t2, smmul(shl(t1, 1), rc_Q31));
+#pragma unroll
+        for (int n = 0; n < ORD - k; n++) {
+            const i32 t1 = C0[n + k + 1], t2 = C1[n];
+            C0[n + k + 1] = addw(t1, smmul(shl(t2, 1), rc_Q31));
+            C1[n] = addw(t2, smmul(shl(t1, 1), rc_Q31));
         }
     }
-    return C[0][1];
+    return C1[0];
 }
-
-// ---- SKP_Silk_k2a_Q16.c:40-60 ---------------------------------------------------------------------
-SB_FN void k2a_q16(i32* A_Q24, const i32* rc_Q16, int order) {
-    i32 Atmp[16];
-    for (int k = 0; k < order; k++) {
+template <int ORD> SB_HD void k2a_q16_r(i32 (&A_Q24)[ORD], const i32 (&rc_Q16)[ORD]) {
+#pragma unroll
+    for (int k = 0; k < ORD; k++) {
+        i32 Atmp[ORD];
+#pragma unroll
         for (int n = 0; n < k; n++) Atmp[n] = A_Q24[n];
+#pragma unroll
         for (int n = 0; n < k; n++) A_Q24[n] = smlaww(A_Q24[n], Atmp[k - n - 1], rc_Q16[k]);
         A_Q24[k] = negw(shl(rc_Q16[k], 8));
     }
+}
+template <int ORD> SB_HD void bwexpander_32_r(i32 (&ar)[ORD], i32 chirp_Q16) {
+    i32 t = chirp_Q16;
+#pragma unroll
+    for (int i = 0; i < ORD - 1; i++) { ar[i] = smulww(ar[i], t); t = smulww(chirp_Q16, t); }
+    ar[ORD - 1] = smulww(ar[ORD - 1], t);
 }
 
 // ---- SKP_Silk_bwexpander.c:31-48 / SKP_Silk_bwexpander_32.c:31-47 -------------------------------------
