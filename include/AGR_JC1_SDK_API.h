@@ -65,6 +65,13 @@ SKP_int32 AGR_Sate_Encoder_Encode(void *SATEEnc_State, const SKP_int16 *AGR_Sate
                                   SKP_int32 AGR_Sate_Buf_Size, SKP_int16 *nBytesOut);
 int AGR_Sate_Encoder_Uninit(void *SATEEnc_State);
 
+/* Decoder arithmetic: the reference ships a float build (JC1_SDK_SRC_FLP) and a fixed-point build (JC1_SDK_SRC_ARM) whose
+   decoded PCM differs.  Each Init reads the environment variable SOLO_B200_DEC_ARITH:
+     unset or "flp" : PCM of the float build (the default);
+     "fix"          : PCM of the fixed-point build, bit for bit (40 ms packets and joint mode 1; with 20 ms packets the
+                      fixed-point build decodes every payload twice, a defect not reproduced: Init returns NULL);
+     anything else  : Init prints a message and returns NULL.
+   The setting stays with the handle; changing the variable later affects only later Inits. */
 void *AGR_Sate_Decoder_Init(USER_Ctrl_dec *dec_Ctrl);
 SKP_int32 AGR_Sate_Decoder_Decode(void *SATEDec_State, SKP_int16 *AGR_Sate_PCM, SKP_int16 *nSamplesOut,
                                   const SKP_uint8 *AGR_Sate_Bit, SKP_int16 nBytes[], SKP_int32 lostflag);

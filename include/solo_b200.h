@@ -69,7 +69,19 @@ int solo_b200_enc_batch_set_control_device(solo_b200_enc_batch *b, const int32_t
    out-of-range value (nothing applied). */
 int solo_b200_encoder_set_control(void *SATEEnc_State, int32_t rate_bps, int32_t dtx, int32_t loss_perc);
 
+/* Decoder arithmetic of a batch's streams.  The reference ships two builds whose decoded PCM differs (by up to ~1 800 LSB on
+   speech); the low band is the same integer decoder in both, the high-band synthesis and the synthesis filter bank are not.
+     SOLO_B200_DEC_FLP : PCM of the float build (JC1_SDK_SRC_FLP), what solo_b200_dec_batch_create gives.
+     SOLO_B200_DEC_FIX : PCM of the fixed-point build (JC1_SDK_SRC_ARM), bit for bit; 40 ms packets and joint mode 1 only.
+                         With 20 ms packets the fixed-point build decodes every payload twice (it always decodes two SILK
+                         frames per call), which is its defect, not a mode worth reproducing: create returns NULL.
+   The arithmetic is part of each stream's state, so exported blobs carry it. */
+#define SOLO_B200_DEC_FLP 0
+#define SOLO_B200_DEC_FIX 1
 solo_b200_dec_batch *solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_dec *ctrl, int device);
+/* The same with the arithmetic: NULL, with solo_b200_last_error() set, for an unknown value or SOLO_B200_DEC_FIX with 20 ms
+   packets. */
+solo_b200_dec_batch *solo_b200_dec_batch_create_arith(int n_streams, const USER_Ctrl_dec *ctrl, int device, int arith);
 int solo_b200_dec_batch_decode_host(solo_b200_dec_batch *b, int16_t *pcm, const uint8_t *bits, int cap,
                                     const int16_t *nbytes, const int32_t *lostflag, int32_t *ret);
 int solo_b200_dec_batch_decode_device(solo_b200_dec_batch *b, int16_t *d_pcm, const uint8_t *d_bits, int cap,

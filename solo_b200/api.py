@@ -55,6 +55,8 @@ def lib():
         L.solo_b200_encoder_set_control.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
         L.solo_b200_dec_batch_create.restype = vp
         L.solo_b200_dec_batch_create.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int]
+        L.solo_b200_dec_batch_create_arith.restype = vp
+        L.solo_b200_dec_batch_create_arith.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int, C.c_int]
         L.solo_b200_dec_batch_decode_host.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
         L.solo_b200_dec_batch_decode_device.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp, vp]
         L.solo_b200_dec_batch_destroy.argtypes = [vp]
@@ -256,14 +258,22 @@ class EncoderBatch:
     __del__ = close
 
 
+DEC_ARITH = {"flp": 0, "fix": 1}   # SOLO_B200_DEC_FLP / SOLO_B200_DEC_FIX
+
+
 class DecoderBatch:
     """N decoder streams resident on one GPU."""
 
-    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0):
+    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0, arith="flp"):
+        """arith: "flp" decodes to the reference float build's PCM, "fix" to its fixed-point build's (40 ms packets and
+        joint mode 1 only; see solo_b200_dec_batch_create_arith in include/solo_b200.h)."""
+        if arith not in DEC_ARITH:
+            raise SoloError("arith must be one of %s, not %r" % (sorted(DEC_ARITH), arith))
         self.n = int(n)
         self.samples = 16 * framesize_ms
+        self.arith = arith
         self.ctrl = DecCtrl(0, 16000, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
-        self.h = lib().solo_b200_dec_batch_create(self.n, C.byref(self.ctrl), device)
+        self.h = lib().solo_b200_dec_batch_create_arith(self.n, C.byref(self.ctrl), device, DEC_ARITH[arith])
         if not self.h:
             raise SoloError("solo_b200_dec_batch_create failed: " + _err())
 

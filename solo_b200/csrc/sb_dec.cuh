@@ -13,6 +13,9 @@
 //   SKP_Silk_PLC.c:43-387, SKP_Silk_CNG.c:31-149, SKP_Silk_LPC_synthesis_filter.c:41-94,
 //   SKP_Silk_wrappers_FLP.c:54-73, SKP_Silk_create_init_destroy.c:35-55, SKP_Silk_decoder_set_fs.c:31-86.
 // Float code must be compiled without FMA contraction (-fmad=false / -ffp-contract=off).
+// A stream may instead follow the reference's fixed-point build (DEC_FIX, per stream in DecState::arith): same low band,
+// integer high-band synthesis and integer filter bank (JC1_SDK_SRC_ARM/src/libBWE/AGR_BWE_decode_frame_FIX.c:40-115,
+// AGR_BWE_LPC_synthesizer.c:56-136, AGR_BWE_quant_highband.c:106-121, AGR_BWE_qmf.c:86-182 with FIXED_POINT).
 #pragma once
 #include "sb_rangecoder.cuh"
 #include "sb_sigproc.cuh"
@@ -27,10 +30,14 @@ struct DecMd {
     i32 prevDeltaGainIndex;
 };
 
+// decoder arithmetic of a stream: the reference's float build (the default) or its fixed-point build
+enum { DEC_FLP = 0, DEC_FIX = 1 };
+
 struct DecState {
     i32 useMDIndex;
     i32 frames_per_packet;  // 2: 40 ms packets, 1: 20 ms packets
     i32 hb_frame;           // 160, or 320 with joint_mode 1
+    i32 arith;              // DEC_FLP or DEC_FIX
     i32 seen_good;  // 0 until the first frame has been range-decoded (reference state is still at fs = 24 kHz)
     DecMd md[2];
     i32 prev_inv_gain_Q16;
@@ -53,9 +60,12 @@ struct DecState {
     i32 cng_smth_NLSF_Q15[LPC_ORDER];
     i32 cng_synth_state[LPC_ORDER];
     i32 cng_smth_Gain_Q16, cng_rand_seed;
-    // high band + QMF synthesis (AGR_BWE_structs.h, FLP)
+    // high band + QMF synthesis (AGR_BWE_structs.h).  A stream uses either the float fields (DEC_FLP) or their fixed-point
+    // counterparts (DEC_FIX), so they share storage.  The filter-bank memories hold int16-valued samples in both modes.
     i32 hb_lossCnt, hb_first;
-    float hb_prev_NLSFq[HB_ORDER], hb_prev_Gain, hb_sLPC[16];
+    union { float hb_prev_NLSFq[HB_ORDER]; i32 hb_prev_NLSF_Q15[HB_ORDER]; };
+    union { float hb_prev_Gain; i32 hb_prev_Gain_fix; };
+    union { float hb_sLPC[16]; i32 hb_synth_Q14[HB_ORDER]; };   // HB_synth_state: [HB_ORDER - 1] newest
     float g0_mem[64], g1_mem[64];
 };
 
@@ -71,9 +81,10 @@ struct DecCtrl {
 };
 
 // SKP_Silk_init_decoder + AGR_Sate_Decoder_Init, expressed for the 8 kHz core the first good frame selects.
-SB_FN void dec_state_init(DecState* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0) {
+SB_FN void dec_state_init(DecState* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0, i32 arith = DEC_FLP) {
     memset(st, 0, sizeof(DecState));
     st->useMDIndex = useMDIndex;
+    st->arith = arith == DEC_FIX ? DEC_FIX : DEC_FLP;
     st->frames_per_packet = framesize_ms == 20 ? 1 : 2;
     st->hb_frame = joint_hb ? 320 : HB_FRAME;
     st->first_frame_after_reset = 1;
@@ -649,11 +660,50 @@ SB_HD void qmf_synth_group(const float* xx1, const float* xx2, const float* a, i
     }
 }
 
-// ---- scalar model of the synthesis kernel: AGR_Sate_qmf_synth, float branch (AGR_BWE_qmf.c:86-182), N = 2 * N2 = 640
-// or 320, M = 64, into int16 PCM.  low / high: the band signals dec_packet handed out.
+// The same group in the fixed-point build (AGR_BWE_qmf.c:134-168 with FIXED_POINT): int16 band signals, memories and
+// coefficients (qmf_fix), int32 MAC16_16 sums in the reference's "multiply twice" order, PSHR32(y, 15) and
+// SATURATE32(., 32767), which clamps to [-32767, 32767].  The sums wrap as the reference's int32 additions do.
+SB_HD void qmf_synth_group_fix(const i16* xx1, const i16* xx2, const i16* a, int N2, int i, i16* pcm4) {
+    enum { M2 = 32 };
+    u32 y0 = 0, y1 = 0, y2 = 0, y3 = 0;
+    i32 x10 = xx1[N2 - 2 - i], x20 = xx2[N2 - 2 - i];
+    for (int j = 0; j < M2; j += 2) {
+        i32 a0 = a[2 * j], a1 = a[2 * j + 1], na0 = (i16)(-a0);
+        const i32 x11 = xx1[N2 - 1 + j - i], x21 = xx2[N2 - 1 + j - i];
+        y0 += (u32)(a0 * x11); y0 += (u32)(na0 * x21);
+        y1 += (u32)(a1 * x11); y1 += (u32)(a1 * x21);
+        y2 += (u32)(a0 * x10); y2 += (u32)(na0 * x20);
+        y3 += (u32)(a1 * x10); y3 += (u32)(a1 * x20);
+        a0 = a[2 * j + 2]; a1 = a[2 * j + 3]; na0 = (i16)(-a0);
+        x10 = xx1[N2 + j - i];
+        x20 = xx2[N2 + j - i];
+        y0 += (u32)(a0 * x10); y0 += (u32)(na0 * x20);
+        y1 += (u32)(a1 * x10); y1 += (u32)(a1 * x20);
+        y2 += (u32)(a0 * x11); y2 += (u32)(na0 * x21);
+        y3 += (u32)(a1 * x11); y3 += (u32)(a1 * x21);
+    }
+    const u32 y4[4] = {y0, y1, y2, y3};
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const i32 t = (i32)(y4[q] + (1u << 14)) >> 15;
+        pcm4[q] = (i16)(t > 32767 ? 32767 : (t < -32767 ? -32767 : t));
+    }
+}
+
+// ---- scalar model of the synthesis kernel: AGR_Sate_qmf_synth (AGR_BWE_qmf.c:86-182), N = 2 * N2 = 640 or 320, M = 64,
+// into int16 PCM, float branch or (DEC_FIX) fixed-point branch.  low / high: the band signals dec_packet handed out.
 SB_FN void dec_synth(DecState* st, const i16* low, const float* high, i16* pcm) {
     enum { M2 = 32, N2MAX = PACKET / 2 };
     const int N2 = st->frames_per_packet * FRAME;
+    if (st->arith == DEC_FIX) {
+        i16 yy1[M2 + N2MAX], yy2[M2 + N2MAX];
+        const i16* a = SB_T(qmf_fix);
+        for (int i = 0; i < N2; i++) { yy1[i] = low[N2 - 1 - i]; yy2[i] = (i16)(i32)high[N2 - 1 - i]; }
+        for (int i = 0; i < M2; i++) { yy1[N2 + i] = (i16)(i32)st->g0_mem[2 * i + 1]; yy2[N2 + i] = (i16)(i32)st->g1_mem[2 * i + 1]; }
+        for (int i = 0; i < N2; i += 2) qmf_synth_group_fix(yy1, yy2, a, N2, i, pcm + 2 * i);
+        for (int i = 0; i < M2; i++) { st->g0_mem[2 * i + 1] = (float)yy1[i]; st->g1_mem[2 * i + 1] = (float)yy2[i]; }
+        return;
+    }
     float xx1[M2 + N2MAX], xx2[M2 + N2MAX];
     const float* a = SB_T(qmf_flt);
     for (int i = 0; i < N2; i++) { xx1[i] = (float)low[N2 - 1 - i]; xx2[i] = high[N2 - 1 - i]; }
@@ -723,6 +773,73 @@ SB_FN void hb_decode_frame(DecState* st, const u8* hb4, float* OutHigh, const i3
     else hb_decode_frame_t<2 * SUBFR>(st, hb4, OutHigh, res_Q10, lostflag);
 }
 
+// ---- AGR_Bwe_decode_frame_FIX (AGR_BWE_decode_frame_FIX.c:40-115): one 20 ms high-band frame, fixed-point build --------
+// Same arguments; the int16 output goes to OutHigh as float (exact), which the synthesis stage turns back into int16.
+// res_Q10 == nullptr: all-zero excitation, which is what the reference's memset of MAX_INTERNAL_FRAME_SIZE excitation words
+// on a lost high band (:65) leaves for every frame of the packet.  Its AGR_Sate_PLC_interp_HB_parameters_fix and the loss
+// branch at :82-88 are unreachable and have no counterpart here.
+template <int SF> SB_FN void hb_decode_frame_fix_t(DecState* st, const u8* hb4, float* OutHigh, const i32* res_Q10, int lostflag) {
+    enum { FOLDING_GAIN_FIX = 2867 };   // 0.7 in Q12
+    i32 QHB_LSP_Q15[HB_ORDER];
+    i16 A_Q12[HB_ORDER];
+    const bool lost = lostflag == 1 || lostflag == 2;
+    const u32 w = lost ? 0u : ((u32)hb4[0] << 24) | ((u32)hb4[1] << 16) | ((u32)hb4[2] << 8) | (u32)hb4[3];
+    const i32 prev_gain = st->hb_prev_Gain_fix;
+    // gain of sub-frame s: the previous frame's last one on loss (looked up where it is used: no array in local memory)
+    auto QGain = [&](int s) -> i32 { return lost ? prev_gain : SB_T(hb_gain_cb_fix)[(w >> (15 - 5 * s)) & 31]; };
+    if (lost) {
+        for (int i = 0; i < HB_ORDER; i++) QHB_LSP_Q15[i] = st->hb_prev_NLSF_Q15[i];
+        st->hb_lossCnt++;
+    } else {
+        int hb_idx = (w >> 20) & 0xFFF;
+        int idx1 = hb_idx & 0xFF, idx2 = hb_idx >> 8;
+        // AGR_Sate_lsp_dequant_highband (AGR_BWE_quant_highband.c:106-121)
+        for (int i = 0; i < HB_ORDER; i++)
+            QHB_LSP_Q15[i] = (i32)SB_T(hb_lsp_cb1_fix)[idx1 * HB_ORDER + i] + (i32)SB_T(hb_lsp_cb2_fix)[idx2 * HB_ORDER + i];
+        if (st->hb_first) {
+            for (int i = 0; i < HB_ORDER; i++) st->hb_prev_NLSF_Q15[i] = QHB_LSP_Q15[i];
+            st->hb_prev_Gain_fix = QGain(3);
+        }
+        st->hb_lossCnt = 0;
+    }
+    // the reference converts the same LSPs once per sub-frame
+    nlsf2a_stable(A_Q12, QHB_LSP_Q15, HB_ORDER);
+    // AGR_Sate_LPC_synthesis_filter_fix (AGR_BWE_LPC_synthesizer.c:56-136): its little-endian branch accumulates
+    // A_Q12[0] * S[7], A_Q12[1] * S[6], ... with SMLAWB / SMLAWT, i.e. smlawb in coefficient order
+    i32 S[HB_ORDER];
+    for (int i = 0; i < HB_ORDER; i++) S[i] = st->hb_synth_Q14[i];
+    for (int s = 0; s < 4; s++) {
+        const i32 Gain_Q16 = -FOLDING_GAIN_FIX * QGain(s);
+        for (int k = 0; k < SF; k++) {
+            i32 out32_Q10 = 0;
+#pragma unroll
+            for (int j = 0; j < HB_ORDER; j++) out32_Q10 = smlawb(out32_Q10, S[HB_ORDER - 1 - j], A_Q12[j]);
+            out32_Q10 = add_sat32(out32_Q10, smulww(Gain_Q16, res_Q10 ? res_Q10[s * SF + k] : 0));
+#pragma unroll
+            for (int j = 0; j < HB_ORDER - 1; j++) S[j] = S[j + 1];
+            S[HB_ORDER - 1] = lshift_sat32(out32_Q10, 4);
+            OutHigh[s * SF + k] = (float)sat16(rshift_round(out32_Q10, 10));
+        }
+    }
+    for (int i = 0; i < HB_ORDER; i++) st->hb_synth_Q14[i] = S[i];
+    if (lostflag == 0 || lostflag == 4 || lostflag == 3) {
+        st->hb_prev_Gain_fix = QGain(3);
+        for (int i = 0; i < HB_ORDER; i++) st->hb_prev_NLSF_Q15[i] = QHB_LSP_Q15[i];
+    }
+    st->hb_first = 0;
+}
+
+// Out of line on the device: inlined, it tipped the float path's dec_packet out of the decode kernel (a call per packet).
+#ifdef __CUDACC__
+__host__ __device__ __noinline__
+#else
+inline
+#endif
+void hb_decode_frame_fix(DecState* st, const u8* hb4, float* OutHigh, const i32* res_Q10, int lostflag) {
+    if (st->hb_frame == HB_FRAME) hb_decode_frame_fix_t<SUBFR>(st, hb4, OutHigh, res_Q10, lostflag);
+    else hb_decode_frame_fix_t<2 * SUBFR>(st, hb4, OutHigh, res_Q10, lostflag);
+}
+
 // A payload outliving its packet.  The reference keeps the range decoders (with their own copy of the payload) in the
 // persistent state (structs.h:85-92, 295-303) and re-initialises them only when the previous packet is finished.  A
 // corrupted packet whose last frame terminator decodes as "more frames" (with bytes left) therefore makes the following
@@ -744,7 +861,7 @@ struct DecPacketWork {
 };
 
 // Band signals handed from the decoder kernel to the synthesis-filter-bank kernel: int16 low band and float high band of
-// the packet (16-byte aligned on the device).
+// the packet (16-byte aligned on the device; a DEC_FIX stream's high band holds int16 values).
 struct DecBands { i16* low; float* high; };
 
 // bits/cap: payload row as handed in by the caller; nb: {n0, n1} (not modified); returns the reference's return code.
@@ -812,13 +929,16 @@ SB_FN i32 dec_packet(DecState* st, DecPacketWork* W, const u8* bits, int cap, co
         }
     }
     const int hb_lost = (lostflag == 1 || lostflag == 2);
+    const bool fix = st->arith == DEC_FIX;
     for (int f = 0; f < nhb; f++) {
         // App. A Q12: with the high band lost, the reference's memset after the first high-band frame wipes the excitation
-        // of the rest of the packet -- later frames are synthesised from zeros
-        const i32* res = (hb_lost && f > 0) ? nullptr : W->res_Q10 + f * F;
+        // of the rest of the packet -- later frames are synthesised from zeros.  The fixed-point build's memset comes before
+        // the first frame's synthesis, so there every frame is.
+        const i32* res = (hb_lost && (f > 0 || fix)) ? nullptr : W->res_Q10 + f * F;
         u8 hb4[4] = {0, 0, 0, 0};
         if (!hb_lost) for (int i = 0; i < 4; i++) hb4[i] = bits[hb_off + 4 * f + i];
-        hb_decode_frame(st, hb4, W->OutHigh + f * F, res, lostflag);
+        if (fix) hb_decode_frame_fix(st, hb4, W->OutHigh + f * F, res, lostflag);
+        else hb_decode_frame(st, hb4, W->OutHigh + f * F, res, lostflag);
     }
     // the 64-tap synthesis filter bank has no recurrence: on the device it runs as its own kernel
 #ifdef __CUDA_ARCH__

@@ -186,9 +186,10 @@ __global__ void __launch_bounds__(SB_TPB, SB_FINISH_MINB) sb_enc_finish_kernel(E
     enc_store_high_band(st, scr, k, lb, nb1, out, cap, &nbytes[2 * s]);
 }
 
-__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecState* states, int n, int mdi, int framesize_ms, int joint_hb) {
+static_assert(SOLO_B200_DEC_FLP == DEC_FLP && SOLO_B200_DEC_FIX == DEC_FIX, "decoder arithmetic codes");
+__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecState* states, int n, int mdi, int framesize_ms, int joint_hb, int arith) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb);
+    if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb, arith);
 }
 
 __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(DecState* states, const u8* __restrict__ bits, int cap,
@@ -207,14 +208,22 @@ __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(D
 
 // ---- synthesis filter bank + float -> int16, one warp per stream (AGR_BWE_qmf.c:86-182, AGR_BWE_decode_frame_FLP.c:222-231) ----
 // 160 (80) independent groups of four outputs per packet: lanes over groups, band signals and filter memories staged in
-// shared memory; the PCM row is written with 8-byte stores, 256 contiguous bytes per warp instruction.
+// shared memory; the PCM row is written with 8-byte stores, 256 contiguous bytes per warp instruction.  A DEC_FIX stream
+// takes the integer filter bank in the same layout, its band signals staged as int16 in the first half of each row.
 #define SB_SYN_WARPS 4
+__device__ __forceinline__ void store_pcm4(i16* out, int g, const i16* y) {
+    int2 pk;
+    pk.x = (int)((u16)y[0] | ((u32)(u16)y[1] << 16));
+    pk.y = (int)((u16)y[2] | ((u32)(u16)y[3] << 16));
+    reinterpret_cast<int2*>(out)[g] = pk;
+}
 __global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecState* states, const i16* __restrict__ band_low, const float* __restrict__ band_high,
                                                                         const i32* __restrict__ ret_int, i16* __restrict__ pcm, int spp, int n) {
     __shared__ float xx[SB_SYN_WARPS][2][32 + PACKET / 2];
     __shared__ float coef[64];
+    __shared__ i16 coef_fix[64];
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < 64; i += blockDim.x) coef[i] = SB_T(qmf_flt)[i];
+    for (int i = threadIdx.x; i < 64; i += blockDim.x) { coef[i] = SB_T(qmf_flt)[i]; coef_fix[i] = SB_T(qmf_fix)[i]; }
     __syncthreads();
     const int s = blockIdx.x * SB_SYN_WARPS + w;
     if (s >= n || ret_int[s] < 0) return;         // a rejected packet leaves its PCM row and the filter memories alone
@@ -224,18 +233,32 @@ __global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecStat
     DecState* st = &states[s];
     const i16* lo = band_low + (size_t)s * N2;
     const float* hi = band_high + (size_t)s * N2;
+    i16* out = pcm + (size_t)s * spp;
+    if (st->arith == DEC_FIX) {                   // warp-uniform: one stream per warp
+        i16* yy1 = reinterpret_cast<i16*>(xx1);
+        i16* yy2 = reinterpret_cast<i16*>(xx2);
+        for (int i = lane; i < N2; i += 32) { yy1[i] = lo[N2 - 1 - i]; yy2[i] = (i16)__float2int_rz(hi[N2 - 1 - i]); }
+        yy1[N2 + lane] = (i16)__float2int_rz(st->g0_mem[2 * lane + 1]);
+        yy2[N2 + lane] = (i16)__float2int_rz(st->g1_mem[2 * lane + 1]);
+        __syncwarp();
+        for (int g = lane; g < N2 / 2; g += 32) {
+            i16 y[4];
+            qmf_synth_group_fix(yy1, yy2, coef_fix, N2, 2 * g, y);
+            store_pcm4(out, g, y);
+        }
+        __syncwarp();
+        st->g0_mem[2 * lane + 1] = (float)yy1[lane];
+        st->g1_mem[2 * lane + 1] = (float)yy2[lane];
+        return;
+    }
     for (int i = lane; i < N2; i += 32) { xx1[i] = (float)lo[N2 - 1 - i]; xx2[i] = hi[N2 - 1 - i]; }
     xx1[N2 + lane] = st->g0_mem[2 * lane + 1];
     xx2[N2 + lane] = st->g1_mem[2 * lane + 1];
     __syncwarp();
-    i16* out = pcm + (size_t)s * spp;
     for (int g = lane; g < N2 / 2; g += 32) {
         i16 y[4];
         qmf_synth_group(xx1, xx2, coef, N2, 2 * g, y);
-        int2 pk;
-        pk.x = (int)((u16)y[0] | ((u32)(u16)y[1] << 16));
-        pk.y = (int)((u16)y[2] | ((u32)(u16)y[3] << 16));
-        reinterpret_cast<int2*>(out)[g] = pk;
+        store_pcm4(out, g, y);
     }
     __syncwarp();
     st->g0_mem[2 * lane + 1] = xx1[lane];
@@ -611,8 +634,19 @@ int solo_b200_enc_batch_set_control_host(solo_b200_enc_batch* b, const int32_t* 
 void solo_b200_enc_batch_destroy(solo_b200_enc_batch* b) { batch_destroy(b); }
 
 // ---- decoder batch --------------------------------------------------------------------------------
-static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst) {
+// The fixed-point build decodes two SILK frames per call whatever the packet length (AGR_BWE_decode_frame_FIX.c:173,
+// HB2LB_NUM = 2), so with 20 ms packets it decodes every payload twice: that defect is not reproduced, 20 ms is refused.
+static int check_dec_arith(const USER_Ctrl_dec* c, int arith) {
+    if (arith != SOLO_B200_DEC_FLP && arith != SOLO_B200_DEC_FIX) { snprintf(g_err, sizeof g_err, "bad decoder arithmetic %d", arith); return -1; }
+    if (arith == SOLO_B200_DEC_FIX && c && c->framesize_ms == 20) {
+        snprintf(g_err, sizeof g_err, "fixed-point decoding of 20 ms packets is not supported");
+        return -1;
+    }
+    return 0;
+}
+static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst, int arith) {
     if (n_streams <= 0 || check_dec_ctrl(ctrl)) { snprintf(g_err, sizeof g_err, "bad decoder configuration"); return nullptr; }
+    if (check_dec_arith(ctrl, arith)) return nullptr;
     if (require_gpu(device)) return nullptr;
     solo_b200_dec_batch* b = new solo_b200_dec_batch();
     if (!batch_setup(b, n_streams, device, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
@@ -624,13 +658,19 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
         fail("dec_batch_create", cudaGetLastError());
         return batch_destroy(b);
     }
-    sb_dec_init_kernel<<<(n_streams + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0);
+    sb_dec_init_kernel<<<(n_streams + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0,
+                                                                              arith);
     count_launch();
     cudaError_t e = cudaStreamSynchronize(b->st[0]);
     if (e != cudaSuccess) { fail("dec init kernel", e); return batch_destroy(b); }
     return b;
 }
-solo_b200_dec_batch* solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_dec* ctrl, int device) { return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS); }
+solo_b200_dec_batch* solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_dec* ctrl, int device) {
+    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, SOLO_B200_DEC_FLP);
+}
+solo_b200_dec_batch* solo_b200_dec_batch_create_arith(int n_streams, const USER_Ctrl_dec* ctrl, int device, int arith) {
+    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith);
+}
 
 static int dec_launch(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
                       i32* d_ret, cudaStream_t st) {
@@ -895,10 +935,19 @@ void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
         return nullptr;
     }
     if (check_dec_ctrl(dec_Ctrl)) { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: unsupported configuration\n"); return nullptr; }
+    // SOLO_B200_DEC_ARITH, read at every Init: unset or "flp" = the float build's PCM, "fix" = the fixed-point build's
+    const char* e = getenv("SOLO_B200_DEC_ARITH");
+    int arith;
+    if (!e || !strcmp(e, "flp")) arith = SOLO_B200_DEC_FLP;
+    else if (!strcmp(e, "fix")) arith = SOLO_B200_DEC_FIX;
+    else { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: SOLO_B200_DEC_ARITH must be \"flp\" or \"fix\", not \"%s\"\n", e); return nullptr; }
+    if (check_dec_arith(dec_Ctrl, arith)) { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: %s\n", g_err); return nullptr; }
+    // the arithmetic is a property of the slot, not of the segment: one segment holds handles of both kinds
     return arena_open(g_dec_segs, DEC_MAGIC, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, "AGR_Sate_Decoder_Init", "decoder",
-                      [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1); },
+                      [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1, SOLO_B200_DEC_FLP); },
                       [&](solo_b200_dec_batch* b, int slot) {
-                          sb_dec_init_kernel<<<1, SB_TPB, 0, b->st[0]>>>(b->d_states + slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable ? 1 : 0);
+                          sb_dec_init_kernel<<<1, SB_TPB, 0, b->st[0]>>>(b->d_states + slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable ? 1 : 0,
+                                                                        arith);
                       });
 }
 SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, SKP_int16* nSamplesOut, const SKP_uint8* AGR_Sate_Bit,
