@@ -19,13 +19,15 @@
  *     invalid joint_mode                                                            [AGR_BWE_SDK_API.c:34-36,73-76]
  *   - Decode: lostflag 1 = lost, 2 = MD1 only, 3 = MD2+HB only, 4 = both; the
  *     caller pre-trims payload / nBytes as test/dec_main.c:245-307; nBytes[] is
- *     rewritten in place; *nSamplesOut = framesize_ms*16                            [AGR_BWE_decode_frame_FLP.c:171-190]
+ *     rewritten in place; *nSamplesOut = framesize_ms * samplerate / 1000         [AGR_BWE_decode_frame_FLP.c:171-190]
  *   - Encode/Decode/Uninit return -1 on a NULL handle; Decode returns -1 when
  *     nBytes[0] <= 0                                                                [AGR_BWE_SDK_API.c:139-141,261-270]
- * Accepted configurations (the ones the reference SDK itself can run at 16 kHz, AGR_BWE_SDK_API.c:40-110): samplerate 16000
- * with joint_enable 0 and framesize_ms 40 or 20, or joint_enable 1 / joint_mode 1 / framesize_ms 40 (one 40 ms high-band
- * frame per packet).  Anything else (joint modes 0, 2, 3 -- "Unsupport" in the reference too -- or 32 kHz input) makes Init
- * return NULL.
+ * Accepted configurations (the ones the reference SDK itself can run, AGR_BWE_SDK_API.c:40-110): joint_enable 0 and
+ * framesize_ms 40 or 20, or joint_enable 1 / joint_mode 1 / framesize_ms 40 (one 40 ms high-band frame per packet), at
+ * samplerate 16000 for both directions and at samplerate 32000 for the DECODER only (16 kHz SILK core, 8-16 kHz high band;
+ * the core rates that decode are in solo_b200.h and INTEGRATION.md).  AGR_Sate_Encoder_Init with samplerate 32000 returns
+ * NULL: the 32 kHz encoder is not built yet.  Anything else (joint modes 0, 2, 3 -- "Unsupport" in the reference too)
+ * makes Init return NULL.
  */
 #ifndef SOLO_B200_AGR_JC1_SDK_API_H
 #define SOLO_B200_AGR_JC1_SDK_API_H
@@ -43,7 +45,7 @@ typedef uint8_t SKP_uint8;
 typedef struct {
     SKP_int32 mode;            /* ignored by the reference as well */
     SKP_int32 targetRate_bps;  /* total rate incl. 1600 b/s high band; <= 0 selects 15600 (written back) */
-    SKP_int32 samplerate;      /* must be 16000 */
+    SKP_int32 samplerate;      /* must be 16000 (no 32 kHz encoder yet) */
     SKP_int32 dtx_enable;      /* 0 / 1 */
     SKP_int32 framesize_ms;    /* 40 or 20 */
     SKP_int32 joint_enable;    /* 0, or 1 together with joint_mode 1 and framesize_ms 40 */
@@ -53,7 +55,7 @@ typedef struct {
 
 typedef struct {
     SKP_int32 packetLoss_perc; /* ignored by the reference as well */
-    SKP_int32 samplerate;      /* must be 16000 */
+    SKP_int32 samplerate;      /* 16000 or 32000 */
     SKP_int32 framesize_ms;    /* 40 or 20 (must match the encoder) */
     SKP_int32 joint_enable;    /* as in USER_Ctrl_enc */
     SKP_int32 joint_mode;

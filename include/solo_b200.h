@@ -15,7 +15,20 @@
  * (one frame, 4 high-band bytes, 320 samples per row) -- the two packet sizes of the reference (AGR_BWE_SDK_API.c:78-110);
  * with joint_enable = 1, joint_mode = 1 (40 ms packets only) the high band is coded as one 40 ms frame (4 bytes, :63-66).
  *
- * Layouts (row = stream):  pcm  int16 [N][16 * framesize_ms]   bits uint8 [N][cap]
+ * Sample rate: ctrl->samplerate = 16000 (8 kHz SILK core, 4-8 kHz parametric high band) or, for the DECODER only, 32000
+ * (the reference's 32 kHz API, AGR_BWE_SDK_API.c:86-94,196-200: 16 kHz SILK core with order-16 LPC, 8-16 kHz high band).
+ *   - 32 kHz decoding covers every packet configuration above, in both decoder arithmetics (the fixed-point one with 40 ms
+ *     packets and joint mode 1, as at 16 kHz).  PCM rows are 32 * framesize_ms samples (1280 or 640); the drop-in
+ *     AGR_Sate_Decoder_Decode reports *nSamplesOut = 1280 / 640.
+ *   - Core rate: a 32 kHz stream decodes when its SILK core is 16 kHz.  The reference encoder chooses its core from the core
+ *     bitrate (user rate - 1600, or - 800 with joint mode 1; SKP_Silk_control_audio_bandwidth.c:38-114): see INTEGRATION.md
+ *     for the user rates that keep the 16 kHz core.  A frame that codes another core rate (8 or 12 kHz, which the reference
+ *     would resample to 16 kHz) is that stream's error, ret = -12, exactly like a corrupted packet; the other streams of the
+ *     batch are not affected.
+ *   - There is no 32 kHz ENCODER yet: solo_b200_enc_batch_create and AGR_Sate_Encoder_Init return NULL for samplerate 32000,
+ *     with solo_b200_last_error() saying so.
+ *
+ * Layouts (row = stream):  pcm  int16 [N][samplerate / 1000 * framesize_ms]   bits uint8 [N][cap]
  *                          nbytes int16 [N][2]        ({total, len(MD2)+8} as the single-stream API)
  *                          lostflag int32 [N]         (1 lost, 2 MD1 only, 3 MD2+HB only, 4 both)
  * For decode, row i of `bits` holds the payload exactly as the caller would hand it to
@@ -95,6 +108,11 @@ int solo_b200_enc_batch_export_state(solo_b200_enc_batch *b, int idx, void *blob
 int solo_b200_enc_batch_import_state(solo_b200_enc_batch *b, int idx, const void *blob);
 int solo_b200_dec_batch_export_state(solo_b200_dec_batch *b, int idx, void *blob);
 int solo_b200_dec_batch_import_state(solo_b200_dec_batch *b, int idx, const void *blob);
+/* The decoder forms with the blob's size: -1 (nothing copied, solo_b200_last_error() set) when blob_bytes is not the batch's
+   solo_b200_dec_state_bytes_rate(samplerate), i.e. for a blob of a stream of the other sample rate.  The unsized forms
+   above trust the caller's blob to be of the batch's rate. */
+int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch *b, int idx, void *blob, int blob_bytes);
+int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch *b, int idx, const void *blob, int blob_bytes);
 
 /* Packet framing around one payload row [MD1 | MD2 | HB] (reference drivers enc_main.c:212-234, dec_main.c:196-307, README
    "Bitstream sending" / "Bitstream screening and synthesis at receiver").  Host functions, no GPU involved.
@@ -126,9 +144,11 @@ int solo_b200_enable_peer_access(int device, int peer_device);
    slots in use}. */
 int solo_b200_arena_stats(int out[4]);
 
-/* Bytes of device state held per stream (encoder / decoder). */
+/* Bytes of device state held per stream (encoder / 16 kHz decoder; decoder of a sample rate, 16000 or 32000, -1 for any
+   other). */
 int solo_b200_enc_state_bytes(void);
 int solo_b200_dec_state_bytes(void);
+int solo_b200_dec_state_bytes_rate(int samplerate);
 /* Number of kernels this library has launched in this process (for benchmark bookkeeping). */
 long long solo_b200_kernel_launches(void);
 /* Kernel timing with CUDA events recorded on the launching stream (only while enabled).  profile_read fills two arrays

@@ -63,6 +63,8 @@ def lib():
         for f in ("solo_b200_enc_batch_export_state", "solo_b200_enc_batch_import_state", "solo_b200_dec_batch_export_state",
                   "solo_b200_dec_batch_import_state"):
             getattr(L, f).argtypes = [vp, C.c_int, vp]
+        for f in ("solo_b200_dec_batch_export_state_sized", "solo_b200_dec_batch_import_state_sized"):
+            getattr(L, f).argtypes = [vp, C.c_int, vp, C.c_int]
         pp, ip = C.POINTER(vp), C.POINTER(C.c_int)
         L.solo_b200_split_packet.argtypes = [vp, vp, pp, ip, pp, ip]
         L.solo_b200_merge_packets.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp]
@@ -72,6 +74,8 @@ def lib():
         L.solo_b200_enable_peer_access.argtypes = [C.c_int, C.c_int]
         L.solo_b200_enc_state_bytes.restype = C.c_int
         L.solo_b200_dec_state_bytes.restype = C.c_int
+        L.solo_b200_dec_state_bytes_rate.restype = C.c_int
+        L.solo_b200_dec_state_bytes_rate.argtypes = [C.c_int]
         L.solo_b200_profile_enable.argtypes = [C.c_int]
         L.solo_b200_profile_read.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_longlong)]
         L.AGR_Sate_Encoder_Init.restype = vp
@@ -98,6 +102,14 @@ def kernel_launches():
 
 def state_bytes():
     return int(lib().solo_b200_enc_state_bytes()), int(lib().solo_b200_dec_state_bytes())
+
+
+def dec_state_bytes(samplerate=16000):
+    """Bytes of device state per decoder stream of a sample rate (16000 or 32000)."""
+    n = int(lib().solo_b200_dec_state_bytes_rate(int(samplerate)))
+    if n < 0:
+        raise SoloError("no decoder for sample rate %r" % (samplerate,))
+    return n
 
 
 def profile_enable(on=True):
@@ -148,16 +160,17 @@ class SoloEncoder:
 
 
 class SoloDecoder:
-    """One stream through AGR_Sate_Decoder_Init / Decode / Uninit (payload pre-trimmed by the caller)."""
+    """One stream through AGR_Sate_Decoder_Init / Decode / Uninit (payload pre-trimmed by the caller).  samplerate 16000
+    or 32000 (the latter: decoder only, a 16 kHz SILK core; see include/solo_b200.h)."""
 
     def __init__(self, use_md_index=0, samplerate=16000, framesize_ms=40, joint_enable=0, joint_mode=0):
         self.ctrl = DecCtrl(0, samplerate, framesize_ms, joint_enable, joint_mode, use_md_index)
         self.h = lib().AGR_Sate_Decoder_Init(C.byref(self.ctrl))
         if not self.h:
             raise SoloError("AGR_Sate_Decoder_Init returned NULL: " + _err())
-        self._out = np.zeros(960, np.int16)
+        self._out = np.zeros(1920, np.int16)
         self._ns = C.c_int16(0)
-        self.samples = 16 * framesize_ms
+        self.samples = samplerate // 1000 * framesize_ms
 
     def decode(self, payload, nbytes, lostflag):
         buf = np.zeros(1040, np.uint8)
@@ -264,21 +277,23 @@ DEC_ARITH = {"flp": 0, "fix": 1}   # SOLO_B200_DEC_FLP / SOLO_B200_DEC_FIX
 class DecoderBatch:
     """N decoder streams resident on one GPU."""
 
-    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0, arith="flp"):
+    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000):
         """arith: "flp" decodes to the reference float build's PCM, "fix" to its fixed-point build's (40 ms packets and
-        joint mode 1 only; see solo_b200_dec_batch_create_arith in include/solo_b200.h)."""
+        joint mode 1 only; see solo_b200_dec_batch_create_arith in include/solo_b200.h).  samplerate: 16000, or 32000 for
+        streams of the reference's 32 kHz API (16 kHz SILK core; PCM rows of 32 * framesize_ms samples)."""
         if arith not in DEC_ARITH:
             raise SoloError("arith must be one of %s, not %r" % (sorted(DEC_ARITH), arith))
         self.n = int(n)
-        self.samples = 16 * framesize_ms
+        self.samplerate = int(samplerate)
+        self.samples = self.samplerate // 1000 * framesize_ms
         self.arith = arith
-        self.ctrl = DecCtrl(0, 16000, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
+        self.ctrl = DecCtrl(0, self.samplerate, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
         self.h = lib().solo_b200_dec_batch_create_arith(self.n, C.byref(self.ctrl), device, DEC_ARITH[arith])
         if not self.h:
             raise SoloError("solo_b200_dec_batch_create failed: " + _err())
 
     def decode(self, bits, nbytes, lostflag, pcm=None, ret=None):
-        """bits uint8 [N, cap], nbytes int16 [N, 2], lostflag int32 [N] -> (pcm int16 [N, 640], ret int32 [N])."""
+        """bits uint8 [N, cap], nbytes int16 [N, 2], lostflag int32 [N] -> (pcm int16 [N, samples], ret int32 [N])."""
         bits = np.ascontiguousarray(bits, dtype=np.uint8)
         nbytes = np.ascontiguousarray(nbytes, dtype=np.int16)
         lostflag = np.ascontiguousarray(lostflag, dtype=np.int32)
@@ -299,14 +314,15 @@ class DecoderBatch:
             raise SoloError("decode_host failed (%d): %s" % (r, _err()))
 
     def export_state(self, idx):
-        blob = np.zeros(lib().solo_b200_dec_state_bytes(), np.uint8)
-        if lib().solo_b200_dec_batch_export_state(self.h, int(idx), blob.ctypes.data):
+        blob = np.zeros(lib().solo_b200_dec_state_bytes_rate(self.samplerate), np.uint8)
+        if lib().solo_b200_dec_batch_export_state_sized(self.h, int(idx), blob.ctypes.data, blob.size):
             raise SoloError(_err())
         return blob
 
     def import_state(self, idx, blob):
+        """A blob of export_state from a batch of the same sample rate (another rate's blob is refused)."""
         blob = np.ascontiguousarray(blob, np.uint8)
-        if blob.size != lib().solo_b200_dec_state_bytes() or lib().solo_b200_dec_batch_import_state(self.h, int(idx), blob.ctypes.data):
+        if lib().solo_b200_dec_batch_import_state_sized(self.h, int(idx), blob.ctypes.data, blob.size):
             raise SoloError("import_state: " + _err())
 
     def decode_device(self, d_pcm, d_bits, cap, d_nbytes, d_flags, d_ret=0, stream=0):

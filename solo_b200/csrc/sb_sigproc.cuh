@@ -669,38 +669,52 @@ SB_FN void nlsf_vq_weights_laroia(i32* pW_Q6, const i32* pNLSF_Q15, int D) {
     pW_Q6[D - 1] = imin(t1 + t2, 32767);
 }
 
-// ---- NLSF codebook accessors (tables_NLSF_CB{0,1}_10.c) ----------------------------------------------
+// ---- NLSF codebook accessors (tables_NLSF_CB{0,1}_10.c; order 16: tables_NLSF_CB{0,1}_16.c) ----------------------------
 struct NlsfCb {
     const i16* cb_q15;       // all stages, concatenated
     const i16* rates_q5;
-    const i32* ndelta_min;   // [LPC_ORDER + 1]
-    const i32* nvec;         // [6]
+    const i32* ndelta_min;   // [order + 1]
+    const i32* nvec;         // [stages]: 6 at order 10, 10 at order 16
     const u16* cdf;
-    const i32* cdf_start;    // [6] element offsets into cdf
-    const i32* cdf_mid;      // [6]
+    const i32* cdf_start;    // [stages] element offsets into cdf
+    const i32* cdf_mid;      // [stages]
 };
-SB_HD NlsfCb nlsf_cb(int sigtype) {
+template <int D = 10> SB_HD NlsfCb nlsf_cb(int sigtype) {
+    static_assert(D == 10 || D == 16, "NLSF codebooks exist for orders 10 and 16");
     NlsfCb c;
-    if (sigtype == 0) {
-        c.cb_q15 = SB_T(nlsf_cb0_q15); c.rates_q5 = SB_T(nlsf_cb0_rates_q5); c.ndelta_min = SB_T(nlsf_cb0_ndelta_min_q15);
-        c.nvec = SB_T(nlsf_cb0_nvec); c.cdf = SB_T(nlsf_cb0_cdf); c.cdf_start = SB_T(nlsf_cb0_cdf_start); c.cdf_mid = SB_T(nlsf_cb0_cdf_mid);
+    if constexpr (D == 10) {
+        if (sigtype == 0) {
+            c.cb_q15 = SB_T(nlsf_cb0_q15); c.rates_q5 = SB_T(nlsf_cb0_rates_q5); c.ndelta_min = SB_T(nlsf_cb0_ndelta_min_q15);
+            c.nvec = SB_T(nlsf_cb0_nvec); c.cdf = SB_T(nlsf_cb0_cdf); c.cdf_start = SB_T(nlsf_cb0_cdf_start); c.cdf_mid = SB_T(nlsf_cb0_cdf_mid);
+        } else {
+            c.cb_q15 = SB_T(nlsf_cb1_q15); c.rates_q5 = SB_T(nlsf_cb1_rates_q5); c.ndelta_min = SB_T(nlsf_cb1_ndelta_min_q15);
+            c.nvec = SB_T(nlsf_cb1_nvec); c.cdf = SB_T(nlsf_cb1_cdf); c.cdf_start = SB_T(nlsf_cb1_cdf_start); c.cdf_mid = SB_T(nlsf_cb1_cdf_mid);
+        }
     } else {
-        c.cb_q15 = SB_T(nlsf_cb1_q15); c.rates_q5 = SB_T(nlsf_cb1_rates_q5); c.ndelta_min = SB_T(nlsf_cb1_ndelta_min_q15);
-        c.nvec = SB_T(nlsf_cb1_nvec); c.cdf = SB_T(nlsf_cb1_cdf); c.cdf_start = SB_T(nlsf_cb1_cdf_start); c.cdf_mid = SB_T(nlsf_cb1_cdf_mid);
+        if (sigtype == 0) {
+            c.cb_q15 = SB_T(nlsf16_cb0_q15); c.rates_q5 = SB_T(nlsf16_cb0_rates_q5); c.ndelta_min = SB_T(nlsf16_cb0_ndelta_min_q15);
+            c.nvec = SB_T(nlsf16_cb0_nvec); c.cdf = SB_T(nlsf16_cb0_cdf); c.cdf_start = SB_T(nlsf16_cb0_cdf_start); c.cdf_mid = SB_T(nlsf16_cb0_cdf_mid);
+        } else {
+            c.cb_q15 = SB_T(nlsf16_cb1_q15); c.rates_q5 = SB_T(nlsf16_cb1_rates_q5); c.ndelta_min = SB_T(nlsf16_cb1_ndelta_min_q15);
+            c.nvec = SB_T(nlsf16_cb1_nvec); c.cdf = SB_T(nlsf16_cb1_cdf); c.cdf_start = SB_T(nlsf16_cb1_cdf_start); c.cdf_mid = SB_T(nlsf16_cb1_cdf_mid);
+        }
     }
     return c;
 }
-// SKP_Silk_NLSF_MSVQ_decode.c:31-98 (order 10, 6 stages)
-SB_FN void nlsf_msvq_decode(i32* pNLSF_Q15, const NlsfCb& cb, const i32* idx) {
-    const i16* e = cb.cb_q15 + idx[0] * 10;
-    for (int i = 0; i < 10; i++) pNLSF_Q15[i] = e[i];
+// number of MSVQ stages of the order-D codebooks
+template <int D> struct NlsfStages { enum { N = D == 16 ? 10 : 6 }; };
+// SKP_Silk_NLSF_MSVQ_decode.c:31-98 (order 10 with 6 stages, order 16 with 10)
+template <int D = 10> SB_FN void nlsf_msvq_decode(i32* pNLSF_Q15, const NlsfCb& cb, const i32* idx) {
+    enum { NST = NlsfStages<D>::N };
+    const i16* e = cb.cb_q15 + idx[0] * D;
+    for (int i = 0; i < D; i++) pNLSF_Q15[i] = e[i];
     int base = cb.nvec[0];
-    for (int s = 1; s < 6; s++) {
-        e = cb.cb_q15 + (base + idx[s]) * 10;
-        for (int i = 0; i < 10; i++) pNLSF_Q15[i] += e[i];
+    for (int s = 1; s < NST; s++) {
+        e = cb.cb_q15 + (base + idx[s]) * D;
+        for (int i = 0; i < D; i++) pNLSF_Q15[i] += e[i];
         base += cb.nvec[s];
     }
-    nlsf_stabilize(pNLSF_Q15, cb.ndelta_min, 10);
+    nlsf_stabilize(pNLSF_Q15, cb.ndelta_min, D);
 }
 
 }  // namespace sb

@@ -11,6 +11,8 @@
 //   sb_enc_finish_kernel         2 threads per stream  range coding of one description each, high-band gains, payload assembly
 //   sb_decode_kernel             thread per stream     range decoding, synthesis, concealment, comfort noise, high band
 //   sb_dec_synth_kernel          warp per stream       QMF synthesis filter bank + float -> int16
+// The two decoder kernels exist once per SILK core rate (template argument KHZ): 8 for 16 kHz streams, 16 for 32 kHz
+// streams.  A batch holds one configuration, so it picks its instantiation when it is created.
 // Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
@@ -187,18 +189,20 @@ __global__ void __launch_bounds__(SB_TPB, SB_FINISH_MINB) sb_enc_finish_kernel(E
 }
 
 static_assert(SOLO_B200_DEC_FLP == DEC_FLP && SOLO_B200_DEC_FIX == DEC_FIX, "decoder arithmetic codes");
-__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecState* states, int n, int mdi, int framesize_ms, int joint_hb, int arith) {
+template <int KHZ>
+__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecStateT<KHZ>* states, int n, int mdi, int framesize_ms, int joint_hb, int arith) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb, arith);
 }
 
-__global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(DecState* states, const u8* __restrict__ bits, int cap,
+template <int KHZ>
+__global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(DecStateT<KHZ>* states, const u8* __restrict__ bits, int cap,
                                                            const i16* __restrict__ nbytes, const i32* __restrict__ lostflag,
                                                            i32* __restrict__ ret, i32* __restrict__ ret_int, DecStale* stale,
                                                            i16* __restrict__ band_low, float* __restrict__ band_high, int spp, int n) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
-    DecPacketWork W;
+    DecPacketWorkT<KHZ> W;
     i16 nb[2] = {nbytes[2 * s], nbytes[2 * s + 1]};
     const DecBands bands = {band_low + (size_t)s * (spp / 2), band_high + (size_t)s * (spp / 2)};
     i32 r = dec_packet(&states[s], &W, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
@@ -207,8 +211,8 @@ __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(D
 }
 
 // ---- synthesis filter bank + float -> int16, one warp per stream (AGR_BWE_qmf.c:86-182, AGR_BWE_decode_frame_FLP.c:222-231) ----
-// 160 (80) independent groups of four outputs per packet: lanes over groups, band signals and filter memories staged in
-// shared memory; the PCM row is written with 8-byte stores, 256 contiguous bytes per warp instruction.  A DEC_FIX stream
+// N2 / 2 independent groups of four outputs per packet (160 or 80 for 16 kHz streams, twice that for 32 kHz): lanes over
+// groups, band signals and filter memories staged in shared memory; the PCM row is written with 8-byte stores, 256 contiguous bytes per warp instruction.  A DEC_FIX stream
 // takes the integer filter bank in the same layout, its band signals staged as int16 in the first half of each row.
 #define SB_SYN_WARPS 4
 __device__ __forceinline__ void store_pcm4(i16* out, int g, const i16* y) {
@@ -217,9 +221,10 @@ __device__ __forceinline__ void store_pcm4(i16* out, int g, const i16* y) {
     pk.y = (int)((u16)y[2] | ((u32)(u16)y[3] << 16));
     reinterpret_cast<int2*>(out)[g] = pk;
 }
-__global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecState* states, const i16* __restrict__ band_low, const float* __restrict__ band_high,
+template <int KHZ>
+__global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecStateT<KHZ>* states, const i16* __restrict__ band_low, const float* __restrict__ band_high,
                                                                         const i32* __restrict__ ret_int, i16* __restrict__ pcm, int spp, int n) {
-    __shared__ float xx[SB_SYN_WARPS][2][32 + PACKET / 2];
+    __shared__ float xx[SB_SYN_WARPS][2][32 + 2 * DecCore<KHZ>::FRAME];
     __shared__ float coef[64];
     __shared__ i16 coef_fix[64];
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -230,7 +235,7 @@ __global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecStat
     const int N2 = spp >> 1;
     float* xx1 = xx[w][0];
     float* xx2 = xx[w][1];
-    DecState* st = &states[s];
+    DecStateT<KHZ>* st = &states[s];
     const i16* lo = band_low + (size_t)s * N2;
     const float* hi = band_high + (size_t)s * N2;
     i16* out = pcm + (size_t)s * spp;
@@ -377,7 +382,8 @@ struct solo_b200_enc_batch : Batch {
     ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); cudaFree(d_ctrl); }
 };
 struct solo_b200_dec_batch : Batch {
-    DecState* d_states;
+    int khz;                    // SILK core rate: 8 (16 kHz streams, DecState) or 16 (32 kHz streams, DecState32)
+    void* d_states;             // DecStateT<khz>[n]
     DecStale* d_stale;          // payload copies that outlive a packet call (only touched after a corrupted packet, see sb_dec.cuh)
     i32* d_flags; i32* d_ret;   // staging for the *_host entry points and the arena
     i16* d_band_low; float* d_band_high; i32* d_ret_int;   // decoder kernel -> synthesis kernel
@@ -387,15 +393,19 @@ struct solo_b200_dec_batch : Batch {
     }
 };
 
-// Supported configurations (AGR_BWE_SDK_API.c:40-81): 16 kHz input; no joint coding with 40 or 20 ms packets ("40ms 2MD",
-// "20ms 2MD"); joint mode 1 (one 40 ms high-band frame per 40 ms packet).  Joint modes 0, 2, 3 are "Unsupport" in the
-// reference as well; 32 kHz input is out of scope here.
+// Supported configurations (AGR_BWE_SDK_API.c:40-81): no joint coding with 40 or 20 ms packets ("40ms 2MD", "20ms 2MD");
+// joint mode 1 (one 40 ms high-band frame per 40 ms packet).  Joint modes 0, 2, 3 are "Unsupport" in the reference as
+// well.  16 kHz streams encode and decode; 32 kHz streams (AGR_BWE_SDK_API.c:86-94,196-200) only decode so far.
 static int check_modes(int samplerate, int framesize_ms, int joint_enable, int joint_mode) {
-    if (samplerate != 16000) return -1;
+    if (samplerate != 16000 && samplerate != 32000) return -1;
     if (!joint_enable) return (framesize_ms == 40 || framesize_ms == 20) ? 0 : -1;
     return (joint_mode == 1 && framesize_ms == 40) ? 0 : -1;
 }
-static int check_enc_ctrl(const USER_Ctrl_enc* c) { return c ? check_modes(c->samplerate, c->framesize_ms, c->joint_enable, c->joint_mode) : -1; }
+static int check_enc_ctrl(const USER_Ctrl_enc* c) {
+    if (c && c->samplerate == 32000) { snprintf(g_err, sizeof g_err, "the 32 kHz encoder is not built yet (32 kHz streams can only be decoded)"); return -1; }
+    if (!c || check_modes(c->samplerate, c->framesize_ms, c->joint_enable, c->joint_mode)) { snprintf(g_err, sizeof g_err, "bad encoder configuration"); return -1; }
+    return 0;
+}
 static int check_dec_ctrl(const USER_Ctrl_dec* c) { return c ? check_modes(c->samplerate, c->framesize_ms, c->joint_enable, c->joint_mode) : -1; }
 static int hb_bytes_of(int framesize_ms, int joint_enable) { return joint_enable ? 4 : 4 * (framesize_ms / 20); }
 
@@ -413,8 +423,8 @@ static int require_gpu(int device) {
 }
 
 // the packet layout and `nst` CUDA streams of a new batch; false when a stream cannot be created
-static bool batch_setup(Batch* b, int n, int device, int framesize_ms, int joint_enable, int nst) {
-    b->n = n; b->device = device; b->spp = 16 * framesize_ms; b->hb_bytes = hb_bytes_of(framesize_ms, joint_enable);
+static bool batch_setup(Batch* b, int n, int device, int samplerate, int framesize_ms, int joint_enable, int nst) {
+    b->n = n; b->device = device; b->spp = samplerate / 1000 * framesize_ms; b->hb_bytes = hb_bytes_of(framesize_ms, joint_enable);
     for (; b->nst < nst; b->nst++)
         if (cudaStreamCreateWithFlags(&b->st[b->nst], cudaStreamNonBlocking) != cudaSuccess) return false;
     return true;
@@ -465,11 +475,18 @@ template <class F> static int host_chunks(Batch* b, F f) {
 }
 
 // ---- stream state hand-over (checkpoint / migration, SURVEY.md 8(f) rank 3) ----------------------------------------------
-template <class B> static int state_copy(B* b, int idx, void* host, int to_host) {
+static size_t state_stride(const solo_b200_enc_batch*) { return sizeof(EncState); }
+static size_t state_stride(const solo_b200_dec_batch* b) { return b->khz == 16 ? sizeof(DecState32) : sizeof(DecState); }
+// blob_bytes: the caller's blob size, or -1 when the caller did not say (the unsized entry points)
+template <class B> static int state_copy(B* b, int idx, void* host, int to_host, long long blob_bytes = -1) {
     if (!b || !host || idx < 0 || idx >= b->n) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    const size_t stride = state_stride(b);
+    if (blob_bytes >= 0 && (size_t)blob_bytes != stride) {
+        snprintf(g_err, sizeof g_err, "state blob of %lld bytes, this batch's streams have %zu (a stream of another sample rate?)", blob_bytes, stride);
+        return -1;
+    }
     CK(cudaSetDevice(b->device));
     CK(cudaDeviceSynchronize());    // packet waves run on the batch's streams and on caller streams: wait for all of them
-    const size_t stride = sizeof *b->d_states;
     char* p = (char*)b->d_states + stride * (size_t)idx;
     if (to_host) CK(cudaMemcpy(host, p, stride, cudaMemcpyDeviceToHost));
     else CK(cudaMemcpy(p, host, stride, cudaMemcpyHostToDevice));
@@ -482,6 +499,9 @@ const char* solo_b200_last_error(void) { return g_err; }
 long long solo_b200_kernel_launches(void) { std::lock_guard<std::mutex> lk(g_mu); return g_launches; }
 int solo_b200_enc_state_bytes(void) { return (int)sizeof(EncState); }
 int solo_b200_dec_state_bytes(void) { return (int)sizeof(DecState); }
+int solo_b200_dec_state_bytes_rate(int samplerate) {
+    return samplerate == 16000 ? (int)sizeof(DecState) : samplerate == 32000 ? (int)sizeof(DecState32) : -1;
+}
 void solo_b200_set_chunks(int chunks) { g_chunks = chunks < 0 ? 0 : (chunks > 64 ? 64 : chunks); }   // 0: the default
 void solo_b200_profile_enable(int on) {
     std::lock_guard<std::mutex> lk(g_mu);
@@ -506,10 +526,11 @@ int solo_b200_profile_read(double* ms_total, long long* launches) {
 
 // ---- encoder batch --------------------------------------------------------------------------------
 static solo_b200_enc_batch* enc_batch_create_impl(int n_streams, const USER_Ctrl_enc* ctrl, int device, int nst) {
-    if (n_streams <= 0 || check_enc_ctrl(ctrl)) { snprintf(g_err, sizeof g_err, "bad encoder configuration"); return nullptr; }
+    if (n_streams <= 0) { snprintf(g_err, sizeof g_err, "bad encoder configuration"); return nullptr; }
+    if (check_enc_ctrl(ctrl)) return nullptr;
     if (require_gpu(device)) return nullptr;
     solo_b200_enc_batch* b = new solo_b200_enc_batch();
-    if (!batch_setup(b, n_streams, device, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
+    if (!batch_setup(b, n_streams, device, ctrl->samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
         cudaMalloc(&b->d_states, sizeof(EncState) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_scratch, sizeof(EncScratch) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_bands, sizeof(i16) * (size_t)b->spp * (size_t)n_streams) != cudaSuccess ||
@@ -644,13 +665,21 @@ static int check_dec_arith(const USER_Ctrl_dec* c, int arith) {
     }
     return 0;
 }
+// (re)initialise streams [lo, lo + n) of a decoder batch on its first CUDA stream
+static void dec_init_launch(solo_b200_dec_batch* b, int lo, int n, int mdi, int framesize_ms, int joint_enable, int arith) {
+    const int g = (n + SB_TPB - 1) / SB_TPB, joint = joint_enable ? 1 : 0;
+    if (b->khz == 16) sb_dec_init_kernel<16><<<g, SB_TPB, 0, b->st[0]>>>((DecState32*)b->d_states + lo, n, mdi, framesize_ms, joint, arith);
+    else sb_dec_init_kernel<8><<<g, SB_TPB, 0, b->st[0]>>>((DecState*)b->d_states + lo, n, mdi, framesize_ms, joint, arith);
+    count_launch();
+}
 static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst, int arith) {
     if (n_streams <= 0 || check_dec_ctrl(ctrl)) { snprintf(g_err, sizeof g_err, "bad decoder configuration"); return nullptr; }
     if (check_dec_arith(ctrl, arith)) return nullptr;
     if (require_gpu(device)) return nullptr;
     solo_b200_dec_batch* b = new solo_b200_dec_batch();
-    if (!batch_setup(b, n_streams, device, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
-        cudaMalloc(&b->d_states, sizeof(DecState) * (size_t)n_streams) != cudaSuccess ||
+    b->khz = ctrl->samplerate == 32000 ? 16 : 8;
+    if (!batch_setup(b, n_streams, device, ctrl->samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
+        cudaMalloc(&b->d_states, state_stride(b) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_stale, sizeof(DecStale) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_band_low, sizeof(i16) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_band_high, sizeof(float) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
@@ -658,9 +687,7 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
         fail("dec_batch_create", cudaGetLastError());
         return batch_destroy(b);
     }
-    sb_dec_init_kernel<<<(n_streams + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0,
-                                                                              arith);
-    count_launch();
+    dec_init_launch(b, 0, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable, arith);
     cudaError_t e = cudaStreamSynchronize(b->st[0]);
     if (e != cudaSuccess) { fail("dec init kernel", e); return batch_destroy(b); }
     return b;
@@ -672,16 +699,26 @@ solo_b200_dec_batch* solo_b200_dec_batch_create_arith(int n_streams, const USER_
     return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith);
 }
 
+// the two decoder kernels of core rate KHZ for streams [lo, lo + n) of b
+extern "C++" {
+template <int KHZ>
+static void dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
+                        i32* d_ret, cudaStream_t st) {
+    DecStateT<KHZ>* states = (DecStateT<KHZ>*)b->d_states + lo;
+    const size_t half = (size_t)(b->spp / 2);
+    sb_decode_kernel<KHZ><<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(states, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, d_lostflag + lo,
+                                                                       d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_stale + lo,
+                                                                       b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half, b->spp, n);
+    sb_dec_synth_kernel<KHZ><<<(n + SB_SYN_WARPS - 1) / SB_SYN_WARPS, SB_SYN_WARPS * 32, 0, st>>>(states, b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half,
+                                                                                               b->d_ret_int + lo, d_pcm + (size_t)lo * b->spp, b->spp, n);
+}
+}  // extern "C++"
 static int dec_launch(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
                       i32* d_ret, cudaStream_t st) {
     if (n <= 0) return 0;
     EvPair ev; prof_begin(st, 3, &ev);
-    const size_t half = (size_t)(b->spp / 2);
-    sb_decode_kernel<<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(b->d_states + lo, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, d_lostflag + lo,
-                                                                  d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_stale + lo,
-                                                                  b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half, b->spp, n);
-    sb_dec_synth_kernel<<<(n + SB_SYN_WARPS - 1) / SB_SYN_WARPS, SB_SYN_WARPS * 32, 0, st>>>(b->d_states + lo, b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half,
-                                                                                          b->d_ret_int + lo, d_pcm + (size_t)lo * b->spp, b->spp, n);
+    if (b->khz == 16) dec_kernels<16>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
+    else dec_kernels<8>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
     prof_end(st, &ev);
     count_launch(); count_launch();
     CK(cudaGetLastError());
@@ -719,6 +756,12 @@ int solo_b200_enc_batch_export_state(solo_b200_enc_batch* b, int idx, void* blob
 int solo_b200_enc_batch_import_state(solo_b200_enc_batch* b, int idx, const void* blob) { return state_copy(b, idx, (void*)blob, 0); }
 int solo_b200_dec_batch_export_state(solo_b200_dec_batch* b, int idx, void* blob) { return state_copy(b, idx, blob, 1); }
 int solo_b200_dec_batch_import_state(solo_b200_dec_batch* b, int idx, const void* blob) { return state_copy(b, idx, (void*)blob, 0); }
+int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch* b, int idx, void* blob, int blob_bytes) {
+    return state_copy(b, idx, blob, 1, blob_bytes < 0 ? 0 : blob_bytes);
+}
+int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch* b, int idx, const void* blob, int blob_bytes) {
+    return state_copy(b, idx, (void*)blob, 0, blob_bytes < 0 ? 0 : blob_bytes);
+}
 
 // ---- packet framing (host, no GPU involved): enc_main.c:212-234 / dec_main.c:196-307 / README "Bitstream sending" --------
 int solo_b200_split_packet(const uint8_t* bits, const int16_t* nbytes, const uint8_t** p1, int* n1, const uint8_t** p2, int* n2) {
@@ -802,7 +845,7 @@ int solo_b200_enable_peer_access(int device, int peer_device) {
 // Same names / return conventions as AGR_BWE_SDK_API.c:11-296 and libBWE/AGR_BWE_init.c:6-76.
 extern "C++" {
 static constexpr int SB_ARENA_SEG = 256;
-struct ArenaKey { int device, framesize_ms, joint; };
+struct ArenaKey { int device, samplerate, framesize_ms, joint; };
 template <class B> struct ArenaSeg {
     ArenaKey key;
     B* b;
@@ -820,7 +863,8 @@ static std::vector<ArenaSeg<solo_b200_dec_batch>*> g_dec_segs;
 
 template <class B> static ArenaSeg<B>* arena_take(std::vector<ArenaSeg<B>*>& segs, ArenaKey k, int* slot) {
     for (auto* sg : segs)
-        if (sg->key.device == k.device && sg->key.framesize_ms == k.framesize_ms && sg->key.joint == k.joint && sg->n_used < SB_ARENA_SEG)
+        if (sg->key.device == k.device && sg->key.samplerate == k.samplerate && sg->key.framesize_ms == k.framesize_ms && sg->key.joint == k.joint &&
+            sg->n_used < SB_ARENA_SEG)
             for (int i = 0; i < SB_ARENA_SEG; i++)
                 if (!sg->used[i]) { sg->used[i] = 1; sg->n_used++; *slot = i; return sg; }
     return nullptr;
@@ -832,11 +876,11 @@ template <class B> static void arena_release(ArenaSeg<B>* sg, int slot) {   // u
 // A slot on the current device: a free one of a segment with this packet layout, or the first one of a new segment made by
 // create(device).  init(batch, slot) enqueues the (re)initialisation of that one stream with the caller's settings.
 template <class B, class Create, class Init>
-static Handle<B>* arena_open(std::vector<ArenaSeg<B>*>& segs, unsigned magic, int framesize_ms, int joint_enable, const char* who, const char* what,
-                             Create create, Init init) {
+static Handle<B>* arena_open(std::vector<ArenaSeg<B>*>& segs, unsigned magic, int samplerate, int framesize_ms, int joint_enable, const char* who,
+                             const char* what, Create create, Init init) {
     int dev = 0;
     cudaGetDevice(&dev);
-    const ArenaKey k = {dev, framesize_ms, joint_enable ? 1 : 0};
+    const ArenaKey k = {dev, samplerate, framesize_ms, joint_enable ? 1 : 0};
     std::lock_guard<std::mutex> lk(g_arena_mu);
     int slot = -1;
     auto* sg = arena_take(segs, k, &slot);
@@ -852,7 +896,6 @@ static Handle<B>* arena_open(std::vector<ArenaSeg<B>*>& segs, unsigned magic, in
         std::lock_guard<std::mutex> lk2(sg->mu);
         cudaSetDevice(dev);
         init(sg->b, slot);
-        count_launch();
         if (cudaStreamSynchronize(sg->b->st[0]) != cudaSuccess) { arena_release(sg, slot); fprintf(stderr, "solo_b200: %s slot init failed\n", what); return nullptr; }
     }
     return new Handle<B>{magic, sg, slot};
@@ -877,12 +920,13 @@ void* AGR_Sate_Encoder_Init(USER_Ctrl_enc* enc_Ctrl) {
         printf("Error in setting joint mode! It must be 0, 1, 2, 3\n");
         return nullptr;
     }
-    if (check_enc_ctrl(enc_Ctrl)) { fprintf(stderr, "solo_b200: AGR_Sate_Encoder_Init: unsupported configuration\n"); return nullptr; }
-    return arena_open(g_enc_segs, ENC_MAGIC, enc_Ctrl->framesize_ms, enc_Ctrl->joint_enable, "AGR_Sate_Encoder_Init", "encoder",
+    if (check_enc_ctrl(enc_Ctrl)) { fprintf(stderr, "solo_b200: AGR_Sate_Encoder_Init: unsupported configuration: %s\n", g_err); return nullptr; }
+    return arena_open(g_enc_segs, ENC_MAGIC, enc_Ctrl->samplerate, enc_Ctrl->framesize_ms, enc_Ctrl->joint_enable, "AGR_Sate_Encoder_Init", "encoder",
                       [&](int dev) { return enc_batch_create_impl(SB_ARENA_SEG, enc_Ctrl, dev, 1); },
                       [&](solo_b200_enc_batch* b, int slot) {   // the caller's rate / DTX / MD-index settings
                           sb_enc_init_kernel<<<1, SB_TPB, 0, b->st[0]>>>(b->d_states + slot, 1, enc_Ctrl->targetRate_bps, enc_Ctrl->dtx_enable, enc_Ctrl->useMDIndex,
                                                                         enc_Ctrl->framesize_ms, enc_Ctrl->joint_enable ? 1 : 0);
+                          count_launch();
                       });
 }
 SKP_int32 AGR_Sate_Encoder_Encode(void* SATEEnc_State, const SKP_int16* AGR_Sate_PCM, SKP_uint8* AGR_Sate_Bit, SKP_int32 AGR_Sate_Buf_Size,
@@ -934,7 +978,11 @@ void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
         fprintf(stderr, "Error in setting joint mode! It must be 0, 1, 2, 3\n");
         return nullptr;
     }
-    if (check_dec_ctrl(dec_Ctrl)) { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: unsupported configuration\n"); return nullptr; }
+    if (check_dec_ctrl(dec_Ctrl)) {
+        snprintf(g_err, sizeof g_err, "bad decoder configuration");
+        fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: unsupported configuration\n");
+        return nullptr;
+    }
     // SOLO_B200_DEC_ARITH, read at every Init: unset or "flp" = the float build's PCM, "fix" = the fixed-point build's
     const char* e = getenv("SOLO_B200_DEC_ARITH");
     int arith;
@@ -943,11 +991,10 @@ void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
     else { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: SOLO_B200_DEC_ARITH must be \"flp\" or \"fix\", not \"%s\"\n", e); return nullptr; }
     if (check_dec_arith(dec_Ctrl, arith)) { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: %s\n", g_err); return nullptr; }
     // the arithmetic is a property of the slot, not of the segment: one segment holds handles of both kinds
-    return arena_open(g_dec_segs, DEC_MAGIC, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, "AGR_Sate_Decoder_Init", "decoder",
+    return arena_open(g_dec_segs, DEC_MAGIC, dec_Ctrl->samplerate, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, "AGR_Sate_Decoder_Init", "decoder",
                       [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1, SOLO_B200_DEC_FLP); },
                       [&](solo_b200_dec_batch* b, int slot) {
-                          sb_dec_init_kernel<<<1, SB_TPB, 0, b->st[0]>>>(b->d_states + slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable ? 1 : 0,
-                                                                        arith);
+                          dec_init_launch(b, slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, arith);
                       });
 }
 SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, SKP_int16* nSamplesOut, const SKP_uint8* AGR_Sate_Bit,

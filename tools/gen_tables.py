@@ -47,6 +47,17 @@ TABLES = [
     ("nlsf_cb1_cdf", "fix", "SKP_Silk_NLSF_MSVQ_CB1_10_CDF", U16, 78),
     ("nlsf_cb1_cdf_mid", "fix", "SKP_Silk_NLSF_MSVQ_CB1_10_CDF_middle_idx", I32, 6),
     ("lsf_cos_q12", "fix", "SKP_Silk_LSFCosTab_FIX_Q12", I32, 129),
+    # --- NLSF codebooks, order 16 (the 16 kHz core of 32 kHz streams) ---
+    ("nlsf16_cb0_q15", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_Q15", I16, 216 * 16),
+    ("nlsf16_cb0_rates_q5", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_rates_Q5", I16, 216),
+    ("nlsf16_cb0_ndelta_min_q15", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_ndelta_min_Q15", I32, 17),
+    ("nlsf16_cb0_cdf", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_CDF", U16, 226),
+    ("nlsf16_cb0_cdf_mid", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_CDF_middle_idx", I32, 10),
+    ("nlsf16_cb1_q15", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_Q15", I16, 104 * 16),
+    ("nlsf16_cb1_rates_q5", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_rates_Q5", I16, 104),
+    ("nlsf16_cb1_ndelta_min_q15", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_ndelta_min_Q15", I32, 17),
+    ("nlsf16_cb1_cdf", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_CDF", U16, 114),
+    ("nlsf16_cb1_cdf_mid", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_CDF_middle_idx", I32, 10),
     ("nlsf_interp_cdf", "fix", "SKP_Silk_NLSF_interpolation_factor_CDF", U16, 6),
     ("nlsf_interp_offset", "fix", "SKP_Silk_NLSF_interpolation_factor_offset", I32, 1),
     # --- LTP ---
@@ -74,6 +85,11 @@ TABLES = [
     ("pitch_lag_nb_offset", "fix", "SKP_Silk_pitch_lag_NB_CDF_offset", I32, 1),
     ("pitch_contour_nb_cdf", "fix", "SKP_Silk_pitch_contour_NB_CDF", U16, 12),
     ("pitch_contour_nb_offset", "fix", "SKP_Silk_pitch_contour_NB_CDF_offset", I32, 1),
+    ("pitch_lag_wb_cdf", "fix", "SKP_Silk_pitch_lag_WB_CDF", U16, 258),
+    ("pitch_lag_wb_offset", "fix", "SKP_Silk_pitch_lag_WB_CDF_offset", I32, 1),
+    ("pitch_contour_cdf", "fix", "SKP_Silk_pitch_contour_CDF", U16, 35),
+    ("pitch_contour_offset", "fix", "SKP_Silk_pitch_contour_CDF_offset", I32, 1),
+    ("pitch_cb_lags_stage3", "fix", "SKP_Silk_CB_lags_stage3", I16, 4 * 34),
     # --- gains ---
     ("gain_cdf", "fix", "SKP_Silk_gain_CDF", U16, 130),
     ("gain_cdf_offset", "fix", "SKP_Silk_gain_CDF_offset", I32, 1),
@@ -124,6 +140,8 @@ TABLES = [
 PTR_TABLES = [
     ("nlsf_cb0_cdf_start", "fix", "SKP_Silk_NLSF_MSVQ_CB0_10_CDF_start_ptr", 6, "SKP_Silk_NLSF_MSVQ_CB0_10_CDF", 2),
     ("nlsf_cb1_cdf_start", "fix", "SKP_Silk_NLSF_MSVQ_CB1_10_CDF_start_ptr", 6, "SKP_Silk_NLSF_MSVQ_CB1_10_CDF", 2),
+    ("nlsf16_cb0_cdf_start", "fix", "SKP_Silk_NLSF_MSVQ_CB0_16_CDF_start_ptr", 10, "SKP_Silk_NLSF_MSVQ_CB0_16_CDF", 2),
+    ("nlsf16_cb1_cdf_start", "fix", "SKP_Silk_NLSF_MSVQ_CB1_16_CDF_start_ptr", 10, "SKP_Silk_NLSF_MSVQ_CB1_16_CDF", 2),
 ]
 
 
@@ -183,12 +201,13 @@ def main():
         offs = [(p - base) // esz for p in ptrs]
         lines.append("SB_TAB(i32, %s, %d, %s)" % (name, n, ",".join(map(str, offs))))
     # NLSF stage sizes (from the Stage_info structs: nVectors is the first int32 of each 24-byte entry)
-    for cb in (0, 1):
-        L = libs["fix"]
-        off, size = L.tab["SKP_Silk_NLSF_CB%d_10_Stage_info" % cb]
-        raw = (C.c_uint8 * size).from_address(L.bias + off)
-        nv = [int.from_bytes(bytes(raw[i * 24:i * 24 + 4]), "little") for i in range(size // 24)]
-        lines.append("SB_TAB(i32, nlsf_cb%d_nvec, %d, %s)" % (cb, len(nv), ",".join(map(str, nv))))
+    for order, prefix in ((10, "nlsf"), (16, "nlsf16")):
+        for cb in (0, 1):
+            L = libs["fix"]
+            off, size = L.tab["SKP_Silk_NLSF_CB%d_%d_Stage_info" % (cb, order)]
+            raw = (C.c_uint8 * size).from_address(L.bias + off)
+            nv = [int.from_bytes(bytes(raw[i * 24:i * 24 + 4]), "little") for i in range(size // 24)]
+            lines.append("SB_TAB(i32, %s_cb%d_nvec, %d, %s)" % (prefix, cb, len(nv), ",".join(map(str, nv))))
     with open(OUT, "w") as f:
         f.write("\n".join(lines) + "\n")
     print("wrote", OUT, len(lines), "lines")
