@@ -132,7 +132,37 @@ int solo_b200_bitfile_unpack(const uint8_t *in, int in_len, const uint8_t **payl
 int solo_b200_apply_loss_device(const uint8_t *d_bits_in, const int16_t *d_nbytes_in, const int32_t *d_lostflag, uint8_t *d_bits_out,
                                 int16_t *d_nbytes_out, int cap, int n, void *cuda_stream);
 
-/* Multi-GPU ingest through peer memory: after this call kernels launched on `device` may read and write buffers that live in
+/* Activity reports: the audio level and voice activity of every stream's last packet, for the RFC 6464 header extension
+   (client-to-mixer audio level), dominant-speaker detection and receive statistics.  Per stream, one byte each:
+     level : the RFC 6464 level (0-127, -dBov) of the packet's PCM row -- the encoder's input row, the decoder's output row.
+             With E = sum of x^2 over the row (int64) and n = the row length (320, 640 or 1280 samples), level = the number
+             of k in 0..126 with E < T_n[k], T_n[k] = ceil(n * 2^30 * 10^(-(k + 0.5) / 10)).  That is
+             clamp(round(10 * log10(n * 32768^2 / E)), 0, 127), 127 for digital silence, in exact integers: the tables
+             (solo_b200/csrc/sb_level_tables.inc) are generated by tools/gen_level_tables.py in exact decimal arithmetic.
+     flags : bit f (f = 0, 1) = SILK VAD flag of frame f of the packet.  Encoder: the flag coded into that frame (0 for both
+             frames of a DTX-dropped packet).  Decoder: the flag decoded from that frame, 0 when it was concealed.
+             bit 2 + f (decoder only) = frame f was concealed (lost packet, including loss before the first good frame).
+             With 20 ms packets bits 1 and 3 are 0.  RFC 6464's V bit is (flags & 3) != 0.
+   A decoder stream whose packet was rejected (ret < 0) reports level 127 and flags 0.
+     *_activity_host   : after a *_host packet wave, from the PCM that wave staged on the device; fills the host arrays
+                         level[N] and flags[N] and returns when they are filled.
+     *_activity_device : after a *_device packet wave; d_pcm = the device PCM rows passed to that wave (the encoder's input,
+                         the decoder's output).  Only enqueues one kernel on `cuda_stream` that writes d_level[N], d_flags[N].
+   The report is of the last wave: call it before the batch's next wave.  Returns -1 (solo_b200_last_error() set) for a
+   batch that has not run a wave yet, and for *_host after a *_device wave or the reverse.  The packet calls launch exactly
+   the kernels they did without these calls; each activity call adds one launch. */
+int solo_b200_enc_batch_activity_host(solo_b200_enc_batch *b, uint8_t *level, uint8_t *flags);
+int solo_b200_enc_batch_activity_device(solo_b200_enc_batch *b, const int16_t *d_pcm, uint8_t *d_level, uint8_t *d_flags,
+                                        void *cuda_stream);
+int solo_b200_dec_batch_activity_host(solo_b200_dec_batch *b, uint8_t *level, uint8_t *flags);
+int solo_b200_dec_batch_activity_device(solo_b200_dec_batch *b, const int16_t *d_pcm, uint8_t *d_level, uint8_t *d_flags,
+                                        void *cuda_stream);
+/* The same for the last packet of one AGR_Sate_*_Init handle (one byte each): 0, or -1 for a NULL or foreign handle or a
+   handle that has not coded a packet yet. */
+int solo_b200_encoder_last_activity(void *SATEEnc_State, uint8_t *level, uint8_t *flags);
+int solo_b200_decoder_last_activity(void *SATEDec_State, uint8_t *level, uint8_t *flags);
+
+/* Multi-GPU ingest through peer memory:after this call kernels launched on `device` may read and write buffers that live in
    `peer_device`'s memory (same process, or another process's allocation mapped with CUDA IPC).  The *_device entry points
    then accept such addresses for pcm / bits / nbytes / lostflag: the band-split kernel pulls its PCM rows over NVLink and
    the entropy-coding and decoder kernels push their result rows back, so a single-ingest deployment needs no separate

@@ -88,6 +88,11 @@ def lib():
         L.AGR_Sate_Decoder_Decode.restype = C.c_int32
         L.AGR_Sate_Decoder_Decode.argtypes = [vp, vp, vp, vp, vp, C.c_int32]
         L.AGR_Sate_Decoder_Uninit.argtypes = [vp]
+        for f in ("solo_b200_enc_batch_activity_host", "solo_b200_dec_batch_activity_host", "solo_b200_encoder_last_activity",
+                  "solo_b200_decoder_last_activity"):
+            getattr(L, f).argtypes = [vp, vp, vp]
+        for f in ("solo_b200_enc_batch_activity_device", "solo_b200_dec_batch_activity_device"):
+            getattr(L, f).argtypes = [vp, vp, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -110,6 +115,21 @@ def dec_state_bytes(samplerate=16000):
     if n < 0:
         raise SoloError("no decoder for sample rate %r" % (samplerate,))
     return n
+
+
+def _activity_host(fn, h, n):
+    level = np.empty(n, np.uint8)
+    flags = np.empty(n, np.uint8)
+    r = fn(h, level.ctypes.data, flags.ctypes.data)
+    if r:
+        raise SoloError("activity failed (%d): %s" % (r, _err()))
+    return level, flags
+
+
+def _activity_device(fn, h, d_pcm, d_level, d_flags, stream):
+    r = fn(h, d_pcm, d_level, d_flags, stream)
+    if r:
+        raise SoloError("activity_device failed (%d): %s" % (r, _err()))
 
 
 def profile_enable(on=True):
@@ -143,6 +163,12 @@ class SoloEncoder:
         self._nb[:] = 0
         n = lib().AGR_Sate_Encoder_Encode(self.h, pcm.ctypes.data, self._bits.ctypes.data, bufsize, self._nb.ctypes.data)
         return bytes(self._bits[:max(n, 0)]), (int(self._nb[0]), int(self._nb[1])), n
+
+    def last_activity(self):
+        """(level, flags) of the last packet: RFC 6464 level of its input and the VAD flags coded into its frames (see
+        solo_b200_encoder_last_activity in include/solo_b200.h)."""
+        level, flags = _activity_host(lib().solo_b200_encoder_last_activity, self.h, 1)
+        return int(level[0]), int(flags[0])
 
     def set_control(self, rate=None, dtx=None, loss=None):
         """Target rate (b/s), DTX on / off and expected packet loss (%) from the next packet on; None leaves a setting as
@@ -180,6 +206,12 @@ class SoloDecoder:
         self.last_nbytes = (int(nb[0]), int(nb[1]))
         self.last_nsamples = int(self._ns.value)
         return self._out[:self.samples].copy(), ret
+
+    def last_activity(self):
+        """(level, flags) of the last packet: RFC 6464 level of its output, VAD and concealment flags of its frames (see
+        solo_b200_decoder_last_activity in include/solo_b200.h)."""
+        level, flags = _activity_host(lib().solo_b200_decoder_last_activity, self.h, 1)
+        return int(level[0]), int(flags[0])
 
     def close(self):
         if getattr(self, "h", None):
@@ -236,6 +268,16 @@ class EncoderBatch:
         r = lib().solo_b200_enc_batch_encode_device(self.h, d_pcm, d_bits, cap, d_nbytes, stream)
         if r:
             raise SoloError("encode_device failed (%d): %s" % (r, _err()))
+
+    def activity(self):
+        """(level uint8 [N], flags uint8 [N]) of the last encode() wave: the RFC 6464 level of every input row and the VAD
+        flags coded into its frames (bit f = frame f; see include/solo_b200.h)."""
+        return _activity_host(lib().solo_b200_enc_batch_activity_host, self.h, self.n)
+
+    def activity_device(self, d_pcm, d_level, d_flags, stream=0):
+        """The same after an encode_device() wave: d_pcm = that wave's input rows, d_level / d_flags = device uint8 [N]
+        outputs; enqueued on `stream`."""
+        _activity_device(lib().solo_b200_enc_batch_activity_device, self.h, d_pcm, d_level, d_flags, stream)
 
     def set_control(self, rate=None, dtx=None, loss=None):
         """Per-stream target rate (b/s), DTX (0 / 1) and expected packet loss (0-100 %) from the next packet on.  Each is
@@ -329,6 +371,16 @@ class DecoderBatch:
         r = lib().solo_b200_dec_batch_decode_device(self.h, d_pcm, d_bits, cap, d_nbytes, d_flags, d_ret, stream)
         if r:
             raise SoloError("decode_device failed (%d): %s" % (r, _err()))
+
+    def activity(self):
+        """(level uint8 [N], flags uint8 [N]) of the last decode() wave: the RFC 6464 level of every output row, the VAD
+        flags decoded from its frames (bit f) and which frames were concealed (bit 2 + f); a rejected packet gives 127 / 0."""
+        return _activity_host(lib().solo_b200_dec_batch_activity_host, self.h, self.n)
+
+    def activity_device(self, d_pcm, d_level, d_flags, stream=0):
+        """The same after a decode_device() wave: d_pcm = that wave's output rows, d_level / d_flags = device uint8 [N]
+        outputs; enqueued on `stream`."""
+        _activity_device(lib().solo_b200_dec_batch_activity_device, self.h, d_pcm, d_level, d_flags, stream)
 
     def close(self):
         if getattr(self, "h", None):

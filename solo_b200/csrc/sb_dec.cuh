@@ -896,6 +896,7 @@ template <int KHZ> struct DecPacketWorkT {
     DecCtrlT<KHZ> c;
     i32 Pulses[2][FRAME];
     u8 pay[2][MAX_PAYLOAD + 8];
+    u8 act;                     // activity flags of the packet (sb_activity.cuh): bit f VAD flag, bit 2 + f concealed; in padding
     alignas(16) i16 lowout[2 * FRAME];
     i32 res_Q10[2 * FRAME];
     alignas(16) float OutHigh[2 * FRAME];
@@ -950,8 +951,11 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
         }
     }
     for (int i = 0; i < half; i++) { W->res_Q10[i] = 0; W->lowout[i] = 0; }
+    W->act = 0;
     for (int f = 0; f < nf; f++) {
         i32 ret;
+        // a lost packet's frames are concealed; a received frame reports the VAD flag it carried
+        if (lostflag == 1) W->act |= (u8)(4 << f);
         if (!st->seen_good && lostflag == 1) {
             // Loss before any frame was decoded: the reference conceals at its start-up rate of 24 kHz from an all-zero
             // state and resamples to the API rate -> silence; only these side effects survive the later switch to the core rate.
@@ -964,6 +968,7 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
             ret = dec_silk_frame(st, &W->c, rc, W->Pulses, W->pay[0], n0, W->pay[1], n1, lostflag, W->lowout + f * FRAME);
         }
         if (ret < 0) return ret;
+        if (lostflag != 1) W->act |= (u8)((st->vadFlag & 1) << f);
         for (int i = 0; i < FRAME; i++) W->res_Q10[f * FRAME + i] = st->exc_Q10[i];
     }
     if (st->moreInternalDecoderFrames) {     // the payload outlives this call

@@ -14,6 +14,8 @@
 // The two decoder kernels exist once per SILK core rate (template argument KHZ): 8 for 16 kHz streams, 16 for 32 kHz
 // streams.  A batch holds one configuration, so it picks its instantiation when it is created.
 // Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams.
+// After a wave, and only when the caller asks for it, sb_activity_kernel (warp per stream) reports every stream's audio level
+// and voice-activity / concealment flags of that wave (sb_activity.cuh).
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -25,6 +27,7 @@
 #include <vector>
 
 #include "../../include/solo_b200.h"
+#include "sb_activity.cuh"
 #include "sb_dec.cuh"
 #include "sb_enc.cuh"
 #include "sb_nsq_warp.cuh"
@@ -198,7 +201,7 @@ __global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecStateT<KHZ>* sta
 template <int KHZ>
 __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(DecStateT<KHZ>* states, const u8* __restrict__ bits, int cap,
                                                            const i16* __restrict__ nbytes, const i32* __restrict__ lostflag,
-                                                           i32* __restrict__ ret, i32* __restrict__ ret_int, DecStale* stale,
+                                                           i32* __restrict__ ret, i32* __restrict__ ret_int, u8* __restrict__ act, DecStale* stale,
                                                            i16* __restrict__ band_low, float* __restrict__ band_high, int spp, int n) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
@@ -208,6 +211,7 @@ __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(D
     i32 r = dec_packet(&states[s], &W, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
     if (ret) ret[s] = r;
     ret_int[s] = r;
+    act[s] = r < 0 ? (u8)0 : W.act;
 }
 
 // ---- synthesis filter bank + float -> int16, one warp per stream (AGR_BWE_qmf.c:86-182, AGR_BWE_decode_frame_FLP.c:222-231) ----
@@ -268,6 +272,43 @@ __global__ void __launch_bounds__(SB_SYN_WARPS * 32) sb_dec_synth_kernel(DecStat
     __syncwarp();
     st->g0_mem[2 * lane + 1] = xx1[lane];
     st->g1_mem[2 * lane + 1] = xx2[lane];
+}
+
+// ---- activity report of the last wave (sb_activity.cuh), one warp per row ----------------------------------------------
+// The row's sum of squares from 16-byte loads (2-byte loads when the caller's rows are not 16-byte aligned), reduced over
+// the warp in int64, then lane 0 looks up the level and copies the flags: the encoder's from its scratch (enc), the
+// decoder's from the bytes the decode kernel stored (dec_act).  A decoder row whose packet was rejected (dec_ret < 0)
+// reports 127 / 0 without reading its PCM row, which that packet did not write.
+#define SB_ACT_WARPS 8
+__global__ void __launch_bounds__(SB_ACT_WARPS * 32) sb_activity_kernel(const i16* __restrict__ pcm, int spp, int nf, const EncScratch* __restrict__ enc,
+                                                                         const u8* __restrict__ dec_act, const i32* __restrict__ dec_ret,
+                                                                         u8* __restrict__ level, u8* __restrict__ flags, int n) {
+    const int s = blockIdx.x * SB_ACT_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (s >= n) return;                           // whole warps
+    if (dec_ret && dec_ret[s] < 0) {
+        if (lane == 0) { level[s] = 127; flags[s] = 0; }
+        return;
+    }
+    const i16* row = pcm + (size_t)s * spp;       // rows are multiples of 16 bytes: every row is aligned as the first
+    i64 e = 0;
+    if ((((size_t)row) & 15) == 0) {
+        const int4* v = reinterpret_cast<const int4*>(row);
+        for (int i = lane; i < spp / 8; i += 32) {
+            const int4 q = v[i];
+            const int w[4] = {q.x, q.y, q.z, q.w};
+            for (int j = 0; j < 4; j++) {
+                const i32 lo = (i16)(w[j] & 0xffff), hi = w[j] >> 16;
+                e += (i64)((u32)(lo * lo) + (u32)(hi * hi));     // <= 2^31: exact in u32
+            }
+        }
+    } else {
+        for (int i = lane; i < spp; i += 32) { const i32 x = row[i]; e += x * x; }
+    }
+    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+    if (lane == 0) {
+        level[s] = (u8)rfc6464_level(e, spp);
+        flags[s] = enc ? (u8)enc_activity_flags(&enc[s], nf) : dec_act[s];
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -361,17 +402,21 @@ static void chunk_bounds(int n, int C, int c, int* lo, int* hi) {
 
 // What encoder and decoder batches share.  Batches are created value-initialised (every member zero), so the destructors
 // also clean up after a partial create.
+enum { WAVE_NONE = 0, WAVE_HOST, WAVE_DEVICE };
 struct Batch {
     int n, device;
-    int spp;                    // samples per packet and stream: 640 (40 ms) or 320 (20 ms)
+    int spp;                    // samples per packet and stream: 16 kHz 640 (40 ms) or 320 (20 ms), 32 kHz twice that
+    int nf;                     // codec frames per packet: 2 (40 ms) or 1 (20 ms)
     int hb_bytes;               // high-band bytes per packet: 4 per high-band frame
+    int wave;                   // entry point of the last packet wave of the batched API: WAVE_NONE, WAVE_HOST or WAVE_DEVICE
     int nst;                    // CUDA streams in st[]: SB_PIPE_STREAMS for a batch of the batched API, 1 for an arena segment
     cudaStream_t st[SB_PIPE_STREAMS];
     // staging for the *_host entry points and the arena
     i16* d_pcm; u8* d_bits; i16* d_nbytes; int bits_cap;
+    u8* d_act;                  // [2][n]: level | flags of the activity entry points (allocated on first use)
     ~Batch() {
         for (int i = 0; i < nst; i++) cudaStreamDestroy(st[i]);
-        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes);
+        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes); cudaFree(d_act);
     }
 };
 struct solo_b200_enc_batch : Batch {
@@ -386,10 +431,11 @@ struct solo_b200_dec_batch : Batch {
     void* d_states;             // DecStateT<khz>[n]
     DecStale* d_stale;          // payload copies that outlive a packet call (only touched after a corrupted packet, see sb_dec.cuh)
     i32* d_flags; i32* d_ret;   // staging for the *_host entry points and the arena
-    i16* d_band_low; float* d_band_high; i32* d_ret_int;   // decoder kernel -> synthesis kernel
+    i16* d_band_low; float* d_band_high; i32* d_ret_int;   // decoder kernel -> synthesis kernel (and activity kernel)
+    u8* d_act_flags;            // [n]: decoder kernel -> activity kernel, the flags of each stream's last packet
     ~solo_b200_dec_batch() {
         cudaFree(d_states); cudaFree(d_stale); cudaFree(d_flags); cudaFree(d_ret);
-        cudaFree(d_band_low); cudaFree(d_band_high); cudaFree(d_ret_int);
+        cudaFree(d_band_low); cudaFree(d_band_high); cudaFree(d_ret_int); cudaFree(d_act_flags);
     }
 };
 
@@ -424,7 +470,7 @@ static int require_gpu(int device) {
 
 // the packet layout and `nst` CUDA streams of a new batch; false when a stream cannot be created
 static bool batch_setup(Batch* b, int n, int device, int samplerate, int framesize_ms, int joint_enable, int nst) {
-    b->n = n; b->device = device; b->spp = samplerate / 1000 * framesize_ms; b->hb_bytes = hb_bytes_of(framesize_ms, joint_enable);
+    b->n = n; b->device = device; b->spp = samplerate / 1000 * framesize_ms; b->nf = framesize_ms / 20; b->hb_bytes = hb_bytes_of(framesize_ms, joint_enable);
     for (; b->nst < nst; b->nst++)
         if (cudaStreamCreateWithFlags(&b->st[b->nst], cudaStreamNonBlocking) != cudaSuccess) return false;
     return true;
@@ -491,6 +537,46 @@ template <class B> static int state_copy(B* b, int idx, void* host, int to_host,
     if (to_host) CK(cudaMemcpy(host, p, stride, cudaMemcpyDeviceToHost));
     else CK(cudaMemcpy(p, host, stride, cudaMemcpyHostToDevice));
     return 0;
+}
+
+// ---- activity reports of the last packet wave (sb_activity.cuh) -------------------------------------------------------
+// the activity kernel over streams [lo, lo + n) on st: `pcm` is the wave's PCM matrix (row 0 = stream 0); the encoder's
+// flags come from its scratch, the decoder's from the bytes and return codes its decode kernel left
+static int activity_launch(const solo_b200_enc_batch* b, int lo, int n, const i16* pcm, u8* level, u8* flags, cudaStream_t st) {
+    sb_activity_kernel<<<(n + SB_ACT_WARPS - 1) / SB_ACT_WARPS, SB_ACT_WARPS * 32, 0, st>>>(pcm + (size_t)lo * b->spp, b->spp, b->nf, b->d_scratch + lo,
+                                                                                         nullptr, nullptr, level, flags, n);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+static int activity_launch(const solo_b200_dec_batch* b, int lo, int n, const i16* pcm, u8* level, u8* flags, cudaStream_t st) {
+    sb_activity_kernel<<<(n + SB_ACT_WARPS - 1) / SB_ACT_WARPS, SB_ACT_WARPS * 32, 0, st>>>(pcm + (size_t)lo * b->spp, b->spp, b->nf, nullptr,
+                                                                                         b->d_act_flags + lo, b->d_ret_int + lo, level, flags, n);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+// the report of streams [lo, lo + n) from the staged PCM rows into host arrays of n entries, on the batch's first CUDA
+// stream; returns when the arrays are filled
+template <class B> static int activity_host(B* b, int lo, int n, u8* level, u8* flags) {
+    cudaStream_t st = b->st[0];
+    if (!b->d_act) CK(cudaMalloc(&b->d_act, 2 * (size_t)b->n));
+    u8* dl = b->d_act + lo;
+    u8* df = b->d_act + b->n + lo;
+    if (int e = activity_launch(b, lo, n, b->d_pcm, dl, df, st)) return e;
+    CK(cudaMemcpyAsync(level, dl, (size_t)n, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(flags, df, (size_t)n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+}
+// the activity entry point of kind `want` (WAVE_HOST / WAVE_DEVICE) reports on a last wave of the same kind only: the
+// other kind's PCM rows are not where it looks
+static int activity_wave_check(const Batch* b, int want) {
+    if (b->wave == want) return 0;
+    snprintf(g_err, sizeof g_err, "%s", b->wave == WAVE_NONE ? "activity: the batch has not run a packet wave yet"
+                                        : want == WAVE_HOST ? "activity_host: the last packet wave was a *_device call"
+                                                            : "activity_device: the last packet wave was a *_host call");
+    return -1;
 }
 
 extern "C" {
@@ -586,6 +672,7 @@ static int enc_launch(solo_b200_enc_batch* b, int lo, int n, const i16* d_pcm, u
 int solo_b200_enc_batch_encode_device(solo_b200_enc_batch* b, const int16_t* d_pcm, uint8_t* d_bits, int cap, int16_t* d_nbytes, void* cuda_stream) {
     if (!b || !d_pcm || !d_bits || !d_nbytes || cap < 16) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
     CK(cudaSetDevice(b->device));
+    b->wave = WAVE_DEVICE;
     return enc_launch(b, 0, b->n, d_pcm, d_bits, cap, d_nbytes, (cudaStream_t)cuda_stream);
 }
 
@@ -594,6 +681,7 @@ int solo_b200_enc_batch_encode_host(solo_b200_enc_batch* b, const int16_t* pcm, 
     CK(cudaSetDevice(b->device));
     int r = staging(b, cap);
     if (r) return r;
+    b->wave = WAVE_HOST;
     return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {   // per chunk: H2D, encoder kernels, D2H
         const size_t m = (size_t)(hi - lo);
         CK(cudaMemcpyAsync(b->d_pcm + (size_t)lo * b->spp, pcm + (size_t)lo * b->spp, sizeof(i16) * b->spp * m, cudaMemcpyHostToDevice, st));
@@ -683,7 +771,8 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
         cudaMalloc(&b->d_stale, sizeof(DecStale) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_band_low, sizeof(i16) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_band_high, sizeof(float) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
-        cudaMalloc(&b->d_ret_int, sizeof(i32) * (size_t)n_streams) != cudaSuccess) {
+        cudaMalloc(&b->d_ret_int, sizeof(i32) * (size_t)n_streams) != cudaSuccess ||
+        cudaMalloc(&b->d_act_flags, (size_t)n_streams) != cudaSuccess) {
         fail("dec_batch_create", cudaGetLastError());
         return batch_destroy(b);
     }
@@ -707,7 +796,7 @@ static void dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const
     DecStateT<KHZ>* states = (DecStateT<KHZ>*)b->d_states + lo;
     const size_t half = (size_t)(b->spp / 2);
     sb_decode_kernel<KHZ><<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(states, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, d_lostflag + lo,
-                                                                       d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_stale + lo,
+                                                                       d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_act_flags + lo, b->d_stale + lo,
                                                                        b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half, b->spp, n);
     sb_dec_synth_kernel<KHZ><<<(n + SB_SYN_WARPS - 1) / SB_SYN_WARPS, SB_SYN_WARPS * 32, 0, st>>>(states, b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half,
                                                                                                b->d_ret_int + lo, d_pcm + (size_t)lo * b->spp, b->spp, n);
@@ -729,6 +818,7 @@ int solo_b200_dec_batch_decode_device(solo_b200_dec_batch* b, int16_t* d_pcm, co
                                       const int32_t* d_lostflag, int32_t* d_ret, void* cuda_stream) {
     if (!b || !d_pcm || !d_bits || !d_nbytes || !d_lostflag || cap < 16) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
     CK(cudaSetDevice(b->device));
+    b->wave = WAVE_DEVICE;
     return dec_launch(b, 0, b->n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, (cudaStream_t)cuda_stream);
 }
 
@@ -738,6 +828,7 @@ int solo_b200_dec_batch_decode_host(solo_b200_dec_batch* b, int16_t* pcm, const 
     CK(cudaSetDevice(b->device));
     int r = dec_staging(b, cap);
     if (r) return r;
+    b->wave = WAVE_HOST;
     return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {   // per chunk: H2D, decoder kernels, D2H
         const size_t m = (size_t)(hi - lo);
         CK(cudaMemcpyAsync(b->d_bits + (size_t)lo * cap, bits + (size_t)lo * cap, (size_t)cap * m, cudaMemcpyHostToDevice, st));
@@ -761,6 +852,31 @@ int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch* b, int idx, void
 }
 int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch* b, int idx, const void* blob, int blob_bytes) {
     return state_copy(b, idx, (void*)blob, 0, blob_bytes < 0 ? 0 : blob_bytes);
+}
+
+int solo_b200_enc_batch_activity_host(solo_b200_enc_batch* b, uint8_t* level, uint8_t* flags) {
+    if (!b || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_HOST)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_host(b, 0, b->n, level, flags);
+}
+int solo_b200_enc_batch_activity_device(solo_b200_enc_batch* b, const int16_t* d_pcm, uint8_t* d_level, uint8_t* d_flags, void* cuda_stream) {
+    if (!b || !d_pcm || !d_level || !d_flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_DEVICE)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_launch(b, 0, b->n, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
+}
+int solo_b200_dec_batch_activity_host(solo_b200_dec_batch* b, uint8_t* level, uint8_t* flags) {
+    if (!b || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_HOST)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_host(b, 0, b->n, level, flags);
+}
+int solo_b200_dec_batch_activity_device(solo_b200_dec_batch* b, const int16_t* d_pcm, uint8_t* d_level, uint8_t* d_flags, void* cuda_stream) {
+    if (!b || !d_pcm || !d_level || !d_flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_DEVICE)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_launch(b, 0, b->n, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
 }
 
 // ---- packet framing (host, no GPU involved): enc_main.c:212-234 / dec_main.c:196-307 / README "Bitstream sending" --------
@@ -853,7 +969,7 @@ template <class B> struct ArenaSeg {
     int n_used;
     std::mutex mu;
 };
-template <class B> struct Handle { unsigned magic; ArenaSeg<B>* seg; int slot; };
+template <class B> struct Handle { unsigned magic; ArenaSeg<B>* seg; int slot; int coded; };   // coded: a packet went through
 typedef Handle<solo_b200_enc_batch> EncHandle;
 typedef Handle<solo_b200_dec_batch> DecHandle;
 static const unsigned ENC_MAGIC = 0x53424531u, DEC_MAGIC = 0x53424431u;   // "SBE1", "SBD1"
@@ -911,6 +1027,16 @@ template <class B> static int arena_close(void* handle, unsigned magic) {
     delete h;
     return 0;
 }
+// the activity report of a handle's last packet, from its slot of the segment
+template <class B> static int handle_activity(void* handle, unsigned magic, u8* level, u8* flags) {
+    Handle<B>* h = (Handle<B>*)handle;
+    if (!h || h->magic != magic || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument (NULL or foreign handle)"); return -1; }
+    if (!h->coded) { snprintf(g_err, sizeof g_err, "activity: the handle has not coded a packet yet"); return -1; }
+    B* b = h->seg->b;
+    std::lock_guard<std::mutex> lk(h->seg->mu);
+    CK(cudaSetDevice(b->device));
+    return activity_host(b, h->slot, 1, level, flags);
+}
 }  // extern "C++"
 
 void* AGR_Sate_Encoder_Init(USER_Ctrl_enc* enc_Ctrl) {
@@ -948,6 +1074,7 @@ SKP_int32 AGR_Sate_Encoder_Encode(void* SATEEnc_State, const SKP_int16* AGR_Sate
         ok = ok && cudaMemcpyAsync(nb, b->d_nbytes + 2 * s, sizeof nb, cudaMemcpyDeviceToHost, st) == cudaSuccess;
         ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
         if (!ok) { fprintf(stderr, "solo_b200: encode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError())); return -1; }
+        h->coded = 1;
     }
     // DTX packets return the high-band bytes (4 per 20 ms frame) with nBytesOut[0] == 0 (App. A Q16)
     int total = nb[0] ? nb[0] : b->hb_bytes;
@@ -1023,6 +1150,7 @@ SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, 
         ok = ok && cudaMemcpyAsync(&ret, b->d_ret + s, sizeof ret, cudaMemcpyDeviceToHost, st) == cudaSuccess;
         ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
         if (!ok) { fprintf(stderr, "solo_b200: decode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError())); return -1; }
+        h->coded = 1;
     }
     // the reference rewrites the caller's nBytes[] while splitting the payload (AGR_BWE_decode_frame_FLP.c:171-190)
     dec_split_lengths(nb, lostflag, b->hb_bytes);
@@ -1032,6 +1160,12 @@ SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, 
     return ret;
 }
 SKP_int32 AGR_Sate_Decoder_Uninit(void* SATEDec_State) { return arena_close<solo_b200_dec_batch>(SATEDec_State, DEC_MAGIC); }
+int solo_b200_encoder_last_activity(void* SATEEnc_State, uint8_t* level, uint8_t* flags) {
+    return handle_activity<solo_b200_enc_batch>(SATEEnc_State, ENC_MAGIC, level, flags);
+}
+int solo_b200_decoder_last_activity(void* SATEDec_State, uint8_t* level, uint8_t* flags) {
+    return handle_activity<solo_b200_dec_batch>(SATEDec_State, DEC_MAGIC, level, flags);
+}
 /* arena bookkeeping for tests: segments and slots in use (encoder, decoder) */
 int solo_b200_arena_stats(int out[4]) {
     std::lock_guard<std::mutex> lk(g_arena_mu);
