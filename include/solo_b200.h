@@ -162,6 +162,44 @@ int solo_b200_dec_batch_activity_device(solo_b200_dec_batch *b, const int16_t *d
 int solo_b200_encoder_last_activity(void *SATEEnc_State, uint8_t *level, uint8_t *flags);
 int solo_b200_decoder_last_activity(void *SATEDec_State, uint8_t *level, uint8_t *flags);
 
+/* Conference mixer (MCU): per room, the mix-minus of its loudest talkers, from the decoder's PCM rows to the downlink
+   encoder's input rows, for top-N mixing with an RFC 6465 (mixer-to-client audio level) header.
+   Inputs:
+     in          : int16 [n][spp], the decoder's output rows, spp = 320, 640 or 1280.
+     level, flags: uint8 [n] each, in the activity report's format: exactly what solo_b200_dec_batch_activity_{host,device}
+                   writes.
+     rooms, CSR  : room_start int32 [R+1] with room_start[0] = 0, non-decreasing, room_start[R] = M; members int32 [M],
+                   stream indices in any order.  Room r is members[room_start[r] .. room_start[r+1]).
+     k           : 1 to 8.
+   Selection:
+     A member j of a room is eligible when (flags[j] & 3) != 0, i.e. RFC 6464's V bit; concealed and rejected packets
+     report flags 0, so they are never mixed.  The room's talkers are its up-to-k eligible members with the smallest
+     (level[j], j): lower level is louder, ties go to the lower index.  They are written to talkers int32 [R][k] in that
+     order, padded with -1: the CSRC list (and, with level[], the levels) of an RFC 6465 header.
+   Mixing:
+     For every member i of room r and every sample t:
+       out[i][t] = clamp(sum over talkers j of r with j != i of in[j][t], -32768, 32767).
+     A listener hears all the talkers, a talker hears the others, a room without talkers gives zeros.  The sum is in int32;
+     with k <= 8 it cannot overflow, so the result does not depend on the order of summation.  No floating point is used.
+     Rows of streams that are in no room are not written.
+   Policy stays with the caller, in the two byte arrays: mute a participant with flags 0, pin a moderator with level 0,
+   apply hysteresis by rewriting the bytes before the call.
+     mix_host   : host arrays.  Checks everything first and returns -1, writing nothing (solo_b200_last_error() set), for a
+                  bad spp, n or k, offsets that do not start at 0 or decrease, a member outside [0, n), or a stream listed
+                  twice (in one room or in two).  Runs on the calling thread's current CUDA device and returns when out[]
+                  and talkers[] are filled.
+     mix_device : device arrays; only enqueues work on `cuda_stream` (at most two kernel launches).  It checks the scalars
+                  (-1 for a bad spp, n or k, for d_in / d_out not 16-byte aligned, and for d_in and d_out overlapping:
+                  they must not), not the arrays' contents, and never reads or writes out of bounds whatever they hold:
+                  room bounds are clamped to [0, room_start[R]], a member outside [0, n) is skipped (neither a talker nor
+                  written), and a stream listed twice gives unspecified rows but no fault.
+   n_rooms = 0 is a call that does nothing. */
+int solo_b200_mix_host(const int16_t *in, int16_t *out, int spp, int n, const uint8_t *level, const uint8_t *flags,
+                       const int32_t *room_start, const int32_t *members, int n_rooms, int k, int32_t *talkers);
+int solo_b200_mix_device(const int16_t *d_in, int16_t *d_out, int spp, int n, const uint8_t *d_level,
+                         const uint8_t *d_flags, const int32_t *d_room_start, const int32_t *d_members, int n_rooms,
+                         int k, int32_t *d_talkers, void *cuda_stream);
+
 /* Multi-GPU ingest through peer memory:after this call kernels launched on `device` may read and write buffers that live in
    `peer_device`'s memory (same process, or another process's allocation mapped with CUDA IPC).  The *_device entry points
    then accept such addresses for pcm / bits / nbytes / lostflag: the band-split kernel pulls its PCM rows over NVLink and

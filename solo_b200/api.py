@@ -93,6 +93,8 @@ def lib():
             getattr(L, f).argtypes = [vp, vp, vp]
         for f in ("solo_b200_enc_batch_activity_device", "solo_b200_dec_batch_activity_device"):
             getattr(L, f).argtypes = [vp, vp, vp, vp, vp]
+        L.solo_b200_mix_host.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp]
+        L.solo_b200_mix_device.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]
         _lib = L
     return _lib
 
@@ -454,3 +456,45 @@ def enable_peer_access(device, peer_device):
 def apply_loss_device(d_bits_in, d_nbytes_in, d_lostflag, d_bits_out, d_nbytes_out, cap, n, stream=0):
     if lib().solo_b200_apply_loss_device(d_bits_in, d_nbytes_in, d_lostflag, d_bits_out, d_nbytes_out, cap, n, stream):
         raise SoloError(_err())
+
+
+# ---- conference mixer (include/solo_b200.h, solo_b200_mix_*) ----------------------------------------------------------
+def rooms_csr(rooms):
+    """(room_start int32 [R+1], members int32 [M]) of a list of index arrays, one per room."""
+    sizes = [len(r) for r in rooms]
+    room_start = np.zeros(len(rooms) + 1, np.int32)
+    room_start[1:] = np.cumsum(sizes, dtype=np.int64)
+    members = np.concatenate([np.asarray(r, np.int32).ravel() for r in rooms]) if rooms else np.zeros(0, np.int32)
+    return room_start, np.ascontiguousarray(members, np.int32)
+
+
+def mix(pcm, level, flags, rooms, k, out=None):
+    """Mix-minus of each room's up-to-k loudest talkers: pcm int16 [n, spp] (the decoder's rows), level / flags uint8 [n]
+    (DecoderBatch.activity()), rooms = a list of index arrays -> (out int16 [n, spp], talkers int32 [R, k]).  Rows of streams
+    in no room keep what `out` held (zeros when it is None).  Raises SoloError, with `out` untouched, for a bad argument,
+    a member outside [0, n) or a stream listed twice."""
+    pcm = np.ascontiguousarray(pcm, np.int16)
+    n, spp = pcm.shape
+    level = np.ascontiguousarray(level, np.uint8)
+    flags = np.ascontiguousarray(flags, np.uint8)
+    if level.shape != (n,) or flags.shape != (n,):
+        raise SoloError("mix: level and flags must be uint8 [%d]" % n)
+    if out is None:
+        out = np.zeros((n, spp), np.int16)
+    if out.shape != (n, spp) or out.dtype != np.int16 or not out.flags.c_contiguous:
+        raise SoloError("mix: out must be a C-contiguous int16 [%d, %d] array" % (n, spp))
+    room_start, members = rooms_csr(rooms)
+    talkers = np.empty((len(rooms), max(int(k), 0)), np.int32)
+    r = lib().solo_b200_mix_host(pcm.ctypes.data, out.ctypes.data, spp, n, level.ctypes.data, flags.ctypes.data,
+                                 room_start.ctypes.data, members.ctypes.data, len(rooms), int(k), talkers.ctypes.data)
+    if r:
+        raise SoloError("mix failed (%d): %s" % (r, _err()))
+    return out, talkers
+
+
+def mix_device(d_in, d_out, spp, n, d_level, d_flags, d_room_start, d_members, n_rooms, k, d_talkers, stream=0):
+    """The same on device arrays (addresses): enqueued on `stream`; contents are not checked (see solo_b200_mix_device)."""
+    r = lib().solo_b200_mix_device(d_in, d_out, int(spp), int(n), d_level, d_flags, d_room_start, d_members, int(n_rooms),
+                                   int(k), d_talkers, stream)
+    if r:
+        raise SoloError("mix_device failed (%d): %s" % (r, _err()))

@@ -16,6 +16,8 @@
 // Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams.
 // After a wave, and only when the caller asks for it, sb_activity_kernel (warp per stream) reports every stream's audio level
 // and voice-activity / concealment flags of that wave (sb_activity.cuh).
+// The conference mixer (solo_b200_mix_*, sb_mix.cuh) is two launches of its own: sb_mix_select_kernel (warp per room) picks
+// each room's loudest talkers, sb_mix_kernel (warp per member) writes each member's mix-minus row.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -30,6 +32,7 @@
 #include "sb_activity.cuh"
 #include "sb_dec.cuh"
 #include "sb_enc.cuh"
+#include "sb_mix.cuh"
 #include "sb_nsq_warp.cuh"
 
 using namespace sb;
@@ -308,6 +311,109 @@ __global__ void __launch_bounds__(SB_ACT_WARPS * 32) sb_activity_kernel(const i1
     if (lane == 0) {
         level[s] = (u8)rfc6464_level(e, spp);
         flags[s] = enc ? (u8)enc_activity_flags(&enc[s], nf) : dec_act[s];
+    }
+}
+
+// ---- conference mixer (sb_mix.cuh): talker selection, one warp per room -------------------------------------------------
+// Lane l keeps the top 8 keys of members lo + l, lo + l + 32, ...; then k rounds each take the smallest head of the 32 lists
+// (a shuffle reduction) and the lane that held it drops it.  Members are fetched SB_MIX_UNROLL per lane at a time so that the
+// gathers of flags / level of a large room overlap.  Room bounds are clamped to [0, M] (M = room_start[R]) and members outside
+// [0, n) are skipped, so no contents of the arrays lead to an access out of bounds.
+#define SB_MIX_WARPS 8
+#define SB_MIX_UNROLL 16
+__global__ void __launch_bounds__(SB_MIX_WARPS * 32) sb_mix_select_kernel(const u8* __restrict__ level, const u8* __restrict__ flags,
+                                                                           const i32* __restrict__ room_start, const i32* __restrict__ members,
+                                                                           int n, int R, int k, i32* __restrict__ talkers) {
+    const int r = blockIdx.x * SB_MIX_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= R) return;                           // whole warps
+    const i32 M = imax(room_start[R], 0);
+    const i32 lo = imin(imax(room_start[r], 0), M), hi = imin(imax(room_start[r + 1], lo), M);
+    u64 L[SB_MIX_KMAX];
+#pragma unroll
+    for (int i = 0; i < SB_MIX_KMAX; i++) L[i] = SB_MIX_NONE;
+    for (i32 base = lo; base < hi; base += 32 * SB_MIX_UNROLL) {
+        i32 j[SB_MIX_UNROLL];
+        u8 f[SB_MIX_UNROLL], lv[SB_MIX_UNROLL];
+#pragma unroll
+        for (int u = 0; u < SB_MIX_UNROLL; u++) {
+            const i32 m = base + u * 32 + lane;
+            j[u] = m < hi ? members[m] : -1;
+        }
+#pragma unroll
+        for (int u = 0; u < SB_MIX_UNROLL; u++) {
+            const bool ok = (u32)j[u] < (u32)n;
+            f[u] = ok ? flags[j[u]] : (u8)0;
+            lv[u] = ok ? level[j[u]] : (u8)0;
+        }
+#pragma unroll
+        for (int u = 0; u < SB_MIX_UNROLL; u++) {
+            const u64 key = mix_key(lv[u], j[u]);
+            if (mix_eligible(f[u]) && key < L[SB_MIX_KMAX - 1]) mix_topk_insert(L, key);
+        }
+    }
+    for (int t = 0; t < k; t++) {
+        u64 best = L[0];
+        for (int o = 16; o > 0; o >>= 1) {
+            const u64 v = __shfl_xor_sync(0xffffffffu, best, o);
+            best = v < best ? v : best;
+        }
+        mix_topk_pop(L, best);
+        if (lane == 0) talkers[(size_t)r * k + t] = mix_key_stream(best);
+    }
+}
+
+// ---- conference mixer: one warp per member row ---------------------------------------------------------------------------
+// Member position m (grid-stride over M = room_start[R], which the host cannot read without a synchronise) finds its room by
+// the warp's 33-ary search (one probe per lane and round), lanes 0..k-1 read the room's talkers and the warp keeps those the
+// listener hears.  Then each lane sums 16-byte chunks c = lane, lane + 32, ... of those rows in int32 and stores the
+// saturated chunk with one 16-byte store.  The talker rows are read by every member of the room: after the first they come
+// from L2 (or L1, for members in one block).  The kernel is a chain of dependent loads per member (bounds, member, search,
+// talkers, rows), so it is sized for 6 resident blocks per SM (40 registers, 36 bytes of spill stores): the more members in flight, the more
+// of the chain overlaps.
+__global__ void __launch_bounds__(SB_MIX_WARPS * 32, 6) sb_mix_kernel(const i16* __restrict__ in, i16* __restrict__ out, int spp, int n,
+                                                                       const i32* __restrict__ room_start, const i32* __restrict__ members,
+                                                                       int R, int k, const i32* __restrict__ talkers) {
+    const int lane = threadIdx.x & 31, nv = spp / 8;
+    const i32 M = room_start[R];
+    for (i32 m = blockIdx.x * SB_MIX_WARPS + (threadIdx.x >> 5); m < M; m += gridDim.x * SB_MIX_WARPS) {
+        const i32 i = members[m];
+        if ((u32)i >= (u32)n) continue;           // whole warps
+        int r = 0, span = R;
+        while (span > 1) {
+            const int step = mix_search_step(span), p = r + lane * step;
+            mix_search_narrow(&r, &span, step, __ballot_sync(0xffffffffu, p < r + span && room_start[p] <= m));
+        }
+        const i32 tj = lane < k ? talkers[(size_t)r * k + lane] : -1;
+        unsigned hear = __ballot_sync(0xffffffffu, (u32)tj < (u32)n && mix_hears(i, tj));
+        const int nt = __popc(hear);
+        i32 src[SB_MIX_KMAX];                     // the talker rows heard, as stream indices
+#pragma unroll
+        for (int t = 0; t < SB_MIX_KMAX; t++) {
+            src[t] = 0;
+            if (t < nt) {
+                const int l = __ffs(hear) - 1;
+                hear &= hear - 1;
+                src[t] = __shfl_sync(0xffffffffu, tj, l);
+            }
+        }
+        const int4* rows = reinterpret_cast<const int4*>(in);
+        int4* dst = reinterpret_cast<int4*>(out + (size_t)i * spp);
+        for (int c = lane; c < nv; c += 32) {
+            i32 acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+            for (int t = 0; t < SB_MIX_KMAX; t++) {
+                if (t < nt) {
+                    const int4 q = __ldg(rows + (size_t)src[t] * nv + c);
+                    const int w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+                    for (int h = 0; h < 4; h++) { acc[2 * h] += (i16)(w[h] & 0xffff); acc[2 * h + 1] += w[h] >> 16; }
+                }
+            }
+            int w[4];
+#pragma unroll
+            for (int h = 0; h < 4; h++) w[h] = (i32)((u32)(u16)mix_out(acc[2 * h]) | ((u32)(u16)mix_out(acc[2 * h + 1]) << 16));
+            dst[c] = make_int4(w[0], w[1], w[2], w[3]);
+        }
     }
 }
 
@@ -933,6 +1039,87 @@ int solo_b200_apply_loss_device(const uint8_t* d_bits_in, const int16_t* d_nbyte
     count_launch();
     CK(cudaGetLastError());
     return 0;
+}
+
+// ---- conference mixer (sb_mix.cuh) ---------------------------------------------------------------------------------------
+static int mix_scalars_ok(int spp, int n, int n_rooms, int k) {
+    if ((spp == 320 || spp == 640 || spp == 1280) && n > 0 && n_rooms >= 0 && k >= 1 && k <= SB_MIX_KMAX) return 1;
+    snprintf(g_err, sizeof g_err, "mix: bad argument (spp %d, n %d, n_rooms %d, k %d)", spp, n, n_rooms, k);
+    return 0;
+}
+// the two kernels of one mix call on st; nothing when there are no rooms
+static int mix_launch(const i16* in, i16* out, int spp, int n, const u8* level, const u8* flags, const i32* room_start,
+                      const i32* members, int R, int k, i32* talkers, cudaStream_t st) {
+    if (R == 0) return 0;
+    sb_mix_select_kernel<<<(R + SB_MIX_WARPS - 1) / SB_MIX_WARPS, SB_MIX_WARPS * 32, 0, st>>>(level, flags, room_start, members, n, R, k, talkers);
+    count_launch();
+    CK(cudaGetLastError());
+    sb_mix_kernel<<<(n + SB_MIX_WARPS - 1) / SB_MIX_WARPS, SB_MIX_WARPS * 32, 0, st>>>(in, out, spp, n, room_start, members, R, k, talkers);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int solo_b200_mix_device(const int16_t* d_in, int16_t* d_out, int spp, int n, const uint8_t* d_level, const uint8_t* d_flags,
+                         const int32_t* d_room_start, const int32_t* d_members, int n_rooms, int k, int32_t* d_talkers, void* cuda_stream) {
+    if (!d_in || !d_out || !d_level || !d_flags || !d_room_start || !d_members || !d_talkers) { snprintf(g_err, sizeof g_err, "mix: bad argument"); return -1; }
+    if (!mix_scalars_ok(spp, n, n_rooms, k)) return -1;
+    const size_t bytes = sizeof(i16) * (size_t)spp * (size_t)n;
+    const uintptr_t a = (uintptr_t)d_in, b = (uintptr_t)d_out;
+    if (((a | b) & 15) != 0) { snprintf(g_err, sizeof g_err, "mix_device: d_in and d_out must be 16-byte aligned"); return -1; }
+    if (a < b + bytes && b < a + bytes) { snprintf(g_err, sizeof g_err, "mix_device: d_in and d_out overlap"); return -1; }
+    return mix_launch(d_in, d_out, spp, n, d_level, d_flags, d_room_start, d_members, n_rooms, k, d_talkers, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_mix_host(const int16_t* in, int16_t* out, int spp, int n, const uint8_t* level, const uint8_t* flags,
+                       const int32_t* room_start, const int32_t* members, int n_rooms, int k, int32_t* talkers) {
+    if (!in || !out || !level || !flags || !room_start || !talkers) { snprintf(g_err, sizeof g_err, "mix: bad argument"); return -1; }
+    if (!mix_scalars_ok(spp, n, n_rooms, k)) return -1;
+    if (room_start[0] != 0) { snprintf(g_err, sizeof g_err, "mix: room_start[0] is %d, not 0", room_start[0]); return -1; }
+    for (int r = 0; r < n_rooms; r++)
+        if (room_start[r + 1] < room_start[r]) { snprintf(g_err, sizeof g_err, "mix: room_start decreases at room %d", r); return -1; }
+    const i32 M = room_start[n_rooms];
+    if (M > 0 && !members) { snprintf(g_err, sizeof g_err, "mix: bad argument (members NULL)"); return -1; }
+    {
+        std::vector<u8> seen((size_t)n, 0);
+        for (i32 m = 0; m < M; m++) {
+            const i32 j = members[m];
+            if (j < 0 || j >= n) { snprintf(g_err, sizeof g_err, "mix: member %d is stream %d, outside [0, %d)", m, j, n); return -1; }
+            if (seen[j]++) { snprintf(g_err, sizeof g_err, "mix: stream %d is listed twice", j); return -1; }
+        }
+    }
+    if (n_rooms == 0) return 0;
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    if (int e = require_gpu(dev)) return e;
+    // `out` goes to the device too: rows of streams in no room come back as they were
+    const size_t bytes = sizeof(i16) * (size_t)spp * (size_t)n, tk = sizeof(i32) * (size_t)n_rooms * (size_t)k;
+    cudaStream_t st;
+    CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    i16 *d_in = nullptr, *d_out = nullptr;
+    u8* d_lf = nullptr;
+    i32 *d_rs = nullptr, *d_tk = nullptr;
+    int r = 0;
+    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
+    ok(cudaMallocAsync(&d_in, bytes, st), "cudaMallocAsync") && ok(cudaMallocAsync(&d_out, bytes, st), "cudaMallocAsync") &&
+        ok(cudaMallocAsync(&d_lf, 2 * (size_t)n, st), "cudaMallocAsync") &&
+        ok(cudaMallocAsync(&d_rs, sizeof(i32) * ((size_t)n_rooms + 1 + (size_t)M), st), "cudaMallocAsync") &&
+        ok(cudaMallocAsync(&d_tk, tk, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, st), "copy in") &&
+        ok(cudaMemcpyAsync(d_out, out, bytes, cudaMemcpyHostToDevice, st), "copy out") &&
+        ok(cudaMemcpyAsync(d_lf, level, (size_t)n, cudaMemcpyHostToDevice, st), "copy level") &&
+        ok(cudaMemcpyAsync(d_lf + n, flags, (size_t)n, cudaMemcpyHostToDevice, st), "copy flags") &&
+        ok(cudaMemcpyAsync(d_rs, room_start, sizeof(i32) * ((size_t)n_rooms + 1), cudaMemcpyHostToDevice, st), "copy room_start") &&
+        (M == 0 || ok(cudaMemcpyAsync(d_rs + n_rooms + 1, members, sizeof(i32) * (size_t)M, cudaMemcpyHostToDevice, st), "copy members"));
+    if (!r) r = mix_launch(d_in, d_out, spp, n, d_lf, d_lf + n, d_rs, d_rs + n_rooms + 1, n_rooms, k, d_tk, st);
+    // the results go to the caller's arrays only when every step succeeded
+    ok(cudaStreamSynchronize(st), "mix") && ok(cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, st), "copy out") &&
+        ok(cudaMemcpyAsync(talkers, d_tk, tk, cudaMemcpyDeviceToHost, st), "copy talkers");
+    for (void* p : {(void*)d_in, (void*)d_out, (void*)d_lf, (void*)d_rs, (void*)d_tk})
+        if (p) cudaFreeAsync(p, st);
+    ok(cudaStreamSynchronize(st), "mix");
+    cudaStreamDestroy(st);
+    return r;
 }
 
 // ---- multi-GPU ingest through peer memory --------------------------------------------------------------------------------
