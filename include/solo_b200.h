@@ -200,6 +200,62 @@ int solo_b200_mix_device(const int16_t *d_in, int16_t *d_out, int spp, int n, co
                          const uint8_t *d_flags, const int32_t *d_room_start, const int32_t *d_members, int n_rooms,
                          int k, int32_t *d_talkers, void *cuda_stream);
 
+/* Receive queue: per stream, holds the two descriptions of each packet (solo_b200_split_packet) as they arrive early, out
+   of order or twice, pairs them and hands the decoder one row per tick, for N streams on the device.  It is independent
+   of the codec batches: a pull writes rows for any decoder batch with the same N and cap.
+   Created with depth D (a power of two, 2 to 32) and desc_cap (the largest description in bytes, 16 to 1024, a multiple
+   of 16).  Per stream it keeps:
+     last     : the last played packet index (uint32), 0xFFFFFFFF at create, so packet 0 plays first;
+     D slots  : slot j holds at most one packet index t with t = j (mod D), and for it description 1 and / or 2;
+     counters : 8 uint32, in this order: stored, duplicate, late, dropped, malformed, played_both, played_one,
+                played_none.
+   Packet index: the caller derives it from the RTP timestamp (timestamp / samples per packet); it wraps at 2^32.  Index p
+   is CURRENT for a stream when (p - last) mod 2^32 lies in [1, 2^31), otherwise LATE; among current indices the newer one
+   has the larger distance (p - last) mod 2^32.
+   insert: arrival a is (stream[a], index[a], desc[a], len[a] bytes at payload + off[a]).
+     - An arrival whose stream is outside [0, N) only counts in the queue-wide bad_stream counter.
+     - It is malformed when desc is not 1 or 2, len is outside [1, desc_cap], or its bytes are not inside
+       payload[0, payload_bytes).
+     - Per slot, from its held packet and the call's valid, current arrivals for it: the slot keeps the NEWEST of those
+       indices (a held index that is no longer current does not compete).  If that is not the held index, the held
+       descriptions are discarded.  For each description of the kept index a held one stays, otherwise the FIRST arrival
+       in array order is stored.
+     - Every arrival counts exactly once, as stored; duplicate (its (index, desc) was already held or stored); late;
+       dropped (its slot keeps a newer index); or malformed.  Held descriptions that are discarded count as dropped too.
+     The result does not depend on thread scheduling: the same calls give the same state and counters.
+   pull: for each stream s, with t = play[s] (play = NULL: last + 1), writes row s of bits [N][cap], nbytes[s][2] and
+     lostflag[s] exactly as solo_b200_merge_packets does for the descriptions of t its slot holds (4 both, 2 only
+     description 1, 3 only description 2, 1 neither: 16 zero bytes and {16, 8}).  Row bytes after nbytes[0] are not
+     written.  cap must be at least 2 * desc_cap (else -1), so a merge always fits.  Then last = t, and the slot is
+     emptied when it held t or an index that is no longer current (counted as dropped); one of played_both, played_one
+     or played_none is incremented.
+   reset: for a participant joining or rejoining a stream: empties the listed streams' slots, zeroes their counters and
+     sets last = start - 1.  Host arrays; -1 (nothing done) for a stream outside [0, N) or listed twice.
+   stats: counters uint32 [N][8] and the bad_stream count (either may be NULL).
+   Entry points:
+     *_host   : host arrays; run on the queue's own CUDA stream and return when done.
+     *_device : device arrays; only enqueue work on `cuda_stream`.  They check the scalars (-1 for n_arrivals < 0,
+                payload_bytes < 0, a cap below 2 * desc_cap, d_bits not 16-byte aligned), not the arrays' contents, and
+                never read or write out of bounds whatever those hold: bad entries are classified and counted as above.
+     reset, stats : host arrays, ordered on `cuda_stream`; return after synchronising it.
+   Launches: an insert of n_arrivals = 0 launches nothing, any other insert three kernels; a pull one kernel. */
+typedef struct solo_b200_rx solo_b200_rx;
+/* NULL (solo_b200_last_error() set) for a bad n_streams, depth, desc_cap or device. */
+solo_b200_rx *solo_b200_rx_create(int n_streams, int depth, int desc_cap, int device);
+void solo_b200_rx_destroy(solo_b200_rx *q);
+int solo_b200_rx_insert_host(solo_b200_rx *q, const int32_t *stream, const uint32_t *index, const uint8_t *desc,
+                             const int32_t *off, const int32_t *len, int n_arrivals, const uint8_t *payload,
+                             int64_t payload_bytes);
+int solo_b200_rx_insert_device(solo_b200_rx *q, const int32_t *d_stream, const uint32_t *d_index, const uint8_t *d_desc,
+                               const int32_t *d_off, const int32_t *d_len, int n_arrivals, const uint8_t *d_payload,
+                               int64_t payload_bytes, void *cuda_stream);
+int solo_b200_rx_pull_host(solo_b200_rx *q, const uint32_t *play, uint8_t *bits, int cap, int16_t *nbytes,
+                           int32_t *lostflag);
+int solo_b200_rx_pull_device(solo_b200_rx *q, const uint32_t *d_play, uint8_t *d_bits, int cap, int16_t *d_nbytes,
+                             int32_t *d_lostflag, void *cuda_stream);
+int solo_b200_rx_reset(solo_b200_rx *q, const int32_t *streams, const uint32_t *start, int n, void *cuda_stream);
+int solo_b200_rx_stats(solo_b200_rx *q, uint32_t *counters, uint64_t *bad_stream, void *cuda_stream);
+
 /* Multi-GPU ingest through peer memory:after this call kernels launched on `device` may read and write buffers that live in
    `peer_device`'s memory (same process, or another process's allocation mapped with CUDA IPC).  The *_device entry points
    then accept such addresses for pcm / bits / nbytes / lostflag: the band-split kernel pulls its PCM rows over NVLink and

@@ -95,6 +95,15 @@ def lib():
             getattr(L, f).argtypes = [vp, vp, vp, vp, vp]
         L.solo_b200_mix_host.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp]
         L.solo_b200_mix_device.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]
+        L.solo_b200_rx_create.restype = vp
+        L.solo_b200_rx_create.argtypes = [C.c_int] * 4
+        L.solo_b200_rx_destroy.argtypes = [vp]
+        L.solo_b200_rx_insert_host.argtypes = [vp] * 6 + [C.c_int, vp, C.c_int64]
+        L.solo_b200_rx_insert_device.argtypes = [vp] * 6 + [C.c_int, vp, C.c_int64, vp]
+        L.solo_b200_rx_pull_host.argtypes = [vp, vp, vp, C.c_int, vp, vp]
+        L.solo_b200_rx_pull_device.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
+        L.solo_b200_rx_reset.argtypes = [vp, vp, vp, C.c_int, vp]
+        L.solo_b200_rx_stats.argtypes = [vp, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -498,3 +507,90 @@ def mix_device(d_in, d_out, spp, n, d_level, d_flags, d_room_start, d_members, n
                                    int(k), d_talkers, stream)
     if r:
         raise SoloError("mix_device failed (%d): %s" % (r, _err()))
+
+
+# ---- receive queue (include/solo_b200.h, solo_b200_rx_*) --------------------------------------------------------------
+RX_COUNTERS = ("stored", "duplicate", "late", "dropped", "malformed", "played_both", "played_one", "played_none")
+
+
+class RxQueue:
+    """Receive queue of N streams on one GPU: holds each packet's two descriptions as they arrive (early, out of order,
+    twice), pairs them and hands the decoder one row per stream and tick (see solo_b200_rx_* in include/solo_b200.h)."""
+
+    def __init__(self, n, depth=8, desc_cap=128, device=0):
+        self.n, self.depth, self.desc_cap = int(n), int(depth), int(desc_cap)
+        self.h = lib().solo_b200_rx_create(self.n, self.depth, self.desc_cap, int(device))
+        if not self.h:
+            raise SoloError("solo_b200_rx_create failed: " + _err())
+
+    def insert(self, streams, index, desc, payloads):
+        """Arrival a is description desc[a] (1 or 2) of packet index[a] of stream streams[a], bytes payloads[a]; the
+        payloads are laid out back to back for the call."""
+        streams = np.ascontiguousarray(streams, np.int32)
+        index = np.ascontiguousarray(np.asarray(index, np.int64) & 0xFFFFFFFF, np.uint32)
+        desc = np.ascontiguousarray(desc, np.uint8)
+        lens = np.array([len(p) for p in payloads], np.int32)
+        off = np.zeros(len(lens), np.int32)
+        if len(lens):
+            off[1:] = np.cumsum(lens[:-1], dtype=np.int64)
+        flat = np.frombuffer(b"".join(bytes(p) for p in payloads), np.uint8).copy()
+        if not (len(streams) == len(index) == len(desc) == len(lens)):
+            raise SoloError("RxQueue.insert: streams, index, desc and payloads differ in length")
+        r = lib().solo_b200_rx_insert_host(self.h, streams.ctypes.data, index.ctypes.data, desc.ctypes.data, off.ctypes.data,
+                                           lens.ctypes.data, len(streams), flat.ctypes.data, flat.size)
+        if r:
+            raise SoloError("rx_insert_host failed (%d): %s" % (r, _err()))
+
+    def insert_device(self, d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes, stream=0):
+        """insert on device arrays (addresses), enqueued on `stream`: three kernel launches, none for n_arrivals = 0."""
+        r = lib().solo_b200_rx_insert_device(self.h, d_stream, d_index, d_desc, d_off, d_len, int(n_arrivals), d_payload,
+                                             int(payload_bytes), stream)
+        if r:
+            raise SoloError("rx_insert_device failed (%d): %s" % (r, _err()))
+
+    def pull(self, play=None, cap=256):
+        """One tick: -> (bits uint8 [N, cap], nbytes int16 [N, 2], lostflag int32 [N]) of packet play[s] (None: each
+        stream's last + 1), ready for DecoderBatch.decode.  Row bytes after nbytes[s, 0] are zero."""
+        p = None
+        if play is not None:
+            p = np.ascontiguousarray(np.asarray(play, np.int64) & 0xFFFFFFFF, np.uint32)
+            if p.shape != (self.n,):
+                raise SoloError("RxQueue.pull: play must have %d entries" % self.n)
+        bits = np.zeros((self.n, int(cap)), np.uint8)
+        nbytes = np.zeros((self.n, 2), np.int16)
+        lostflag = np.zeros(self.n, np.int32)
+        r = lib().solo_b200_rx_pull_host(self.h, p.ctypes.data if p is not None else None, bits.ctypes.data, int(cap),
+                                         nbytes.ctypes.data, lostflag.ctypes.data)
+        if r:
+            raise SoloError("rx_pull_host failed (%d): %s" % (r, _err()))
+        return bits, nbytes, lostflag
+
+    def pull_device(self, d_play, d_bits, cap, d_nbytes, d_lostflag, stream=0):
+        """pull on device arrays (d_play = 0 for last + 1), enqueued on `stream`: one kernel launch."""
+        r = lib().solo_b200_rx_pull_device(self.h, d_play or None, d_bits, int(cap), d_nbytes, d_lostflag, stream)
+        if r:
+            raise SoloError("rx_pull_device failed (%d): %s" % (r, _err()))
+
+    def reset(self, streams, start, stream=0):
+        """Empty the listed streams' slots, zero their counters, and play packet start[i] next on stream streams[i]."""
+        streams = np.ascontiguousarray(streams, np.int32).ravel()
+        start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
+        r = lib().solo_b200_rx_reset(self.h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
+        if r:
+            raise SoloError("rx_reset failed (%d): %s" % (r, _err()))
+
+    def stats(self, stream=0):
+        """(counters uint32 [N, 8] in the order of RX_COUNTERS, arrivals for streams outside [0, N))."""
+        cnt = np.zeros((self.n, 8), np.uint32)
+        bad = C.c_uint64()
+        r = lib().solo_b200_rx_stats(self.h, cnt.ctypes.data, C.byref(bad), stream)
+        if r:
+            raise SoloError("rx_stats failed (%d): %s" % (r, _err()))
+        return cnt, int(bad.value)
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().solo_b200_rx_destroy(self.h)
+            self.h = None
+
+    __del__ = close

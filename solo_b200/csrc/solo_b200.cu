@@ -18,6 +18,9 @@
 // and voice-activity / concealment flags of that wave (sb_activity.cuh).
 // The conference mixer (solo_b200_mix_*, sb_mix.cuh) is two launches of its own: sb_mix_select_kernel (warp per room) picks
 // each room's loudest talkers, sb_mix_kernel (warp per member) writes each member's mix-minus row.
+// The receive queue (solo_b200_rx_*, sb_rx.cuh) pairs, reorders and screens the two descriptions of each stream's packets:
+// an insert is sb_rx_elect_kernel, sb_rx_classify_kernel and sb_rx_commit_kernel over the arrivals, a pull is
+// sb_rx_pull_kernel (warp per stream), which writes the decoder's input rows.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -34,6 +37,7 @@
 #include "sb_enc.cuh"
 #include "sb_mix.cuh"
 #include "sb_nsq_warp.cuh"
+#include "sb_rx.cuh"
 
 using namespace sb;
 
@@ -415,6 +419,185 @@ __global__ void __launch_bounds__(SB_MIX_WARPS * 32, 6) sb_mix_kernel(const i16*
             dst[c] = make_int4(w[0], w[1], w[2], w[3]);
         }
     }
+}
+
+// ---- receive queue (sb_rx.cuh) -------------------------------------------------------------------------------------------
+// The queue's device arrays.  Slot metadata (index, the two lengths, the election words) is kept apart from the payload
+// store, so the election and classify passes touch a few bytes per slot.  Slot sl = s * depth + j; description d of it is
+// store[(2 * sl + d) * desc_cap ...], 16-byte aligned (desc_cap is a multiple of 16); the store has 16 bytes of padding
+// after the last slot for the pull kernel's second aligned load.
+struct RxDev {
+    int n, depth, desc_cap;
+    u32* last;                  // [n] last played index
+    u32* idx;                   // [n][depth] held index
+    u16* len;                   // [n][depth][2] held description lengths, 0 = not held
+    unsigned long long* elect;  // [n][depth][2] election words of the running insert, 0 between calls
+    u32* rep;                   // [n][depth] position of the arrival that commits the slot, RX_NO_REP between calls
+    u32* cnt;                   // [n][RX_NCOUNT]
+    unsigned long long* bad;    // arrivals for streams outside [0, n)
+    u8* store;                  // [n][depth][2][desc_cap] + 16
+};
+struct RxArrivals {
+    const i32* stream; const u32* index; const u8* desc; const i32* off; const i32* len;
+    int n; const u8* payload; i64 payload_bytes;
+};
+__device__ __forceinline__ long long rx_arrival_slot_of(const RxDev& q, const RxArrivals& A, int a, u32* dist) {
+    return rx_arrival_slot(q.n, q.depth, q.desc_cap, q.last, A.stream[a], A.desc[a], A.off[a], A.len[a], A.index[a],
+                           A.payload_bytes, dist);
+}
+
+#define SB_RX_THREADS 256
+#define SB_RX_TEAM 8            // lanes per arrival in the classify pass: 16 bytes each, 128 bytes per round
+// insert, pass 1 (thread per arrival): per (slot, desc) the newest index and its first arrival; per slot the first arrival
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_elect_kernel(RxDev q, RxArrivals A) {
+    const int a = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (a >= A.n) return;
+    u32 dist;
+    const long long sl = rx_arrival_slot_of(q, A, a, &dist);
+    if (sl < 0) return;
+    atomicMax(&q.elect[2 * sl + A.desc[a] - 1], (unsigned long long)rx_key(dist, a));
+    atomicMin(&q.rep[sl], (u32)a);
+}
+
+// insert, pass 2 (SB_RX_TEAM lanes per arrival): count every arrival once and copy the stored ones to their slot, 16-byte
+// stores from byte loads of the unaligned source.  Reads the slots' metadata and election words, writes neither.
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_classify_kernel(RxDev q, RxArrivals A) {
+    const long long g = (long long)blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    const int a = (int)(g / SB_RX_TEAM), t = (int)(g % SB_RX_TEAM);
+    if (a >= A.n) return;
+    const i32 s = A.stream[a];
+    if ((u32)s >= (u32)q.n) {
+        if (t == 0) atomicAdd(q.bad, 1ull);
+        return;
+    }
+    const int d = A.desc[a];
+    const i32 o = A.off[a], l = A.len[a];
+    int cls;
+    long long sl = -1;
+    if (rx_malformed(d, o, l, q.desc_cap, A.payload_bytes)) cls = RX_MALFORMED;
+    else if (!rx_current(A.index[a], q.last[s])) cls = RX_LATE;
+    else {
+        const u32 p = A.index[a], last = q.last[s];
+        sl = (long long)s * q.depth + rx_slot(p, q.depth);
+        const u64 e[2] = {q.elect[2 * sl], q.elect[2 * sl + 1]};
+        const u16 ln[2] = {q.len[2 * sl], q.len[2 * sl + 1]};
+        cls = rx_classify(p - last, d - 1, a, e, q.idx[sl], ln, last);
+    }
+    if (t == 0) atomicAdd(&q.cnt[(size_t)s * RX_NCOUNT + cls], 1u);
+    if (cls != RX_STORED) return;
+    const u8* src = A.payload + o;
+    uint4* dst = reinterpret_cast<uint4*>(q.store + (size_t)(2 * sl + d - 1) * q.desc_cap);
+    for (int c = t; 16 * c < l; c += SB_RX_TEAM) {
+        u32 w[4] = {0, 0, 0, 0};
+#pragma unroll
+        for (int i = 0; i < 16; i++)
+            if (16 * c + i < l) w[i >> 2] |= (u32)src[16 * c + i] << (8 * (i & 3));
+        dst[c] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+}
+
+// insert, pass 3 (thread per arrival): the slot's committing arrival writes its new index and lengths, counts the held
+// descriptions it discards and empties the election words
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_commit_kernel(RxDev q, RxArrivals A) {
+    const int a = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (a >= A.n) return;
+    u32 dist;
+    const long long sl = rx_arrival_slot_of(q, A, a, &dist);
+    if (sl < 0 || q.rep[sl] != (u32)a) return;
+    const i32 s = A.stream[a];
+    const u64 e[2] = {q.elect[2 * sl], q.elect[2 * sl + 1]};
+    u32 id = q.idx[sl];
+    u16 ln[2] = {q.len[2 * sl], q.len[2 * sl + 1]};
+    const int discarded = rx_commit(q.last[s], &id, ln, e, A.len);
+    q.idx[sl] = id;
+    q.len[2 * sl] = ln[0];
+    q.len[2 * sl + 1] = ln[1];
+    if (discarded) atomicAdd(&q.cnt[(size_t)s * RX_NCOUNT + RX_DROPPED], (u32)discarded);
+    q.elect[2 * sl] = 0;
+    q.elect[2 * sl + 1] = 0;
+    q.rep[sl] = RX_NO_REP;
+}
+
+// 16 bytes of the merged row [description 1 (n1 bytes) | description 2] starting at row byte 16c, from the slot's two
+// descriptions at S (16-byte aligned) and S + desc_cap.  Row bytes below n1 come from the aligned chunk c of description 1,
+// the others from description 2 at byte desc_cap + 16c - n1: two aligned loads, a word select and a funnel shift.
+__device__ __forceinline__ void rx_row_chunk(const u8* S, int desc_cap, int n1, int c, u32 w[4]) {
+    const int base = 16 * c;
+    u32 wa[4] = {0, 0, 0, 0}, wb[4] = {0, 0, 0, 0};
+    if (base < n1) {
+        const uint4 x = reinterpret_cast<const uint4*>(S)[c];
+        wa[0] = x.x; wa[1] = x.y; wa[2] = x.z; wa[3] = x.w;
+    }
+    if (base + 16 > n1) {
+        const int b = desc_cap + base - n1;
+        const uint4* src = reinterpret_cast<const uint4*>(S + (b & ~15));
+        const uint4 x = src[0], y = (b & 15) ? src[1] : make_uint4(0, 0, 0, 0);
+        const u32 v[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
+        const int sh = (b & 15) >> 2, bs = (b & 3) * 8;
+        u32 r[5];
+#pragma unroll
+        for (int k = 0; k < 5; k++) r[k] = sh == 0 ? v[k] : sh == 1 ? v[k + 1] : sh == 2 ? v[k + 2] : v[k + 3];
+#pragma unroll
+        for (int k = 0; k < 4; k++) wb[k] = __funnelshift_r(r[k], r[k + 1], bs);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int m = imin(imax(n1 - (base + 4 * k), 0), 4);      // bytes of word k that come from description 1
+        const u32 mask = m >= 4 ? 0xFFFFFFFFu : (1u << (8 * m)) - 1u;
+        w[k] = (wa[k] & mask) | (wb[k] & ~mask);
+    }
+}
+
+// pull (warp per stream): the row, nbytes and lostflag of index t = play[s] (or last + 1), then last = t and the slot
+// emptied when its index is no longer current.  Only bytes below nbytes[0] of the row are written: 16-byte stores when the
+// row is 16-byte aligned, byte stores for the tail.
+#define SB_RX_PULL_WARPS 8
+__global__ void __launch_bounds__(SB_RX_PULL_WARPS * 32) sb_rx_pull_kernel(RxDev q, const u32* __restrict__ play, u8* __restrict__ bits,
+                                                                            int cap, i16* __restrict__ nbytes, i32* __restrict__ lostflag) {
+    const int s = blockIdx.x * SB_RX_PULL_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (s >= q.n) return;                         // whole warps
+    const u32 t = play ? play[s] : q.last[s] + 1u;
+    const size_t sl = (size_t)s * q.depth + rx_slot(t, q.depth);
+    const u32 id = q.idx[sl];
+    u16 ln[2] = {q.len[2 * sl], q.len[2 * sl + 1]};
+    int n1, n2;
+    rx_play(t, id, ln, &n1, &n2);
+    i16 nb[2];
+    i32 lf;
+    const int nrow = rx_merge(n1, n2, nb, &lf);
+    const u8* S = q.store + 2 * sl * (size_t)q.desc_cap;
+    u8* row = bits + (size_t)s * cap;
+    const bool aligned = (cap & 15) == 0;
+    for (int c = lane; 16 * c < nrow; c += 32) {
+        u32 w[4] = {0, 0, 0, 0};
+        if (lf != 1) rx_row_chunk(S, q.desc_cap, n1, c, w);
+        if (aligned && 16 * c + 16 <= nrow) {
+            *reinterpret_cast<uint4*>(row + 16 * c) = make_uint4(w[0], w[1], w[2], w[3]);
+        } else {
+            for (int i = 0; i < 16 && 16 * c + i < nrow; i++) row[16 * c + i] = (u8)(w[i >> 2] >> (8 * (i & 3)));
+        }
+    }
+    if (lane == 0) {
+        nbytes[2 * s] = nb[0];
+        nbytes[2 * s + 1] = nb[1];
+        lostflag[s] = lf;
+        q.last[s] = t;
+        u32* cnt = q.cnt + (size_t)s * RX_NCOUNT;
+        cnt[rx_played_counter(n1, n2)]++;
+        if (const int stale = rx_after_play(t, id, ln)) cnt[RX_DROPPED] += stale;
+        q.len[2 * sl] = ln[0];
+        q.len[2 * sl + 1] = ln[1];
+    }
+}
+
+// reset (thread per listed stream; the host has checked the list): empty slots, zero counters, last = start - 1
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_reset_kernel(RxDev q, const i32* __restrict__ streams, const u32* __restrict__ start, int n) {
+    const int i = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (i >= n) return;
+    const i32 s = streams[i];
+    q.last[s] = start[i] - 1u;
+    for (int k = 0; k < RX_NCOUNT; k++) q.cnt[(size_t)s * RX_NCOUNT + k] = 0;
+    for (int j = 0; j < 2 * q.depth; j++) q.len[(size_t)s * 2 * q.depth + j] = 0;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -997,21 +1180,15 @@ int solo_b200_split_packet(const uint8_t* bits, const int16_t* nbytes, const uin
 }
 int solo_b200_merge_packets(const uint8_t* p1, int n1, const uint8_t* p2, int n2, uint8_t* bits, int cap, int16_t* nbytes, int32_t* lostflag) {
     if (!bits || !nbytes || !lostflag || n1 < 0 || n2 < 0) return -1;
-    const int have1 = p1 && n1 > 0, have2 = p2 && n2 > 0;
-    if (have1 && have2) {
-        if (n1 + n2 > cap) return -1;
-        memmove(bits, p1, (size_t)n1); memmove(bits + n1, p2, (size_t)n2);
-        nbytes[0] = (int16_t)(n1 + n2); nbytes[1] = (int16_t)n2; *lostflag = 4;
-    } else if (have1) {
-        if (n1 > cap) return -1;
-        memmove(bits, p1, (size_t)n1); nbytes[0] = (int16_t)n1; nbytes[1] = 0; *lostflag = 2;
-    } else if (have2) {
-        if (n2 > cap) return -1;
-        memmove(bits, p2, (size_t)n2); nbytes[0] = (int16_t)n2; nbytes[1] = 0; *lostflag = 3;
-    } else {
-        // nothing arrived: the decoder conceals; it still wants nBytes[0] > 0 (AGR_BWE_SDK_API.c:268-270), the bytes are not read
-        nbytes[0] = 16; nbytes[1] = 8; *lostflag = 1;
+    const int m1 = p1 && n1 > 0 ? n1 : 0, m2 = p2 && n2 > 0 ? n2 : 0;   // the descriptions that arrived
+    const long long total = (long long)m1 + m2;
+    if (total > 0 && total > cap) return -1;
+    rx_merge(m1, m2, nbytes, lostflag);
+    if (total == 0) {
         if (cap >= 16) memset(bits, 0, 16);
+    } else {
+        if (m1) memmove(bits, p1, (size_t)m1);
+        if (m2) memmove(bits + m1, p2, (size_t)m2);
     }
     return 0;
 }
@@ -1120,6 +1297,193 @@ int solo_b200_mix_host(const int16_t* in, int16_t* out, int spp, int n, const ui
     ok(cudaStreamSynchronize(st), "mix");
     cudaStreamDestroy(st);
     return r;
+}
+
+// ---- receive queue (sb_rx.cuh) -------------------------------------------------------------------------------------------
+struct solo_b200_rx {
+    int device;
+    cudaStream_t st;            // the _host forms' stream
+    RxDev q;
+    ~solo_b200_rx() {
+        if (st) cudaStreamDestroy(st);
+        cudaFree(q.last); cudaFree(q.idx); cudaFree(q.len); cudaFree(q.elect); cudaFree(q.rep); cudaFree(q.cnt);
+        cudaFree(q.bad); cudaFree(q.store);
+    }
+};
+
+solo_b200_rx* solo_b200_rx_create(int n_streams, int depth, int desc_cap, int device) {
+    if (n_streams <= 0 || depth < 2 || depth > 32 || (depth & (depth - 1)) || desc_cap < 16 || desc_cap > 1024 || desc_cap % 16) {
+        snprintf(g_err, sizeof g_err, "rx_create: bad argument (n %d, depth %d, desc_cap %d)", n_streams, depth, desc_cap);
+        return nullptr;
+    }
+    if (require_gpu(device)) return nullptr;
+    solo_b200_rx* r = new solo_b200_rx();
+    r->device = device;
+    RxDev& q = r->q;
+    q.n = n_streams; q.depth = depth; q.desc_cap = desc_cap;
+    const size_t n = (size_t)n_streams, slots = n * depth, store = slots * 2 * desc_cap + 16;
+    bool ok = cudaStreamCreateWithFlags(&r->st, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaMalloc(&q.last, 4 * n) == cudaSuccess && cudaMalloc(&q.idx, 4 * slots) == cudaSuccess &&
+              cudaMalloc(&q.len, 4 * slots) == cudaSuccess && cudaMalloc(&q.elect, 16 * slots) == cudaSuccess &&
+              cudaMalloc(&q.rep, 4 * slots) == cudaSuccess && cudaMalloc(&q.cnt, 4 * RX_NCOUNT * n) == cudaSuccess &&
+              cudaMalloc(&q.bad, 8) == cudaSuccess && cudaMalloc(&q.store, store) == cudaSuccess;
+    // last = 0xFFFFFFFF (index 0 plays first), slots empty, election words empty, counters zero
+    ok = ok && cudaMemsetAsync(q.last, 0xFF, 4 * n, r->st) == cudaSuccess && cudaMemsetAsync(q.idx, 0, 4 * slots, r->st) == cudaSuccess &&
+         cudaMemsetAsync(q.len, 0, 4 * slots, r->st) == cudaSuccess && cudaMemsetAsync(q.elect, 0, 16 * slots, r->st) == cudaSuccess &&
+         cudaMemsetAsync(q.rep, 0xFF, 4 * slots, r->st) == cudaSuccess && cudaMemsetAsync(q.cnt, 0, 4 * RX_NCOUNT * n, r->st) == cudaSuccess &&
+         cudaMemsetAsync(q.bad, 0, 8, r->st) == cudaSuccess && cudaMemsetAsync(q.store, 0, store, r->st) == cudaSuccess &&
+         cudaStreamSynchronize(r->st) == cudaSuccess;
+    if (!ok) {
+        snprintf(g_err, sizeof g_err, "rx_create: %s", cudaGetErrorString(cudaGetLastError()));
+        delete r;
+        return nullptr;
+    }
+    return r;
+}
+
+void solo_b200_rx_destroy(solo_b200_rx* q) {
+    if (!q) return;
+    cudaSetDevice(q->device);
+    delete q;
+}
+
+// the three insert passes on st; nothing for no arrivals
+static int rx_insert_launch(solo_b200_rx* r, const RxArrivals& A, cudaStream_t st) {
+    if (A.n == 0) return 0;
+    const unsigned g = (unsigned)(((long long)A.n + SB_RX_THREADS - 1) / SB_RX_THREADS);
+    const unsigned g2 = (unsigned)(((long long)A.n * SB_RX_TEAM + SB_RX_THREADS - 1) / SB_RX_THREADS);
+    sb_rx_elect_kernel<<<g, SB_RX_THREADS, 0, st>>>(r->q, A);
+    count_launch();
+    CK(cudaGetLastError());
+    sb_rx_classify_kernel<<<g2, SB_RX_THREADS, 0, st>>>(r->q, A);
+    count_launch();
+    CK(cudaGetLastError());
+    sb_rx_commit_kernel<<<g, SB_RX_THREADS, 0, st>>>(r->q, A);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+static int rx_insert_args_ok(solo_b200_rx* q, const void* stream, const void* index, const void* desc, const void* off,
+                             const void* len, int n_arrivals, const void* payload, int64_t payload_bytes) {
+    if (q && n_arrivals >= 0 && payload_bytes >= 0 && (n_arrivals == 0 || (stream && index && desc && off && len)) &&
+        (payload || payload_bytes == 0))
+        return 1;
+    snprintf(g_err, sizeof g_err, "rx_insert: bad argument (n_arrivals %d, payload_bytes %lld)", n_arrivals, (long long)payload_bytes);
+    return 0;
+}
+
+int solo_b200_rx_insert_device(solo_b200_rx* q, const int32_t* d_stream, const uint32_t* d_index, const uint8_t* d_desc,
+                               const int32_t* d_off, const int32_t* d_len, int n_arrivals, const uint8_t* d_payload,
+                               int64_t payload_bytes, void* cuda_stream) {
+    if (!rx_insert_args_ok(q, d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes)) return -1;
+    if (n_arrivals == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    const RxArrivals A = {d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes};
+    return rx_insert_launch(q, A, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_rx_insert_host(solo_b200_rx* q, const int32_t* stream, const uint32_t* index, const uint8_t* desc,
+                             const int32_t* off, const int32_t* len, int n_arrivals, const uint8_t* payload, int64_t payload_bytes) {
+    if (!rx_insert_args_ok(q, stream, index, desc, off, len, n_arrivals, payload, payload_bytes)) return -1;
+    if (n_arrivals == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    const size_t na = (size_t)n_arrivals, pb = (size_t)payload_bytes;
+    cudaStream_t st = q->st;
+    u8* d = nullptr;            // [stream | index | off | len] int32 x n, desc x n, payload
+    int r = 0;
+    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
+    if (ok(cudaMallocAsync(&d, 17 * na + pb, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d, stream, 4 * na, cudaMemcpyHostToDevice, st), "copy stream") &&
+        ok(cudaMemcpyAsync(d + 4 * na, index, 4 * na, cudaMemcpyHostToDevice, st), "copy index") &&
+        ok(cudaMemcpyAsync(d + 8 * na, off, 4 * na, cudaMemcpyHostToDevice, st), "copy off") &&
+        ok(cudaMemcpyAsync(d + 12 * na, len, 4 * na, cudaMemcpyHostToDevice, st), "copy len") &&
+        ok(cudaMemcpyAsync(d + 16 * na, desc, na, cudaMemcpyHostToDevice, st), "copy desc") &&
+        (pb == 0 || ok(cudaMemcpyAsync(d + 17 * na, payload, pb, cudaMemcpyHostToDevice, st), "copy payload"))) {
+        const RxArrivals A = {(const i32*)d, (const u32*)(d + 4 * na), d + 16 * na, (const i32*)(d + 8 * na),
+                              (const i32*)(d + 12 * na), n_arrivals, d + 17 * na, payload_bytes};
+        r = rx_insert_launch(q, A, st);
+    }
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "rx_insert");
+    return r;
+}
+
+static int rx_pull_args_ok(solo_b200_rx* q, const void* bits, int cap, const void* nbytes, const void* lostflag) {
+    if (!q || !bits || !nbytes || !lostflag) { snprintf(g_err, sizeof g_err, "rx_pull: bad argument"); return 0; }
+    if (cap < 2 * q->q.desc_cap) { snprintf(g_err, sizeof g_err, "rx_pull: cap %d is below 2 * desc_cap = %d", cap, 2 * q->q.desc_cap); return 0; }
+    return 1;
+}
+static int rx_pull_launch(solo_b200_rx* r, const u32* play, u8* bits, int cap, i16* nbytes, i32* lostflag, cudaStream_t st) {
+    sb_rx_pull_kernel<<<(r->q.n + SB_RX_PULL_WARPS - 1) / SB_RX_PULL_WARPS, SB_RX_PULL_WARPS * 32, 0, st>>>(r->q, play, bits, cap, nbytes, lostflag);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int solo_b200_rx_pull_device(solo_b200_rx* q, const uint32_t* d_play, uint8_t* d_bits, int cap, int16_t* d_nbytes,
+                             int32_t* d_lostflag, void* cuda_stream) {
+    if (!rx_pull_args_ok(q, d_bits, cap, d_nbytes, d_lostflag)) return -1;
+    if ((uintptr_t)d_bits & 15) { snprintf(g_err, sizeof g_err, "rx_pull_device: d_bits must be 16-byte aligned"); return -1; }
+    CK(cudaSetDevice(q->device));
+    return rx_pull_launch(q, d_play, d_bits, cap, d_nbytes, d_lostflag, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_rx_pull_host(solo_b200_rx* q, const uint32_t* play, uint8_t* bits, int cap, int16_t* nbytes, int32_t* lostflag) {
+    if (!rx_pull_args_ok(q, bits, cap, nbytes, lostflag)) return -1;
+    CK(cudaSetDevice(q->device));
+    const size_t n = (size_t)q->q.n, rows = n * (size_t)cap;
+    cudaStream_t st = q->st;
+    u8* d = nullptr;            // bits [n][cap] (the caller's rows go in, so bytes past nbytes[0] come back unchanged), nbytes,
+    int r = 0;                  // lostflag, play
+    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
+    const size_t o_nb = (rows + 15) / 16 * 16, o_lf = o_nb + 4 * n, o_play = o_lf + 4 * n;
+    if (ok(cudaMallocAsync(&d, o_play + 4 * n, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d, bits, rows, cudaMemcpyHostToDevice, st), "copy bits") &&
+        (!play || ok(cudaMemcpyAsync(d + o_play, play, 4 * n, cudaMemcpyHostToDevice, st), "copy play")) &&
+        !(r = rx_pull_launch(q, play ? (const u32*)(d + o_play) : nullptr, d, cap, (i16*)(d + o_nb), (i32*)(d + o_lf), st)))
+        ok(cudaMemcpyAsync(bits, d, rows, cudaMemcpyDeviceToHost, st), "copy bits") &&
+            ok(cudaMemcpyAsync(nbytes, d + o_nb, 4 * n, cudaMemcpyDeviceToHost, st), "copy nbytes") &&
+            ok(cudaMemcpyAsync(lostflag, d + o_lf, 4 * n, cudaMemcpyDeviceToHost, st), "copy lostflag");
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "rx_pull");
+    return r;
+}
+
+int solo_b200_rx_reset(solo_b200_rx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
+    if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "rx_reset: bad argument"); return -1; }
+    {
+        std::vector<u8> seen((size_t)q->q.n, 0);
+        for (int i = 0; i < n; i++) {
+            if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "rx_reset: stream %d outside [0, %d)", streams[i], q->q.n); return -1; }
+            if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "rx_reset: stream %d is listed twice", streams[i]); return -1; }
+        }
+    }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    u8* d = nullptr;
+    int r = 0;
+    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
+    if (ok(cudaMallocAsync(&d, 8 * (size_t)n, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d, streams, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy streams") &&
+        ok(cudaMemcpyAsync(d + 4 * (size_t)n, start, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy start")) {
+        sb_rx_reset_kernel<<<(n + SB_RX_THREADS - 1) / SB_RX_THREADS, SB_RX_THREADS, 0, st>>>(q->q, (const i32*)d, (const u32*)(d + 4 * (size_t)n), n);
+        count_launch();
+        ok(cudaGetLastError(), "sb_rx_reset_kernel");
+    }
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "rx_reset");
+    return r;
+}
+
+int solo_b200_rx_stats(solo_b200_rx* q, uint32_t* counters, uint64_t* bad_stream, void* cuda_stream) {
+    if (!q) { snprintf(g_err, sizeof g_err, "rx_stats: bad argument"); return -1; }
+    CK(cudaSetDevice(q->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    if (counters) CK(cudaMemcpyAsync(counters, q->q.cnt, 4 * RX_NCOUNT * (size_t)q->q.n, cudaMemcpyDeviceToHost, st));
+    if (bad_stream) CK(cudaMemcpyAsync(bad_stream, q->q.bad, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 // ---- multi-GPU ingest through peer memory --------------------------------------------------------------------------------
