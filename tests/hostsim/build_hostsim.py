@@ -11,27 +11,36 @@ if ROOT not in sys.path:
 from solo_b200 import build as sb_build  # noqa: E402
 
 OUT_DIR = os.path.join(ROOT, "tests", "_hostsim")
-OUT = os.path.join(OUT_DIR, "libsb_hostsim.so")
 SRC = os.path.join(HERE, "hostsim.cpp")
+
+
+LIB_FLAGS = ["-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w"]
 
 
 def build(force=False, emu=False):
     """emu=True: the cooperative (32 threads per stream) build of the analysis stage, libsb_hostsim_emu.so;
     emu="gw16": the same with the quantiser code in its two-lane-groups-per-warp packing, libsb_hostsim_emu16.so."""
     if emu == "gw16":
-        return _build(os.path.join(OUT_DIR, "libsb_hostsim_emu16.so"), ["-DSB_EMU", "-DSB_EMU_GW16"], force)
+        return _build("libsb_hostsim_emu16.so", SRC, LIB_FLAGS + ["-DSB_EMU", "-DSB_EMU_GW16"], force)
     if emu:
-        return _build(os.path.join(OUT_DIR, "libsb_hostsim_emu.so"), ["-DSB_EMU"], force)
-    return _build(OUT, [], force)
+        return _build("libsb_hostsim_emu.so", SRC, LIB_FLAGS + ["-DSB_EMU"], force)
+    return _build("libsb_hostsim.so", SRC, LIB_FLAGS, force)
 
 
-def _build(OUT, extra, force):
+def build_fuzzer(force=False):
+    """The malformed-packet fuzzer (fuzz_dec.cpp) under AddressSanitizer and UBSan, tests/_hostsim/fuzz_dec."""
+    return _build("fuzz_dec", os.path.join(HERE, "fuzz_dec.cpp"),
+                  ["-O1", "-g", "-std=c++17", "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-w"], force)
+
+
+def _build(name, src, flags, force):
     os.makedirs(OUT_DIR, exist_ok=True)
-    deps = sb_build.sources() + [SRC, os.path.abspath(__file__)]     # the flags live here: a flag change rebuilds
-    if not force and os.path.exists(OUT) and all(os.path.getmtime(d) <= os.path.getmtime(OUT) for d in deps):
-        return OUT
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w"] + extra + [SRC, "-o", OUT])
-    return OUT
+    out = os.path.join(OUT_DIR, name)
+    deps = sb_build.sources() + [src, os.path.abspath(__file__)]     # the flags live here: a flag change rebuilds
+    if not force and os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
+        return out
+    subprocess.check_call(["g++"] + flags + [src, "-o", out])
+    return out
 
 
 if __name__ == "__main__":

@@ -106,6 +106,7 @@ static void run32m(const std::function<void()>& f) {
 #endif
 #include "../../solo_b200/csrc/sb_enc.cuh"
 #include "../../solo_b200/csrc/sb_dec.cuh"
+#include "../../solo_b200/csrc/sb_activity.cuh"
 #include "../../oracle/nsq_io.h"
 #ifdef SB_EMU
 #include "../../solo_b200/csrc/sb_coop.cuh"
@@ -304,6 +305,11 @@ int hs_nsq_run(int kernel_code, int n, int npk, int nf, const NsqStateIO* st0, c
 // rate (b/s), DTX, expected loss (%) from the next packet on: the body of the device's control kernel on the host model's
 // state; -1 or any other out-of-range value leaves a setting alone
 void hs_enc_set_control(void* p, int rate, int dtx, int loss) { sb::enc_set_control(&((HsEnc*)p)->st, rate, dtx, loss); }
+// the activity kernel's flags of the last packet this encoder coded
+int hs_enc_flags(void* p) {
+    HsEnc* h = (HsEnc*)p;
+    return sb::enc_activity_flags(&h->w.scr, h->st.frames_per_packet);
+}
 void hs_enc_destroy(void* p) { free(p); }
 int hs_is_emu() {
 #ifdef SB_EMU
@@ -312,17 +318,41 @@ int hs_is_emu() {
     return 0;
 #endif
 }
+// the RFC 6464 level of a row whose sum of squares is E, and the activity kernel's level of one row of n samples
+int hs_level(long long E, int n) { return sb::rfc6464_level(E, n); }
+int hs_row_level(const short* pcm, int n) {
+    long long e = 0;
+    for (int i = 0; i < n; i++) e += (long long)pcm[i] * pcm[i];
+    return sb::rfc6464_level(e, n);
+}
+}
 
-struct HsDec { sb::DecState st; sb::DecPacketWork w; sb::DecStale stale; };
-void* hs_dec_create3(int mdi, int framesize_ms, int joint_hb) {
-    HsDec* h = (HsDec*)calloc(1, sizeof(HsDec));
-    sb::dec_state_init(&h->st, mdi, framesize_ms, joint_hb);
+// one decoder stream; samplerate (first, so that hs_dec_decode can read it) picks the core rate: 16000 -> KHZ 8, 32000 -> 16
+template <int KHZ> struct HsDec { int samplerate; sb::DecStateT<KHZ> st; sb::DecPacketWorkT<KHZ> w; sb::DecStale stale; };
+template <int KHZ> static void* dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate) {
+    HsDec<KHZ>* h = (HsDec<KHZ>*)calloc(1, sizeof(HsDec<KHZ>));
+    h->samplerate = samplerate;
+    sb::dec_state_init(&h->st, mdi, framesize_ms, joint_hb, arith);
     return h;
 }
-// same calling convention as AGR_Sate_Decoder_Decode (payload pre-trimmed by the caller); nb is not modified
-int hs_dec_decode(void* p, short* pcm, const unsigned char* bits, int cap, const short* nb, int lostflag) {
-    HsDec* h = (HsDec*)p;
-    return sb::dec_packet(&h->st, &h->w, pcm, bits, cap, nb, lostflag, &h->stale);
+template <int KHZ> static int dec_decode(void* p, short* pcm, const unsigned char* bits, int cap, const short* nb, int lostflag, unsigned char* flags) {
+    HsDec<KHZ>* h = (HsDec<KHZ>*)p;
+    const int r = sb::dec_packet(&h->st, &h->w, pcm, bits, cap, nb, lostflag, &h->stale);
+    if (flags) *flags = r < 0 ? 0 : h->w.act;      // what the decode kernel stores for the activity kernel
+    return r;
+}
+
+extern "C" {
+// arith: sb::DEC_FLP or sb::DEC_FIX; samplerate 16000 or 32000 (NULL for any other)
+void* hs_dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate) {
+    if (samplerate == 16000) return dec_create<8>(mdi, framesize_ms, joint_hb, arith, samplerate);
+    if (samplerate == 32000) return dec_create<16>(mdi, framesize_ms, joint_hb, arith, samplerate);
+    return nullptr;
+}
+// same calling convention as AGR_Sate_Decoder_Decode (payload pre-trimmed by the caller); nb is not modified.  flags (may be
+// NULL): the packet's activity flags, 0 for a rejected packet
+int hs_dec_decode(void* p, short* pcm, const unsigned char* bits, int cap, const short* nb, int lostflag, unsigned char* flags) {
+    return *(const int*)p == 32000 ? dec_decode<16>(p, pcm, bits, cap, nb, lostflag, flags) : dec_decode<8>(p, pcm, bits, cap, nb, lostflag, flags);
 }
 void hs_dec_destroy(void* p) { free(p); }
 }

@@ -9,6 +9,7 @@ import numpy as np
 from . import build_hostsim
 
 _libs = {}
+ARITH = {"flp": 0, "fix": 1}   # sb::DEC_FLP / sb::DEC_FIX
 EMU = False   # set tests.hostsim.sim.EMU = True (or use emu=True) to drive the 32-thread cooperative build
 
 
@@ -18,16 +19,19 @@ def lib(emu=None):
         L = C.CDLL(build_hostsim.build(emu=emu))
         L.hs_enc_create3.restype = C.c_void_p
         L.hs_enc_create3.argtypes = [C.c_int] * 5
-        L.hs_dec_create3.restype = C.c_void_p
-        L.hs_dec_create3.argtypes = [C.c_int] * 3
+        L.hs_dec_create.restype = C.c_void_p
+        L.hs_dec_create.argtypes = [C.c_int] * 5
         L.hs_enc_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.hs_enc_destroy.argtypes = [C.c_void_p]
         L.hs_enc_set_control.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.hs_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+        L.hs_enc_flags.argtypes = [C.c_void_p]
+        L.hs_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.hs_dec_destroy.argtypes = [C.c_void_p]
         L.nsq_io_sizes.argtypes = [C.c_void_p]
         L.hs_enc_capture.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_void_p]
         L.hs_nsq_run.argtypes = [C.c_int] * 4 + [C.c_void_p] * 4
+        L.hs_level.argtypes = [C.c_longlong, C.c_int]
+        L.hs_row_level.argtypes = [C.c_void_p, C.c_int]
         if emu:
             L.hs_set_emu_nsq.argtypes = [C.c_int]
             L.hs_enc_encode_pair.argtypes = [C.c_void_p] * 6 + [C.c_int] + [C.c_void_p] * 3
@@ -70,6 +74,11 @@ class SimEncoder:
         assert n >= 0
         return fr, st
 
+    @property
+    def flags(self):
+        """The activity kernel's flags of the last packet: bit f = frame f's coded VAD flag, 0 for a DTX-dropped packet."""
+        return self.L.hs_enc_flags(self.h)
+
     def set_control(self, rate=None, dtx=None, loss=None):
         """Rate (b/s), DTX and expected loss (%) from the next packet on, through enc_set_control; None = unchanged."""
         self.L.hs_enc_set_control(self.h, *(-1 if v is None else int(v) for v in (rate, dtx, loss)))
@@ -109,17 +118,34 @@ def nsq_run(st0, frames, nf, emu=None):
     return out, st
 
 
+def level(E, n):
+    """RFC 6464 level of a row of n samples whose sum of squares is E (sb_activity.cuh)."""
+    return lib().hs_level(int(E), n)
+
+
+def row_level(x):
+    """The activity kernel's level of one int16 row."""
+    x = np.ascontiguousarray(x, np.int16)
+    return lib().hs_row_level(x.ctypes.data, x.size)
+
+
 class SimDecoder:
-    def __init__(self, use_md_index=0, framesize_ms=40, joint_hb=0):
+    def __init__(self, use_md_index=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000):
+        """arith "flp" / "fix": the reference's float or fixed-point build; samplerate 16000 or 32000 (16 kHz SILK core)."""
         self.L = lib()
-        self.h = self.L.hs_dec_create3(use_md_index, framesize_ms, joint_hb)
-        self.pcm = np.zeros(16 * framesize_ms, np.int16)
+        self.h = self.L.hs_dec_create(use_md_index, framesize_ms, joint_hb, ARITH[arith], samplerate)
+        assert self.h, samplerate
+        self.pcm = np.zeros(samplerate // 1000 * framesize_ms, np.int16)
+        self.fl = np.zeros(1, np.uint8)
+        self.flags = 0      # the activity flags of the last packet: bit f VAD flag, bit 2 + f concealed; 0 if rejected
 
     def decode(self, payload, nbytes, lostflag):
         buf = np.zeros(max(len(payload), 1), np.uint8)
         buf[:len(payload)] = np.frombuffer(payload, np.uint8)
         nb = np.array([nbytes[0], nbytes[1]], np.int16)
-        r = self.L.hs_dec_decode(self.h, self.pcm.ctypes.data, buf.ctypes.data, len(buf), nb.ctypes.data, int(lostflag))
+        r = self.L.hs_dec_decode(self.h, self.pcm.ctypes.data, buf.ctypes.data, len(buf), nb.ctypes.data, int(lostflag),
+                                 self.fl.ctypes.data)
+        self.flags = int(self.fl[0])
         return self.pcm.copy(), r
 
     def close(self):

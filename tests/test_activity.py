@@ -1,53 +1,23 @@
 """Activity reports on the CPU: the RFC 6464 level function and the per-frame VAD / concealment flags, through the host build
-of their source (tests/hostsim/activity.cpp: sb_activity.cuh with the encoder and decoder it reports on, compiled by g++).
+of their source (sb_activity.cuh with the encoder and decoder it reports on, in tests/hostsim).
 
 The level is checked at every threshold and against a floating-point restatement; the encoder's flags against the flags
 the decoder parses from the same payloads (and, through golden.npz's byte-identical reference payloads, against the
 reference encoder's VAD); the decoder's flags under the reference driver's 50 % loss process at 16 and 32 kHz."""
-import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 from tests.golden import make_golden_32k as mk
+from tests.parity import sim  # noqa: F401  (fixture)
 from tests.util import GOLDEN, load_clip, load_golden, loss_flags, receive, signal_classes
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "hostsim", "activity.cpp")
 ROWS = (320, 640, 1280)
-ARITH = {"flp": 0, "fix": 1}                    # sb::DEC_FLP / sb::DEC_FIX
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_level_tables  # noqa: E402
-
-
-def load_lib(out):
-    """Compile tests/hostsim/activity.cpp to `out` and load it."""
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w", SRC, "-o", out])
-    lib = C.CDLL(out)
-    lib.act_level.argtypes = [C.c_longlong, C.c_int]
-    lib.act_row_level.argtypes = [C.c_void_p, C.c_int]
-    lib.act_enc_create.restype = C.c_void_p
-    lib.act_enc_create.argtypes = [C.c_int] * 5
-    lib.act_enc_encode.argtypes = [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 2
-    lib.act_enc_destroy.argtypes = [C.c_void_p]
-    lib.act_dec_create.restype = C.c_void_p
-    lib.act_dec_create.argtypes = [C.c_int] * 5
-    lib.act_dec_decode.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
-    lib.act_dec_destroy.argtypes = [C.c_void_p]
-    return lib
-
-
-@pytest.fixture(scope="module")
-def L(tmp_path_factory):
-    return load_lib(str(tmp_path_factory.mktemp("activity") / "libactivity.so"))
-
-
-def row_level(L, x):
-    x = np.ascontiguousarray(x, np.int16)
-    return L.act_row_level(x.ctypes.data, x.size)
 
 
 def float_level(E, n):
@@ -58,53 +28,20 @@ def float_level(E, n):
     return np.clip(np.round(v), 0, 127).astype(np.int64)
 
 
-class Encoder:
-    def __init__(self, L, rate=13600, dtx=0, use_md_index=0, framesize_ms=40, joint_hb=0):
-        self.L, self.samples = L, 16 * framesize_ms
-        self.h = L.act_enc_create(rate, dtx, use_md_index, framesize_ms, joint_hb)
-        self.out, self.nb, self.fl = np.zeros(1024, np.uint8), np.zeros(2, np.int16), np.zeros(1, np.uint8)
-
-    def encode(self, pcm):
-        x = np.ascontiguousarray(pcm, np.int16)
-        n = self.L.act_enc_encode(self.h, x.ctypes.data, self.out.ctypes.data, 1024, self.nb.ctypes.data, self.fl.ctypes.data)
-        return bytes(self.out[:max(n, 0)]), (int(self.nb[0]), int(self.nb[1])), int(self.fl[0])
-
-    def close(self):
-        self.L.act_enc_destroy(self.h)
-
-
-class Decoder:
-    def __init__(self, L, use_md_index=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000):
-        self.L, self.sr = L, samplerate
-        self.h = L.act_dec_create(use_md_index, framesize_ms, joint_hb, ARITH[arith], samplerate)
-        self.pcm, self.fl = np.zeros(samplerate // 1000 * framesize_ms, np.int16), np.zeros(1, np.uint8)
-
-    def decode(self, payload, nbytes, lostflag):
-        buf = np.zeros(max(len(payload), 1), np.uint8)
-        buf[:len(payload)] = np.frombuffer(payload, np.uint8)
-        nb = np.array(nbytes, np.int16)
-        r = self.L.act_dec_decode(self.h, self.sr, self.pcm.ctypes.data, buf.ctypes.data, len(buf), nb.ctypes.data, int(lostflag),
-                                  self.fl.ctypes.data)
-        return self.pcm.copy(), r, int(self.fl[0])
-
-    def close(self):
-        self.L.act_dec_destroy(self.h)
-
-
 # ---- level ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("n", ROWS)
-def test_level_at_every_threshold(L, n):
+def test_level_at_every_threshold(sim, n):
     """At T_n[k] - 1, T_n[k] and T_n[k] + 1 for every k: the level is the number of thresholds above E."""
     T = np.array(gen_level_tables.thresholds(n), np.int64)
     for t in T:
         for E in (t - 1, t, t + 1):
             if E >= 0:
-                assert L.act_level(int(E), n) == int((E < T).sum()), (n, int(E))
-    assert L.act_level(0, n) == 127 and L.act_level(n << 30, n) == 0
+                assert sim.level(E, n) == int((E < T).sum()), (n, int(E))
+    assert sim.level(0, n) == 127 and sim.level(n << 30, n) == 0
 
 
 @pytest.mark.parametrize("n", ROWS)
-def test_level_against_float_restatement(L, n):
+def test_level_against_float_restatement(sim, n):
     """Random rows over the whole dynamic range: equal to round(10 log10(n 2^30 / E)) wherever E is not within 1e-9
     (relative) of a real threshold n 2^30 10^(-(k + 0.5) / 10)."""
     rng = np.random.Generator(np.random.PCG64(n))
@@ -116,30 +53,30 @@ def test_level_against_float_restatement(L, n):
         E = int((x.astype(np.int64) ** 2).sum())
         if E and np.min(np.abs(E - t_real) / t_real) < 1e-9:
             continue
-        assert row_level(L, x) == int(float_level(E, n)), (n, i, E)
+        assert sim.row_level(x) == int(float_level(E, n)), (n, i, E)
         checked += 1
     assert checked > 590
 
 
-def test_level_of_edge_rows(L):
+def test_level_of_edge_rows(sim):
     """Zeros 127, a +-32767 square 0, a full-scale sine 3, single-LSB noise as the float restatement (and near 115 - 10 log10
     of its density)."""
     rng = np.random.Generator(np.random.PCG64(3))
     for n in ROWS:
         t = np.arange(n)
-        assert row_level(L, np.zeros(n, np.int16)) == 127
-        assert row_level(L, np.where(t % 2 == 0, 32767, -32767)) == 0
-        assert row_level(L, np.full(n, -32768)) == 0
-        assert row_level(L, np.round(32767 * np.sin(2 * np.pi * 1000 * t / 16000 + 0.3))) == 3
+        assert sim.row_level(np.zeros(n, np.int16)) == 127
+        assert sim.row_level(np.where(t % 2 == 0, 32767, -32767)) == 0
+        assert sim.row_level(np.full(n, -32768)) == 0
+        assert sim.row_level(np.round(32767 * np.sin(2 * np.pi * 1000 * t / 16000 + 0.3))) == 3
         for p in (1.0, 0.5, 0.1, 1.0 / n):
             x = (rng.random(n) < p) * rng.choice([-1, 1], n)
             if not x.any():
                 x[0] = 1
             E = int((x ** 2).sum())
-            assert row_level(L, x) == int(float_level(E, n)), (n, p)
+            assert sim.row_level(x) == int(float_level(E, n)), (n, p)
         one = np.zeros(n, np.int16)
         one[7] = 1
-        assert row_level(L, one) == int(float_level(1, n)) == int(round(10 * np.log10(n * 2.0 ** 30)))
+        assert sim.row_level(one) == int(float_level(1, n)) == int(round(10 * np.log10(n * 2.0 ** 30)))
 
 
 def test_committed_tables_are_the_generators():
@@ -169,27 +106,32 @@ def inputs():
     return out
 
 
-def encode_with_flags(L, x, **kw):
-    e = Encoder(L, **kw)
+def encode_with_flags(sim, x, **kw):
+    """[(payload, (n0, n1), flags)] of the host encoder over x."""
+    e = sim.SimEncoder(**kw)
     k = e.samples
-    pk = [e.encode(x[i * k:(i + 1) * k]) for i in range(len(x) // k)]
+    pk = []
+    for i in range(len(x) // k):
+        b, nb, _ = e.encode(x[i * k:(i + 1) * k])
+        pk.append((b, nb, e.flags))
     e.close()
     return pk
 
 
 @pytest.mark.parametrize("mode", sorted(MODES))
-def test_encoder_flags_are_what_the_decoder_parses(L, mode):
+def test_encoder_flags_are_what_the_decoder_parses(sim, mode):
     """For every packet of every input: the encoder's flags equal the VAD flags the decoder parses from its payload; a
     DTX-dropped packet (nothing sent) reports 0.  20 ms packets never set bit 1."""
     cfg = MODES[mode]
     nf = cfg["framesize_ms"] // 20
     seen, dropped = set(), 0
     for name, x, kw in inputs():
-        pk = encode_with_flags(L, x, **cfg, **kw)
-        d = Decoder(L, **cfg)
+        pk = encode_with_flags(sim, x, **cfg, **kw)
+        d = sim.SimDecoder(**cfg)
         for p, (b, nb, fl) in enumerate(pk):
             assert fl & ~((1 << nf) - 1) == 0, (mode, name, p, fl)
-            y, r, dfl = d.decode(*receive(b, nb, 4))
+            y, r = d.decode(*receive(b, nb, 4))
+            dfl = d.flags
             assert r == 0
             if nb[0] <= 0:
                 assert fl == 0 and dfl == (0xC if nf == 2 else 0x4), (mode, name, p)
@@ -201,27 +143,27 @@ def test_encoder_flags_are_what_the_decoder_parses(L, mode):
     assert {0, (1 << nf) - 1} <= seen and dropped > 0, (seen, dropped)
 
 
-def test_encoder_flags_match_the_reference_payloads(L):
+def test_encoder_flags_match_the_reference_payloads(sim):
     """golden.npz holds the reference encoder's payloads of the clip (rate 13 600, 40 ms), byte-identical to the host
     model's: the VAD flags parsed from them are the host encoder's flags, packet by packet."""
     g = load_golden()
     clip = load_clip()
-    pk = encode_with_flags(L, clip, rate=13600)
+    pk = encode_with_flags(sim, clip, rate=13600)
     assert len(pk) == g["fix_nbytes"].shape[0]
-    d = Decoder(L)
+    d = sim.SimDecoder()
     for p, (b, nb, fl) in enumerate(pk):
         n0 = int(g["fix_nbytes"][p, 0])
         assert nb == tuple(int(v) for v in g["fix_nbytes"][p]) and b[:n0] == bytes(g["fix_bits"][p, :n0]), p
-        y, r, dfl = d.decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 4)
-        assert r == 0 and dfl == fl, (p, fl, dfl)
+        y, r = d.decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 4)
+        assert r == 0 and d.flags == fl, (p, fl, d.flags)
     d.close()
 
 
 # ---- decoder flags under loss -----------------------------------------------------------------------------------------
-def streams_16k(L):
+def streams_16k(sim):
     """(mode, packets, decoder kwargs) of the clip at 16 kHz, encoded by the host model."""
     clip = load_clip()[:640 * 80]
-    return [(m, [(b, nb) for b, nb, fl in encode_with_flags(L, clip, rate=13600, **cfg)], cfg) for m, cfg in MODES.items()]
+    return [(m, [(b, nb) for b, nb, fl in encode_with_flags(sim, clip, rate=13600, **cfg)], cfg) for m, cfg in MODES.items()]
 
 
 def streams_32k():
@@ -229,19 +171,23 @@ def streams_32k():
     return [(s, mk.packets(f, s), mk.STREAMS[s][1]) for s in ("hb40", "hb20", "joint")]
 
 
-def check_loss(L, pk, cfg, samplerate, arith, seed, lead=0):
+def check_loss(sim, pk, cfg, samplerate, arith, seed, lead=0):
     """One stream under the 50 % loss process of `seed`, its first `lead` packets lost (loss before any good frame)."""
     nf = cfg["framesize_ms"] // 20
     conc = 0xC if nf == 2 else 0x4
-    ref = Decoder(L, arith=arith, samplerate=samplerate, **cfg)
-    parsed = [ref.decode(*receive(b, nb, 4))[2] for b, nb in pk]
+    ref = sim.SimDecoder(arith=arith, samplerate=samplerate, **cfg)
+    parsed = []
+    for b, nb in pk:
+        ref.decode(*receive(b, nb, 4))
+        parsed.append(ref.flags)
     ref.close()
     flags = [1] * lead + loss_flags(len(pk), 50, seed=seed)[lead:]
-    d = Decoder(L, arith=arith, samplerate=samplerate, **cfg)
+    d = sim.SimDecoder(arith=arith, samplerate=samplerate, **cfg)
     n_lost = 0
     for p, (b, nb) in enumerate(pk):
         pb, pnb, fl = receive(b, nb, flags[p])
-        y, r, dfl = d.decode(pb, pnb, fl)
+        y, r = d.decode(pb, pnb, fl)
+        dfl = d.flags
         assert r == 0
         if fl == 1:
             assert dfl == conc, (p, dfl)
@@ -253,33 +199,33 @@ def check_loss(L, pk, cfg, samplerate, arith, seed, lead=0):
 
 
 @pytest.mark.parametrize("arith", ["flp", "fix"])
-def test_decoder_flags_under_loss_16k(L, arith):
+def test_decoder_flags_under_loss_16k(sim, arith):
     """The reference driver's 50 % loss process: the concealed bits are the frames of lost packets (lostflag 1, from the
     first packets on in the second run), the VAD bits of received frames those parsed from the same payloads loss-free."""
-    for mode, pk, cfg in streams_16k(L):
+    for mode, pk, cfg in streams_16k(sim):
         if arith == "fix" and cfg["framesize_ms"] == 20:
             continue
-        check_loss(L, pk, cfg, 16000, arith, 1)
-        check_loss(L, pk, cfg, 16000, arith, 4, lead=3)
+        check_loss(sim, pk, cfg, 16000, arith, 1)
+        check_loss(sim, pk, cfg, 16000, arith, 4, lead=3)
 
 
 @pytest.mark.parametrize("arith", ["flp", "fix"])
-def test_decoder_flags_under_loss_32k(L, arith):
+def test_decoder_flags_under_loss_32k(sim, arith):
     """The same for golden_32k.npz's 32 kHz streams (16 kHz SILK core)."""
     for s, pk, cfg in streams_32k():
         if arith == "fix" and cfg["framesize_ms"] == 20:
             continue
-        check_loss(L, pk, cfg, 32000, arith, 1)
-        check_loss(L, pk, cfg, 32000, arith, 4, lead=3)
+        check_loss(sim, pk, cfg, 32000, arith, 1)
+        check_loss(sim, pk, cfg, 32000, arith, 4, lead=3)
 
 
-def test_rejected_packet_reports_no_flags(L):
+def test_rejected_packet_reports_no_flags(sim):
     """A packet the decoder rejects (bad lostflag, 16 kHz-stream packets to a 32 kHz decoder) gives flags 0."""
     g = load_golden()
     n0 = int(g["fix_nbytes"][0, 0])
-    d = Decoder(L, samplerate=32000)
-    y, r, fl = d.decode(bytes(g["fix_bits"][0, :n0]), tuple(int(v) for v in g["fix_nbytes"][0]), 4)
-    assert r < 0 and fl == 0
-    y, r, fl = d.decode(bytes(16), (16, 8), 7)
-    assert r < 0 and fl == 0
+    d = sim.SimDecoder(samplerate=32000)
+    y, r = d.decode(bytes(g["fix_bits"][0, :n0]), tuple(int(v) for v in g["fix_nbytes"][0]), 4)
+    assert r < 0 and d.flags == 0
+    y, r = d.decode(bytes(16), (16, 8), 7)
+    assert r < 0 and d.flags == 0
     d.close()

@@ -1,60 +1,19 @@
 """32 kHz streams (the reference's 32 kHz API: 16 kHz SILK core, 8-16 kHz high band) through the decoder on the CPU: the host
-build of the kernel source (tests/hostsim/dec32.cpp, the DecState32 instantiation of sb_dec.cuh) against the reference's
-float and fixed-point decoders, at 0 LSB.
+build of the kernel source (tests/hostsim, the DecState32 instantiation of sb_dec.cuh) against the reference's float and
+fixed-point decoders, at 0 LSB.
 
 tests/golden/golden_32k.npz pins the reference's PCM of 32 kHz bitstreams by per-packet md5 (tests/golden/make_golden_32k.py);
 where oracle/_ref is built, the fixture is re-derived from it and the host model runs in lockstep with both reference
 decoders over inputs the fixture does not cover."""
-import ctypes as C
 import hashlib
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from tests.golden import make_golden_32k as mk
-from tests.parity import ref  # noqa: F401  (fixture)
-from tests.util import GOLDEN, load_clip, load_golden, loss_flags, loss_with_bursts, receive
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEC32_SRC = os.path.join(ROOT, "tests", "hostsim", "dec32.cpp")
-ARITH = {"flp": 0, "fix": 1}                    # sb::DEC_FLP / sb::DEC_FIX
-
-
-@pytest.fixture(scope="module")
-def fxlib(tmp_path_factory):
-    """The host build of sb_dec.cuh with its 16 and 32 kHz decoders (tests/hostsim/dec32.cpp), in a temporary directory."""
-    out = str(tmp_path_factory.mktemp("dec32") / "libdec32.so")
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w", DEC32_SRC, "-o", out])
-    L = C.CDLL(out)
-    L.d32_create.restype = C.c_void_p
-    L.d32_create.argtypes = [C.c_int] * 5
-    L.d32_decode.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.d32_destroy.argtypes = [C.c_void_p]
-    return L
-
-
-class Sim32Decoder:
-    """One 32 kHz stream of the host model (samplerate 16000: a 16 kHz stream); the calls of tests.ref32.Ref32Decoder."""
-
-    def __init__(self, L, use_md_index=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=32000):
-        self.L = L
-        self.samplerate = samplerate
-        self.h = L.d32_create(use_md_index, framesize_ms, joint_hb, ARITH[arith], samplerate)
-        self.pcm = np.zeros(samplerate // 1000 * framesize_ms, np.int16)
-
-    def decode(self, payload, nbytes, lostflag):
-        buf = np.zeros(max(len(payload), 1), np.uint8)
-        buf[:len(payload)] = np.frombuffer(payload, np.uint8)
-        nb = np.array([nbytes[0], nbytes[1]], np.int16)
-        r = self.L.d32_decode(self.h, self.samplerate, self.pcm.ctypes.data, buf.ctypes.data, len(buf), nb.ctypes.data, int(lostflag))
-        return self.pcm.copy(), r
-
-    def close(self):
-        if self.h:
-            self.L.d32_destroy(self.h)
-            self.h = None
+from tests.parity import ref, sim  # noqa: F401  (fixtures)
+from tests.util import GOLDEN, fuzz_decoder, load_clip, load_golden, loss_flags, loss_with_bursts, receive
 
 
 def load32():
@@ -65,10 +24,11 @@ CASES = mk.decode_cases()
 
 
 @pytest.mark.parametrize("key,stream,kind,rule", CASES, ids=[c[0] for c in CASES])
-def test_host_model_matches_fixture(fxlib, key, stream, kind, rule):
+def test_host_model_matches_fixture(sim, key, stream, kind, rule):
     """Every pinned 32 kHz decode, in the arithmetic of the reference build that made it: per-packet md5 equal (0 LSB)."""
     f = load32()
-    rows = mk.decode(Sim32Decoder(fxlib, arith=kind, **mk.STREAMS[stream][1]), mk.packets(f, stream), mk.flags_of(f, stream, rule))
+    d = sim.SimDecoder(arith=kind, samplerate=32000, **mk.STREAMS[stream][1])
+    rows = mk.decode(d, mk.packets(f, stream), mk.flags_of(f, stream, rule))
     assert all(len(y) == 32 * mk.STREAMS[stream][1]["framesize_ms"] for y in rows)
     got = mk.packet_md5(rows)
     bad = np.nonzero((got != f[key + "_packet_md5"]).any(axis=1))[0]
@@ -84,36 +44,36 @@ def test_fixture_rederived_from_oracle(ref):
         assert np.array_equal(np.asarray(f[k]), want[k]), k
 
 
-def test_other_core_rate_is_that_streams_error(fxlib):
+def test_other_core_rate_is_that_streams_error(sim):
     """A frame whose sampling-rate index is not the decoder's core rate is a rejected packet (-12), as a corrupted one: 16 kHz
     streams' packets (8 kHz core) to a 32 kHz decoder and 32 kHz streams' packets to a 16 kHz decoder.  The decoder stays
     usable: a good packet after the rejected ones decodes as it does on a fresh decoder."""
     g, f = load_golden(), load32()
     pk32 = mk.packets(f, "hb40")
     for arith in ("flp", "fix"):
-        d = Sim32Decoder(fxlib, arith=arith)
+        d = sim.SimDecoder(arith=arith, samplerate=32000)
         for i in range(3):
             n0 = int(g["fix_nbytes"][i, 0])
             y, r = d.decode(bytes(g["fix_bits"][i, :n0]), tuple(int(v) for v in g["fix_nbytes"][i]), 4)
             assert r == -12, (arith, i, r)
-        d16 = Sim32Decoder(fxlib, arith=arith, samplerate=16000)
+        d16 = sim.SimDecoder(arith=arith)
         for i in range(3):
             y, r = d16.decode(pk32[i][0], pk32[i][1], 4)
             assert r == -12, (arith, i, r)
         d16.close()
-        fresh = Sim32Decoder(fxlib, arith=arith)
+        fresh = sim.SimDecoder(arith=arith, samplerate=32000)
         ya, ra = d.decode(pk32[0][0], pk32[0][1], 4)
         yb, rb = fresh.decode(pk32[0][0], pk32[0][1], 4)
         assert ra == rb == 0 and np.array_equal(ya, yb)
         d.close(), fresh.close()
 
 
-def test_low_rate_handset_stream_is_rejected_not_misdecoded(ref, fxlib):
+def test_low_rate_handset_stream_is_rejected_not_misdecoded(ref, sim):
     """A reference 32 kHz encoder below the 16 kHz-core range (12 kb/s) codes a lower core; every such packet is -12 here."""
     from tests.ref32 import Ref32Encoder, with_high_band
     x = with_high_band(load_clip()[:640 * 10])
     e = Ref32Encoder("fix", rate=12000)
-    d = Sim32Decoder(fxlib)
+    d = sim.SimDecoder(samplerate=32000)
     for p in range(10):
         b, nb, n = e.encode(x[p * 1280:(p + 1) * 1280])
         assert d.decode(*receive(b, nb, 4))[1] == -12
@@ -165,7 +125,7 @@ def flags_for(kind, n, s):
 
 @pytest.mark.parametrize("cfg,rate,mdi,dtx,loss", LOCKSTEP, ids=["%s-%d-mdi%d-dtx%d-%s" % ("joint" if c.get("joint_hb") else "%dms" % c["framesize_ms"], r, m, d, l)
                                                              for c, r, m, d, l in LOCKSTEP])
-def test_lockstep_with_reference_decoders(ref, fxlib, cfg, rate, mdi, dtx, loss):
+def test_lockstep_with_reference_decoders(ref, sim, cfg, rate, mdi, dtx, loss):
     """Reference FIX encoder at 32 kHz -> (receiver under the loss process) -> host model and the reference decoders, float
     and (40 ms packets, joint mode 1) fixed point, over eight signal classes: every packet's PCM identical (0 LSB)."""
     from tests.ref32 import Ref32Decoder, Ref32Encoder
@@ -179,7 +139,7 @@ def test_lockstep_with_reference_decoders(ref, fxlib, cfg, rate, mdi, dtx, loss)
         fl = flags_for(loss, n, s)
         for kind in kinds:
             dr = Ref32Decoder(kind, use_md_index=mdi, **cfg)
-            ds = Sim32Decoder(fxlib, use_md_index=mdi, arith=kind, **cfg)
+            ds = sim.SimDecoder(use_md_index=mdi, arith=kind, samplerate=32000, **cfg)
             for p, (b, nb, _) in enumerate(pk):
                 rx = receive(b, nb, fl[p])
                 (ya, ra), (yb, rb) = dr.decode(*rx), ds.decode(*rx)
@@ -189,21 +149,15 @@ def test_lockstep_with_reference_decoders(ref, fxlib, cfg, rate, mdi, dtx, loss)
 
 
 def test_32k_decoder_survives_malformed_packets_under_asan(tmp_path):
-    """The ASan / UBSan fuzzer of tests/hostsim/dec32.cpp with the fixture's 32 kHz packets as its corpus: bit flips,
-    garbage, lying lengths, short rows and invalid flags into the 32 kHz decoders of both arithmetics."""
+    """The ASan / UBSan fuzzer of tests/hostsim/fuzz_dec.cpp with the fixture's 32 kHz packets as its corpus: bit flips,
+    garbage, lying lengths, short rows and invalid flags into the 32 kHz decoders of both arithmetics (float 40 ms, 20 ms
+    and joint mode 1; fixed point 40 ms and joint mode 1).  Every mode both decodes and rejects some of them."""
     f = load32()
     corpus = tmp_path / "corpus32.bit"
     with open(corpus, "wb") as out:
         for s in mk.STREAMS:
             for b, nb in mk.packets(f, s):
                 out.write(np.array(nb, np.int16).tobytes() + (b if nb[0] > 0 else b""))
-    exe = tmp_path / "fuzz_dec32"
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-w", "-DSB_DEC32_FUZZ",
-           DEC32_SRC, "-o", str(exe)]
-    try:
-        subprocess.check_call(cmd)
-    except (subprocess.CalledProcessError, FileNotFoundError):
-        pytest.skip("sanitizer build not available")
-    p = subprocess.run([str(exe), str(corpus), "1500", "11"], capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0 and "no memory errors" in p.stdout, p.stdout[-2000:] + p.stderr[-4000:]
-
+    counts = fuzz_decoder(1500, 11, corpus)
+    assert sorted(counts) == ["32k fix 40ms", "32k fix joint", "32k flp 20ms", "32k flp 40ms", "32k flp joint"], counts
+    assert all(ok > 0 and bad > 0 and ok + bad == 1500 for ok, bad in counts.values()), counts

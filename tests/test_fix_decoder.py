@@ -4,57 +4,20 @@ reference's fixed-point build (JC1_SDK_SRC_ARM), at 0 LSB.
 The reference ships a float and a fixed-point build whose decoded PCM differs in the high-band synthesis and the synthesis
 filter bank.  tests/golden/golden_fixdec.npz pins the fixed-point build's PCM of the clip's bitstreams by per-packet md5
 (made by tests/golden/make_golden_fixdec.py); where oracle/_ref is built, the fixture is re-derived from it and the host
-model runs in lockstep with the fixed-point decoder on inputs the fixture does not cover.  The host model of the decoder
-with a chosen arithmetic is tests/hostsim/fixdec.cpp, compiled here by g++."""
-import ctypes as C
+model runs in lockstep with the fixed-point decoder on inputs the fixture does not cover.  The decoder's fuzzer
+(tests/test_fuzz_decoder.py) covers the fixed-point arithmetic on malformed packets."""
 import hashlib
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from tests.golden.make_golden_32k import packet_md5
 from tests.parity import lockstep, ref, sim  # noqa: F401  (fixtures)
 from tests.util import GOLDEN, load_clip, load_golden, loss_flags, loss_with_bursts, signal_classes, synth_inputs, trim_payload
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FIXDEC_SRC = os.path.join(ROOT, "tests", "hostsim", "fixdec.cpp")
 CLI_MD5 = "149ad62fe193f19d6c80aacc7336ebce"    # the reference CLI's fixed-point decode of the clip at loss 0 (SURVEY.md 7.2)
-ARITH = {"flp": 0, "fix": 1}                    # sb::DEC_FLP / sb::DEC_FIX
-
-
-@pytest.fixture(scope="module")
-def fxlib(tmp_path_factory):
-    """The host build of sb_dec.cuh with per-stream arithmetic (tests/hostsim/fixdec.cpp), in a temporary directory."""
-    out = str(tmp_path_factory.mktemp("fixdec") / "libfixdec.so")
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-w", FIXDEC_SRC, "-o", out])
-    L = C.CDLL(out)
-    L.fx_dec_create.restype = C.c_void_p
-    L.fx_dec_create.argtypes = [C.c_int] * 4
-    L.fx_dec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.fx_dec_destroy.argtypes = [C.c_void_p]
-    return L
-
-
-class FixSimDecoder:
-    """One stream of the host model's decoder; same calls as oracle.ref.RefDecoder and tests.hostsim.sim.SimDecoder."""
-
-    def __init__(self, L, use_md_index=0, framesize_ms=40, joint_hb=0, arith="fix"):
-        self.L = L
-        self.h = L.fx_dec_create(use_md_index, framesize_ms, joint_hb, ARITH[arith])
-        self.pcm = np.zeros(16 * framesize_ms, np.int16)
-
-    def decode(self, payload, nbytes, lostflag):
-        buf = np.zeros(max(len(payload), 1), np.uint8)
-        buf[:len(payload)] = np.frombuffer(payload, np.uint8)
-        nb = np.array([nbytes[0], nbytes[1]], np.int16)
-        r = self.L.fx_dec_decode(self.h, self.pcm.ctypes.data, buf.ctypes.data, len(buf), nb.ctypes.data, int(lostflag))
-        return self.pcm.copy(), r
-
-    def close(self):
-        if self.h:
-            self.L.fx_dec_destroy(self.h)
-            self.h = None
 
 
 def load_fixdec():
@@ -87,17 +50,13 @@ def decode_all(dec, pk, flags):
     return out
 
 
-def packet_md5(rows):
-    return np.array([np.frombuffer(hashlib.md5(np.ascontiguousarray(x, np.int16).tobytes()).digest(), np.uint8) for x in rows])
-
-
 CASES = ["mode4", "mode2", "mode3", "loss50", "joint_mode4", "joint_loss30"]
 
 
 @pytest.mark.parametrize("case", CASES)
-def test_host_model_matches_fixture(fxlib, case):
+def test_host_model_matches_fixture(sim, case):
     pk, flags, kw, key = fixture_case(case)
-    rows = decode_all(FixSimDecoder(fxlib, **kw), pk, flags)
+    rows = decode_all(sim.SimDecoder(arith="fix", **kw), pk, flags)
     f = load_fixdec()
     got = packet_md5(rows)
     bad = np.nonzero((got != f[key + "_packet_md5"]).any(axis=1))[0]
@@ -115,10 +74,10 @@ def test_fixture_differs_from_the_float_build():
     assert (flp != f["fix_pcm_mode4_packet_md5"]).any(axis=1).sum() > 150
 
 
-def test_float_arithmetic_of_the_same_build_matches_golden(fxlib):
+def test_float_arithmetic_of_the_same_build_matches_golden(sim):
     """The same host build with arith = flp reproduces the float build's golden PCM: the mode switch is what differs."""
     pk, flags, kw, _ = fixture_case("mode4")
-    rows = decode_all(FixSimDecoder(fxlib, arith="flp", **kw), pk, flags)
+    rows = decode_all(sim.SimDecoder(arith="flp", **kw), pk, flags)
     assert np.array_equal(np.concatenate(rows), load_golden()["flp_pcm_mode4"])
 
 
@@ -138,11 +97,11 @@ def test_fixture_matches_oracle(ref):
 
 
 @pytest.fixture(scope="module")
-def fix_pairs(ref, sim, fxlib):
+def fix_pairs(ref, sim):
     def make(**cfg):
         """(FIX encoder, FIX decoder) of the reference and (encoder, fixed-point decoder) of the host model."""
         dcfg = {k: v for k, v in cfg.items() if k not in ("rate", "dtx")}
-        return (ref.RefEncoder("fix", **cfg), ref.RefDecoder("fix", **dcfg)), (sim.SimEncoder(**cfg), FixSimDecoder(fxlib, **dcfg))
+        return (ref.RefEncoder("fix", **cfg), ref.RefDecoder("fix", **dcfg)), (sim.SimEncoder(**cfg), sim.SimDecoder(arith="fix", **dcfg))
     return make
 
 
@@ -183,16 +142,3 @@ def test_joint_mode1_matches_reference(fix_pairs):
         lockstep(*fix_pairs(rate=rate, dtx=dtx, use_md_index=mdi, joint_hb=1), clip[:640 * 60].reshape(60, 640),
                  loss_flags(60, 30, seed=9), tag=("joint", rate))
 
-
-def test_fixed_point_decoder_survives_malformed_packets_under_asan(tmp_path):
-    """The fuzzer of tests/hostsim/fixdec.cpp: fixed-point decoders (40 ms, joint mode 1) fed bit flips, garbage, lying
-    lengths, invalid flags and rows shorter than the declared total, under AddressSanitizer and UBSan."""
-    exe = tmp_path / "fuzz_fixdec"
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-w", "-DSB_FIXDEC_FUZZ",
-           FIXDEC_SRC, "-o", str(exe)]
-    try:
-        subprocess.check_call(cmd)
-    except (subprocess.CalledProcessError, FileNotFoundError):
-        pytest.skip("sanitizer build not available")
-    p = subprocess.run([str(exe), "1500", "11"], capture_output=True, text=True, timeout=600)
-    assert p.returncode == 0 and "no memory errors" in p.stdout, p.stdout[-2000:] + p.stderr[-4000:]

@@ -1,7 +1,6 @@
 """Activity reports on the GPU (sb_activity_kernel through the C ABI), at 0 tolerance: every level equals the host function of
-the PCM row it reports on, every flags byte the host model's (tests/hostsim/activity.cpp), and the packet calls' outputs
+the PCM row it reports on, every flags byte the host model's (tests/hostsim), and the packet calls' outputs
 and launch counts are the same with and without activity calls."""
-import ctypes as C
 import hashlib
 import os
 
@@ -10,8 +9,7 @@ import pytest
 
 from solo_b200 import api
 from tests.golden import make_golden_32k as mk
-from tests.parity import sb  # noqa: F401  (fixture)
-from tests.test_activity import Decoder, Encoder, load_lib
+from tests.parity import sb, sim  # noqa: F401  (fixtures)
 from tests.util import GOLDEN, load_clip, load_golden, loss_flags, receive, signal_classes
 
 pytestmark = pytest.mark.gpu
@@ -19,16 +17,11 @@ CAP = 256
 RATES = (6000, 13600, 24000)
 
 
-@pytest.fixture(scope="module")
-def L(tmp_path_factory):
-    return load_lib(str(tmp_path_factory.mktemp("activity") / "libactivity.so"))
+def levels(sim, rows):
+    return np.array([sim.row_level(r) for r in rows], np.uint8)
 
 
-def levels(L, rows):
-    return np.array([L.act_row_level(np.ascontiguousarray(r).ctypes.data, r.size) for r in rows], np.uint8)
-
-
-def test_encoder_batch(sb, L):
+def test_encoder_batch(sb, sim):
     """N = 256 streams of the eight signal classes at 6 / 13.6 / 24 kb/s, 40 packets, through encode + activity (host
     entry points), encode_device + activity_device and encode alone: level = the host function of the input rows, flags =
     the host model's, and payloads / nbytes byte-identical in all three (and equal to the host model's)."""
@@ -39,7 +32,7 @@ def test_encoder_batch(sb, L):
     ea, eb, ed = (sb.EncoderBatch(N) for _ in range(3))
     for e in (ea, eb, ed):
         e.set_control(rate=rate)
-    hm = [Encoder(L, rate=int(rate[s])) for s in range(N)]
+    hm = [sim.SimEncoder(rate=int(rate[s])) for s in range(N)]
     dev = torch.device("cuda", 0)
     d_pcm = torch.zeros((N, 640), dtype=torch.int16, device=dev)
     d_bits = torch.zeros((N, CAP), dtype=torch.uint8, device=dev)
@@ -58,13 +51,12 @@ def test_encoder_batch(sb, L):
         torch.cuda.synchronize()
         assert np.array_equal(ba, bb) and np.array_equal(na, nb_), p
         assert np.array_equal(d_bits.cpu().numpy(), ba) and np.array_equal(d_nb.cpu().numpy(), na), p
-        assert np.array_equal(lv, levels(L, x[p])), p
+        assert np.array_equal(lv, levels(sim, x[p])), p
         assert np.array_equal(d_lv.cpu().numpy(), lv) and np.array_equal(d_fl.cpu().numpy(), fl), p
-        want = [hm[s].encode(x[p, s]) for s in range(N)]
         for s in range(N):
-            b, nb, f = want[s]
+            b, nb, _ = hm[s].encode(x[p, s])
             assert nb == tuple(int(v) for v in na[s]) and bytes(ba[s, :max(nb[0], 0)]) == b[:max(nb[0], 0)], (p, s)
-            assert fl[s] == f, (p, s, int(fl[s]), f)
+            assert fl[s] == hm[s].flags, (p, s, int(fl[s]), hm[s].flags)
         seen.update(int(v) for v in fl)
     assert {0, 3} <= seen
     for e in (ea, eb, ed):
@@ -98,9 +90,9 @@ def dec_cases():
     return out
 
 
-def enc16(L, cfg):
+def enc16(sim, cfg):
     clip = load_clip()
-    e = Encoder(L, rate=13600, **cfg)
+    e = sim.SimEncoder(rate=13600, **cfg)
     k = e.samples
     pk = [e.encode(clip[p * k:(p + 1) * k])[:2] for p in range(60)]
     e.close()
@@ -108,14 +100,14 @@ def enc16(L, cfg):
 
 
 @pytest.mark.parametrize("case", range(8))
-def test_decoder_batches_under_per_stream_loss(sb, L, case):
+def test_decoder_batches_under_per_stream_loss(sb, sim, case):
     """N = 64 streams per batch, each under its own 50 % loss process (row 0: the fixture's loss flags), through decode +
     activity (host) and decode_device + activity_device: level = the host function of the output rows, flags = the host
     model's, PCM = the host model's (row 0: the fixture's md5); chunking (1 or 3) changes nothing."""
     import torch
     cases = dec_cases()
-    cases += [("16k-20ms-flp", 16000, dict(framesize_ms=20), "flp", enc16(L, dict(framesize_ms=20)), None, None),
-              ("16k-joint-fix", 16000, dict(framesize_ms=40, joint_hb=1), "fix", enc16(L, dict(framesize_ms=40, joint_hb=1)), None, None)]
+    cases += [("16k-20ms-flp", 16000, dict(framesize_ms=20), "flp", enc16(sim, dict(framesize_ms=20)), None, None),
+              ("16k-joint-fix", 16000, dict(framesize_ms=40, joint_hb=1), "fix", enc16(sim, dict(framesize_ms=40, joint_hb=1)), None, None)]
     name, sr, cfg, arith, pk, md5key, pinned = cases[case]
     f32 = np.load(os.path.join(GOLDEN, "golden_32k.npz"))
     N, T = 64, len(pk)
@@ -124,7 +116,7 @@ def test_decoder_batches_under_per_stream_loss(sb, L, case):
         flags[0] = pinned
     dh = sb.DecoderBatch(N, arith=arith, samplerate=sr, **cfg)
     dd = sb.DecoderBatch(N, arith=arith, samplerate=sr, **cfg)
-    hm = [Decoder(L, arith=arith, samplerate=sr, **cfg) for _ in range(N)]
+    hm = [sim.SimDecoder(arith=arith, samplerate=sr, **cfg) for _ in range(N)]
     S = dh.samples
     dev = torch.device("cuda", 0)
     d_pcm = torch.zeros((N, S), dtype=torch.int16, device=dev)
@@ -148,10 +140,10 @@ def test_decoder_batches_under_per_stream_loss(sb, L, case):
         dd.activity_device(d_pcm.data_ptr(), d_lv.data_ptr(), d_fl.data_ptr(), st)
         torch.cuda.synchronize()
         assert np.array_equal(d_pcm.cpu().numpy(), pcm) and np.array_equal(d_lv.cpu().numpy(), lv) and np.array_equal(d_fl.cpu().numpy(), fl), (name, p)
-        assert np.array_equal(lv, levels(L, pcm)), (name, p)
+        assert np.array_equal(lv, levels(sim, pcm)), (name, p)
         for s in range(N):
-            y, r, hf = hm[s].decode(*rx[s])
-            assert r == 0 and np.array_equal(y, pcm[s]) and hf == fl[s], (name, p, s, int(fl[s]), hf)
+            y, r = hm[s].decode(*rx[s])
+            assert r == 0 and np.array_equal(y, pcm[s]) and hm[s].flags == fl[s], (name, p, s, int(fl[s]), hm[s].flags)
         if md5key:
             assert hashlib.md5(pcm[0].tobytes()).digest() == bytes(f32[md5key][p]), (name, p)
         conc = 0xC if cfg["framesize_ms"] == 40 else 0x4
@@ -162,7 +154,7 @@ def test_decoder_batches_under_per_stream_loss(sb, L, case):
         h.close()
 
 
-def test_sample_of_a_65536_stream_batch(sb, L):
+def test_sample_of_a_65536_stream_batch(sb, sim):
     """One 65 536-stream 16 kHz decoder batch under per-row loss, through decode_device + activity_device: a fixed sample
     of 1 024 rows has the host model's flags and the host function's level of its output rows, for 12 packets."""
     import torch
@@ -171,7 +163,7 @@ def test_sample_of_a_65536_stream_batch(sb, L):
     rows = np.unique(np.concatenate([[0, N - 1], np.random.Generator(np.random.PCG64(66)).choice(N, 1022, replace=False)]))
     lost = np.random.Generator(np.random.PCG64(67)).random((T, N)) < 0.5
     db = sb.DecoderBatch(N)
-    hm = [Decoder(L) for _ in rows]
+    hm = [sim.SimDecoder() for _ in rows]
     dev = torch.device("cuda", 0)
     d_pcm = torch.zeros((N, 640), dtype=torch.int16, device=dev)
     d_lv = torch.zeros(N, dtype=torch.uint8, device=dev)
@@ -189,10 +181,10 @@ def test_sample_of_a_65536_stream_batch(sb, L):
         db.activity_device(d_pcm.data_ptr(), d_lv.data_ptr(), d_fl.data_ptr(), st)
         torch.cuda.synchronize()
         pcm, lv, fl = d_pcm[idx].cpu().numpy(), d_lv[idx].cpu().numpy(), d_fl[idx].cpu().numpy()
-        assert np.array_equal(lv, levels(L, pcm)), p
+        assert np.array_equal(lv, levels(sim, pcm)), p
         for i, s in enumerate(rows):
-            y, r, hf = hm[i].decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 1 if lost[p, s] else 4)
-            assert r == 0 and hf == fl[i] and np.array_equal(y, pcm[i]), (p, int(s))
+            y, r = hm[i].decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 1 if lost[p, s] else 4)
+            assert r == 0 and hm[i].flags == fl[i] and np.array_equal(y, pcm[i]), (p, int(s))
     db.close()
     for h in hm:
         h.close()

@@ -1,6 +1,8 @@
 """Shared helpers of the test-suite (input synthesis, the reference driver's loss process, what the receiver decodes)."""
 import os
+import re
 import struct
+import subprocess
 
 import numpy as np
 
@@ -185,3 +187,19 @@ def loss_with_bursts(T, n_rows, seed=3):
         flags[s, a:a + n] = 1
     flags[::5] = 4
     return flags
+
+
+def fuzz_decoder(iters, seed, corpus32=None):
+    """Run tests/hostsim/fuzz_dec.cpp under AddressSanitizer and UBSan: the 16 kHz modes, or with corpus32 (a .bit file of
+    32 kHz packets) the 32 kHz modes.  Checks that it ran clean; returns {mode: (decoded, rejected)}."""
+    import pytest
+    from tests.hostsim import build_hostsim
+    try:
+        exe = build_hostsim.build_fuzzer()
+    except (subprocess.CalledProcessError, FileNotFoundError):
+        pytest.skip("sanitizer build not available")
+    p = subprocess.run([exe, str(iters), str(seed)] + ([str(corpus32)] if corpus32 else []), capture_output=True, text=True,
+                       timeout=900)
+    assert p.returncode == 0 and "no memory errors" in p.stdout, p.stdout[-2000:] + p.stderr[-4000:]
+    print(p.stdout)
+    return {m: (int(a), int(b)) for m, a, b in re.findall(r"^(.+): (\d+) decoded, (\d+) rejected$", p.stdout, re.M)}
