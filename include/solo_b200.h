@@ -199,6 +199,22 @@ int solo_b200_mix_host(const int16_t *in, int16_t *out, int spp, int n, const ui
 int solo_b200_mix_device(const int16_t *d_in, int16_t *d_out, int spp, int n, const uint8_t *d_level,
                          const uint8_t *d_flags, const int32_t *d_room_start, const int32_t *d_members, int n_rooms,
                          int k, int32_t *d_talkers, void *cuda_stream);
+/* Downlink contributor lists: for every member i of room r (rooms, n and k as for solo_b200_mix_*, talkers int32 [R][k]
+   as the mix writes them, level uint8 [n] as the activity report writes it):
+     csrc int32 [n][k]      : the entries j of talkers[r] with 0 <= j < n and j != i, in the mixer's order (loudest first),
+                              padded with -1: the CSRC list of i's downlink packet (as stream indices);
+     csrc_level uint8 [n][k]: level[j] & 0x7f beside each entry, 127 in the padding: its RFC 6465 levels.
+   Rows of streams in no room are all -1 and 127.
+     mix_contributors_host   : host arrays, the checks of mix_host (-1, nothing written, for a bad n or k, bad offsets, a
+                               member outside [0, n) or a stream listed twice); returns when the rows are written.
+     mix_contributors_device : device arrays; only enqueues two memsets and, for n_rooms > 0, one kernel launch (a thread
+                               per member) on `cuda_stream`.  It checks the scalars, and clamps as mix_device does: a member
+                               outside [0, n) is skipped, a stream listed twice gives an unspecified row but no fault. */
+int solo_b200_mix_contributors_host(const int32_t *room_start, const int32_t *members, int n_rooms, int k,
+                                    const int32_t *talkers, const uint8_t *level, int n, int32_t *csrc, uint8_t *csrc_level);
+int solo_b200_mix_contributors_device(const int32_t *d_room_start, const int32_t *d_members, int n_rooms, int k,
+                                      const int32_t *d_talkers, const uint8_t *d_level, int n, int32_t *d_csrc,
+                                      uint8_t *d_csrc_level, void *cuda_stream);
 
 /* Receive queue: per stream, holds the two descriptions of each packet (solo_b200_split_packet) as they arrive early, out
    of order or twice, pairs them and hands the decoder one row per tick, for N streams on the device.  It is independent
@@ -255,6 +271,52 @@ int solo_b200_rx_pull_device(solo_b200_rx *q, const uint32_t *d_play, uint8_t *d
                              int32_t *d_lostflag, void *cuda_stream);
 int solo_b200_rx_reset(solo_b200_rx *q, const int32_t *streams, const uint32_t *start, int n, void *cuda_stream);
 int solo_b200_rx_stats(solo_b200_rx *q, uint32_t *counters, uint64_t *bad_stream, void *cuda_stream);
+
+/* Send queue: turns a wave of the encoder's rows into numbered datagrams, two per row (solo_b200_split_packet), packed
+   back to back in one buffer in the receive queue's arrival format, for N streams on the device.  It is independent of
+   the codec batches: a pack takes the rows of any encoder batch with the same N.
+   Per stream it keeps:
+     next     : the packet index of the stream's next row (uint32), 0 at create; it wraps at 2^32;
+     counters : 4 uint32, in this order: sent (rows that produced datagrams), octets (payload bytes sent, mod 2^32: the RTCP
+                SR sender's octet count), dtx (rows with nbytes[0] <= 0), bad (rows solo_b200_split_packet refuses, i.e.
+                nbytes[1] < 4 or nbytes[1] > nbytes[0], and rows with nbytes[0] > cap).
+   pack: takes the encoder's output as it is, bits [N][cap] and nbytes [N][2].  For each stream s, in stream order:
+     - the row's index is next[s]; then next[s] is incremented, for every stream on every call: the index follows the RTP
+       clock, so it advances through DTX and bad rows too;
+     - a DTX or bad row emits nothing, only its counter changes;
+     - otherwise (n0 = nbytes[s][0], n1 = nbytes[s][1]) the row emits description 1 = bits[s][0, n0 - n1) and description
+       2 = bits[s][n0 - n1, n0), what solo_b200_split_packet returns, and counts sent and n0 octets.  A description of 0
+       bytes is not emitted (the receive queue would count it malformed).  The high-band tail is 8 bytes for 40 ms packets
+       and 4 for 20 ms packets and joint mode 1; the rule does not depend on it.
+     Datagram a of the call: stream[a] int32, index[a] uint32, desc[a] uint8 (1 or 2), off[a] int32, len[a] int32 -- the
+     types solo_b200_rx_insert_* takes -- and its len[a] bytes at payload + off[a].  Datagrams are in the order stream 0
+     description 1, stream 0 description 2, stream 1 description 1, ...; off[a] is the sum of the lengths before a, so
+     the payloads lie back to back from payload[0].  Each entry array has room for 2N entries; the call writes the
+     datagram count (int32) and the byte total (int64).  The result depends only on the inputs and the queue's state.
+   reset: for a participant joining or rejoining a stream: sets next = start for the listed streams and zeroes their
+     counters.  Host arrays; -1 (nothing done) for a stream outside [0, N) or listed twice.
+   stats: counters uint32 [N][4].
+   Entry points:
+     pack_host   : host arrays; runs on the queue's own CUDA stream; returns the datagram count (>= 0) and writes the byte
+                   total to *total, once the arrays are filled (only the first count entries and total bytes are written).
+     pack_device : device arrays; only enqueues work on `cuda_stream`.  It checks the scalars (-1 for cap not a multiple
+                   of 16 or below 16, N * cap above 2^31 - 1, payload_cap below N * cap -- the worst case, so the payload
+                   always fits -- and d_bits or d_payload not 16-byte aligned), not the arrays' contents, and never reads or
+                   writes out of bounds whatever nbytes holds.  The caller copies back the byte total, then that many bytes.
+     reset, stats : host arrays, ordered on `cuda_stream`; return after synchronising it.
+   Launches: a pack is exactly three kernels; a reset one. */
+typedef struct solo_b200_tx solo_b200_tx;
+/* NULL (solo_b200_last_error() set) for a bad n_streams or device. */
+solo_b200_tx *solo_b200_tx_create(int n_streams, int device);
+void solo_b200_tx_destroy(solo_b200_tx *q);
+int solo_b200_tx_pack_host(solo_b200_tx *q, const uint8_t *bits, int cap, const int16_t *nbytes, uint8_t *payload,
+                           int64_t payload_cap, int32_t *stream, uint32_t *index, uint8_t *desc, int32_t *off, int32_t *len,
+                           int64_t *total);
+int solo_b200_tx_pack_device(solo_b200_tx *q, const uint8_t *d_bits, int cap, const int16_t *d_nbytes, uint8_t *d_payload,
+                             int64_t payload_cap, int32_t *d_stream, uint32_t *d_index, uint8_t *d_desc, int32_t *d_off,
+                             int32_t *d_len, int32_t *d_count, int64_t *d_total, void *cuda_stream);
+int solo_b200_tx_reset(solo_b200_tx *q, const int32_t *streams, const uint32_t *start, int n, void *cuda_stream);
+int solo_b200_tx_stats(solo_b200_tx *q, uint32_t *counters, void *cuda_stream);
 
 /* Multi-GPU ingest through peer memory:after this call kernels launched on `device` may read and write buffers that live in
    `peer_device`'s memory (same process, or another process's allocation mapped with CUDA IPC).  The *_device entry points

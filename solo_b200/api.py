@@ -104,6 +104,15 @@ def lib():
         L.solo_b200_rx_pull_device.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
         L.solo_b200_rx_reset.argtypes = [vp, vp, vp, C.c_int, vp]
         L.solo_b200_rx_stats.argtypes = [vp, vp, vp, vp]
+        L.solo_b200_tx_create.restype = vp
+        L.solo_b200_tx_create.argtypes = [C.c_int, C.c_int]
+        L.solo_b200_tx_destroy.argtypes = [vp]
+        L.solo_b200_tx_pack_host.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int64] + [vp] * 6
+        L.solo_b200_tx_pack_device.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int64] + [vp] * 8
+        L.solo_b200_tx_reset.argtypes = [vp, vp, vp, C.c_int, vp]
+        L.solo_b200_tx_stats.argtypes = [vp, vp, vp]
+        L.solo_b200_mix_contributors_host.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
+        L.solo_b200_mix_contributors_device.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -501,6 +510,37 @@ def mix(pcm, level, flags, rooms, k, out=None):
     return out, talkers
 
 
+def mix_contributors(rooms, talkers, level, n):
+    """Every downlink's CSRC list and RFC 6465 levels: rooms = a list of index arrays, talkers int32 [R, k] (what mix
+    returns), level uint8 [n] -> (csrc int32 [n, k], csrc_level uint8 [n, k]).  Member i of room r lists r's talkers
+    except i, loudest first, padded with -1 / 127; rows of streams in no room are all -1 / 127 (see
+    solo_b200_mix_contributors_host).  Raises SoloError for a bad argument, a member outside [0, n) or a stream listed
+    twice."""
+    talkers = np.ascontiguousarray(talkers, np.int32)
+    if talkers.ndim != 2 or talkers.shape[0] != len(rooms):
+        raise SoloError("mix_contributors: talkers must be int32 [%d, k]" % len(rooms))
+    level = np.ascontiguousarray(level, np.uint8)
+    if level.shape != (int(n),):
+        raise SoloError("mix_contributors: level must be uint8 [%d]" % int(n))
+    k = talkers.shape[1]
+    room_start, members = rooms_csr(rooms)
+    csrc = np.empty((int(n), k), np.int32)
+    csrc_level = np.empty((int(n), k), np.uint8)
+    r = lib().solo_b200_mix_contributors_host(room_start.ctypes.data, members.ctypes.data, len(rooms), k, talkers.ctypes.data,
+                                              level.ctypes.data, int(n), csrc.ctypes.data, csrc_level.ctypes.data)
+    if r:
+        raise SoloError("mix_contributors failed (%d): %s" % (r, _err()))
+    return csrc, csrc_level
+
+
+def mix_contributors_device(d_room_start, d_members, n_rooms, k, d_talkers, d_level, n, d_csrc, d_csrc_level, stream=0):
+    """The same on device arrays (addresses): enqueued on `stream`; contents are not checked."""
+    r = lib().solo_b200_mix_contributors_device(d_room_start, d_members, int(n_rooms), int(k), d_talkers, d_level, int(n),
+                                                d_csrc, d_csrc_level, stream)
+    if r:
+        raise SoloError("mix_contributors_device failed (%d): %s" % (r, _err()))
+
+
 def mix_device(d_in, d_out, spp, n, d_level, d_flags, d_room_start, d_members, n_rooms, k, d_talkers, stream=0):
     """The same on device arrays (addresses): enqueued on `stream`; contents are not checked (see solo_b200_mix_device)."""
     r = lib().solo_b200_mix_device(d_in, d_out, int(spp), int(n), d_level, d_flags, d_room_start, d_members, int(n_rooms),
@@ -591,6 +631,73 @@ class RxQueue:
     def close(self):
         if getattr(self, "h", None):
             lib().solo_b200_rx_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+
+# ---- send queue (include/solo_b200.h, solo_b200_tx_*) -----------------------------------------------------------------
+TX_COUNTERS = ("sent", "octets", "dtx", "bad")
+
+
+class TxQueue:
+    """Send queue of N streams on one GPU: turns each wave of encoded rows into numbered datagrams, two per row, packed
+    back to back in RxQueue's arrival format (see solo_b200_tx_* in include/solo_b200.h)."""
+
+    def __init__(self, n, device=0):
+        self.n = int(n)
+        self.h = lib().solo_b200_tx_create(self.n, int(device))
+        if not self.h:
+            raise SoloError("solo_b200_tx_create failed: " + _err())
+
+    def pack(self, bits, nbytes):
+        """bits uint8 [N, cap], nbytes int16 [N, 2] (an encoder wave) -> (payload uint8 [total], stream int32, index uint32,
+        desc uint8, off int32, len int32 [count])."""
+        bits = np.ascontiguousarray(bits, np.uint8)
+        nbytes = np.ascontiguousarray(nbytes, np.int16)
+        if bits.ndim != 2 or bits.shape[0] != self.n or nbytes.shape != (self.n, 2):
+            raise SoloError("TxQueue.pack: bits must be [%d, cap] and nbytes [%d, 2]" % (self.n, self.n))
+        cap = bits.shape[1]
+        payload = np.empty(self.n * cap, np.uint8)
+        e = 2 * self.n
+        stream, index, desc = np.empty(e, np.int32), np.empty(e, np.uint32), np.empty(e, np.uint8)
+        off, lens = np.empty(e, np.int32), np.empty(e, np.int32)
+        total = C.c_int64()
+        c = lib().solo_b200_tx_pack_host(self.h, bits.ctypes.data, cap, nbytes.ctypes.data, payload.ctypes.data, payload.size,
+                                         stream.ctypes.data, index.ctypes.data, desc.ctypes.data, off.ctypes.data,
+                                         lens.ctypes.data, C.byref(total))
+        if c < 0:
+            raise SoloError("tx_pack_host failed (%d): %s" % (c, _err()))
+        return payload[:total.value], stream[:c], index[:c], desc[:c], off[:c], lens[:c]
+
+    def pack_device(self, d_bits, cap, d_nbytes, d_payload, payload_cap, d_stream, d_index, d_desc, d_off, d_len, d_count,
+                    d_total, stream=0):
+        """pack on device arrays (addresses), enqueued on `stream`: three kernel launches.  d_count int32 [1] and d_total
+        int64 [1] receive the datagram count and byte total."""
+        r = lib().solo_b200_tx_pack_device(self.h, d_bits, int(cap), d_nbytes, d_payload, int(payload_cap), d_stream, d_index,
+                                           d_desc, d_off, d_len, d_count, d_total, stream)
+        if r:
+            raise SoloError("tx_pack_device failed (%d): %s" % (r, _err()))
+
+    def reset(self, streams, start, stream=0):
+        """Give the listed streams' next rows index start[i] and zero their counters."""
+        streams = np.ascontiguousarray(streams, np.int32).ravel()
+        start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
+        r = lib().solo_b200_tx_reset(self.h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
+        if r:
+            raise SoloError("tx_reset failed (%d): %s" % (r, _err()))
+
+    def stats(self, stream=0):
+        """counters uint32 [N, 4] in the order of TX_COUNTERS."""
+        cnt = np.zeros((self.n, 4), np.uint32)
+        r = lib().solo_b200_tx_stats(self.h, cnt.ctypes.data, stream)
+        if r:
+            raise SoloError("tx_stats failed (%d): %s" % (r, _err()))
+        return cnt
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().solo_b200_tx_destroy(self.h)
             self.h = None
 
     __del__ = close

@@ -21,6 +21,9 @@
 // The receive queue (solo_b200_rx_*, sb_rx.cuh) pairs, reorders and screens the two descriptions of each stream's packets:
 // an insert is sb_rx_elect_kernel, sb_rx_classify_kernel and sb_rx_commit_kernel over the arrivals, a pull is
 // sb_rx_pull_kernel (warp per stream), which writes the decoder's input rows.
+// The send queue (solo_b200_tx_*, sb_tx.cuh) turns the encoder's rows into numbered datagrams packed back to back: a pack
+// is sb_tx_sizes_kernel (thread per stream), sb_tx_scan_kernel (one block) and sb_tx_pack_kernel (warp per stream).
+// sb_mix_contributors_kernel (thread per member) writes each downlink's CSRC list and RFC 6465 levels.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -38,6 +41,7 @@
 #include "sb_mix.cuh"
 #include "sb_nsq_warp.cuh"
 #include "sb_rx.cuh"
+#include "sb_tx.cuh"
 
 using namespace sb;
 
@@ -598,6 +602,159 @@ __global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_reset_kernel(RxDev q, con
     q.last[s] = start[i] - 1u;
     for (int k = 0; k < RX_NCOUNT; k++) q.cnt[(size_t)s * RX_NCOUNT + k] = 0;
     for (int j = 0; j < 2 * q.depth; j++) q.len[(size_t)s * 2 * q.depth + j] = 0;
+}
+
+// ---- send queue (sb_tx.cuh) ----------------------------------------------------------------------------------------------
+// The queue's device arrays.  The scan words (bytes << 32 | datagrams) are scratch of the running pack: the sizes pass
+// writes each stream's prefix within its block and each block's total, the scan pass turns the totals into the blocks'
+// prefixes, the pack pass adds the two.
+struct TxDev {
+    int n;
+    u32* next;                  // [n] index of the stream's next row
+    u32* cnt;                   // [n][TX_NCOUNT]
+    unsigned long long* pre;    // [n] scan word of the streams before s in its block
+    unsigned long long* blk;    // [ceil(n / SB_TX_BLOCK)] block totals, then their exclusive prefix
+};
+struct TxOut {
+    u8* payload; i32* stream; u32* index; u8* desc; i32* off; i32* len; i32* count; i64* total;
+};
+
+// inclusive scan of v over the warp
+__device__ __forceinline__ unsigned long long tx_warp_scan(unsigned long long v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += y;
+    }
+    return v;
+}
+
+// pack, pass 1 (thread per stream): each row's datagrams and bytes, their exclusive prefix within the block (warp scans
+// and the warps' totals in shared memory) and the block's total
+__global__ void __launch_bounds__(SB_TX_BLOCK) sb_tx_sizes_kernel(TxDev q, const i16* __restrict__ nbytes, int cap) {
+    __shared__ unsigned long long warp_total[SB_TX_BLOCK / 32];
+    const int s = blockIdx.x * SB_TX_BLOCK + threadIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int l1 = 0, l2 = 0;
+    if (s < q.n) tx_row(nbytes[2 * s], nbytes[2 * s + 1], cap, &l1, &l2);
+    const unsigned long long x = tx_scan_word(l1, l2), v = tx_warp_scan(x, lane);
+    if (lane == 31) warp_total[w] = v;
+    __syncthreads();
+    unsigned long long base = 0, tot = 0;
+#pragma unroll
+    for (int i = 0; i < SB_TX_BLOCK / 32; i++) {
+        const unsigned long long t = warp_total[i];
+        base += i < w ? t : 0ull;
+        tot += t;
+    }
+    if (s < q.n) q.pre[s] = base + v - x;
+    if (threadIdx.x == 0) q.blk[blockIdx.x] = tot;
+}
+
+// pack, pass 2 (one block): the exclusive prefix of the block totals, SB_TX_SCAN_THREADS at a time in order, and the
+// call's datagram count and byte total
+#define SB_TX_SCAN_THREADS 1024
+__global__ void __launch_bounds__(SB_TX_SCAN_THREADS) sb_tx_scan_kernel(TxDev q, int nblk, i32* __restrict__ count, i64* __restrict__ total) {
+    __shared__ unsigned long long warp_total[SB_TX_SCAN_THREADS / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    unsigned long long carry = 0;
+    for (int b0 = 0; b0 < nblk; b0 += SB_TX_SCAN_THREADS) {
+        const int b = b0 + threadIdx.x;
+        const unsigned long long x = b < nblk ? q.blk[b] : 0ull, v = tx_warp_scan(x, lane);
+        if (lane == 31) warp_total[w] = v;
+        __syncthreads();
+        unsigned long long base = carry, tot = 0;
+        for (int i = 0; i < SB_TX_SCAN_THREADS / 32; i++) {
+            const unsigned long long t = warp_total[i];
+            base += i < w ? t : 0ull;
+            tot += t;
+        }
+        if (b < nblk) q.blk[b] = base + v - x;
+        carry += tot;
+        __syncthreads();                          // warp_total is rewritten by the next round
+    }
+    if (threadIdx.x == 0) {
+        *count = tx_word_datagrams(carry);
+        *total = tx_word_bytes(carry);
+    }
+}
+
+// pack, pass 3 (warp per stream): the row's index and counters, its datagram entries, and its n0 bytes at payload offset
+// b0.  The 16-byte words of payload that lie inside [b0, b0 + n0) get one 16-byte store each, built from two aligned
+// 16-byte loads of the row (aligned: d_bits is, and cap is a multiple of 16) funnel-shifted by the stream's constant
+// misalignment.  The partial words at both ends are shared with the neighbouring streams' datagrams: byte stores only.
+#define SB_TX_PACK_WARPS 8
+__global__ void __launch_bounds__(SB_TX_PACK_WARPS * 32) sb_tx_pack_kernel(TxDev q, const u8* __restrict__ bits, int cap,
+                                                                            const i16* __restrict__ nbytes, TxOut o) {
+    const int s = blockIdx.x * SB_TX_PACK_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (s >= q.n) return;                         // whole warps
+    int l1, l2;
+    const int cls = tx_row(nbytes[2 * s], nbytes[2 * s + 1], cap, &l1, &l2);
+    const u32 idx = q.next[s];
+    if (lane == 0) {
+        q.next[s] = idx + 1u;
+        tx_count(q.cnt + (size_t)s * TX_NCOUNT, cls, l1, l2);
+    }
+    if (cls != TX_SENT) return;
+    const unsigned long long at = q.blk[s / SB_TX_BLOCK] + q.pre[s];
+    const i32 k0 = tx_word_datagrams(at);
+    const i64 b0 = tx_word_bytes(at), end = b0 + l1 + l2;
+    if (lane < 2) {                               // lane d - 1: the entry of description d, when it is not empty
+        const int len = lane ? l2 : l1;
+        if (len > 0) {
+            const i32 k = k0 + (lane && l1 > 0);
+            o.stream[k] = s;
+            o.index[k] = idx;
+            o.desc[k] = (u8)(lane + 1);
+            o.off[k] = (i32)(b0 + (lane ? l1 : 0));
+            o.len[k] = len;
+        }
+    }
+    const u8* row = bits + (size_t)s * cap;       // payload byte x is row byte x - b0
+    const i64 h_end = end < ((b0 + 15) & ~15ll) ? end : ((b0 + 15) & ~15ll);
+    const i64 t_beg = (end & ~15ll) > h_end ? (end & ~15ll) : h_end;
+    {
+        const i64 x = lane < 16 ? b0 + lane : t_beg + (lane - 16);
+        if (x < (lane < 16 ? h_end : end)) o.payload[x] = row[x - b0];
+    }
+    const int mis = (int)((h_end - b0) & 15);     // the row offset of every full payload word, mod 16
+    const int ws = mis >> 2, bs = (mis & 3) * 8;
+    for (i64 x = h_end + 16 * lane; x < t_beg; x += 16 * 32) {
+        const uint4* src = reinterpret_cast<const uint4*>(row + (x - b0 - mis));
+        const uint4 a = src[0], b = mis ? src[1] : make_uint4(0, 0, 0, 0);
+        const u32 v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        u32 r[5], w[4];
+#pragma unroll
+        for (int k = 0; k < 5; k++) r[k] = ws == 0 ? v[k] : ws == 1 ? v[k + 1] : ws == 2 ? v[k + 2] : v[k + 3];
+#pragma unroll
+        for (int k = 0; k < 4; k++) w[k] = __funnelshift_r(r[k], r[k + 1], bs);
+        *reinterpret_cast<uint4*>(o.payload + x) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+}
+
+// reset (thread per listed stream; the host has checked the list): next = start, counters zero
+__global__ void __launch_bounds__(SB_TX_BLOCK) sb_tx_reset_kernel(TxDev q, const i32* __restrict__ streams, const u32* __restrict__ start, int n) {
+    const int i = blockIdx.x * SB_TX_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    const i32 s = streams[i];
+    q.next[s] = start[i];
+    for (int k = 0; k < TX_NCOUNT; k++) q.cnt[(size_t)s * TX_NCOUNT + k] = 0;
+}
+
+// ---- downlink contributor lists (sb_tx.cuh), thread per member --------------------------------------------------------------
+// Member position m (grid-stride over M = room_start[R]) finds its room by binary search and writes its stream's row.
+// Rows of streams in no room were set to -1 / 127 by the caller's memsets; members outside [0, n) are skipped.
+#define SB_CONTRIB_THREADS 256
+__global__ void __launch_bounds__(SB_CONTRIB_THREADS) sb_mix_contributors_kernel(const i32* __restrict__ room_start, const i32* __restrict__ members,
+                                                                                  int R, int k, const i32* __restrict__ talkers,
+                                                                                  const u8* __restrict__ level, int n, i32* __restrict__ csrc,
+                                                                                  u8* __restrict__ csrc_level) {
+    const i32 M = room_start[R];
+    for (i32 m = blockIdx.x * SB_CONTRIB_THREADS + threadIdx.x; m < M; m += gridDim.x * SB_CONTRIB_THREADS) {
+        const i32 i = members[m];
+        if ((u32)i >= (u32)n) continue;
+        const int r = tx_room_of(room_start, R, m);
+        tx_contributors(i, talkers + (size_t)r * k, k, level, n, csrc + (size_t)i * k, csrc_level + (size_t)i * k);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1484,6 +1641,235 @@ int solo_b200_rx_stats(solo_b200_rx* q, uint32_t* counters, uint64_t* bad_stream
     if (bad_stream) CK(cudaMemcpyAsync(bad_stream, q->q.bad, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return 0;
+}
+
+// ---- send queue (sb_tx.cuh) ----------------------------------------------------------------------------------------------
+struct solo_b200_tx {
+    int device;
+    cudaStream_t st;            // the _host form's stream
+    TxDev q;
+    ~solo_b200_tx() {
+        if (st) cudaStreamDestroy(st);
+        cudaFree(q.next); cudaFree(q.cnt); cudaFree(q.pre); cudaFree(q.blk);
+    }
+};
+static int tx_blocks(int n) { return (n + SB_TX_BLOCK - 1) / SB_TX_BLOCK; }
+
+solo_b200_tx* solo_b200_tx_create(int n_streams, int device) {
+    if (n_streams <= 0) { snprintf(g_err, sizeof g_err, "tx_create: bad argument (n %d)", n_streams); return nullptr; }
+    if (require_gpu(device)) return nullptr;
+    solo_b200_tx* t = new solo_b200_tx();
+    t->device = device;
+    TxDev& q = t->q;
+    q.n = n_streams;
+    const size_t n = (size_t)n_streams;
+    bool ok = cudaStreamCreateWithFlags(&t->st, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaMalloc(&q.next, 4 * n) == cudaSuccess && cudaMalloc(&q.cnt, 4 * TX_NCOUNT * n) == cudaSuccess &&
+              cudaMalloc(&q.pre, 8 * n) == cudaSuccess && cudaMalloc(&q.blk, 8 * (size_t)tx_blocks(n_streams)) == cudaSuccess;
+    ok = ok && cudaMemsetAsync(q.next, 0, 4 * n, t->st) == cudaSuccess &&
+         cudaMemsetAsync(q.cnt, 0, 4 * TX_NCOUNT * n, t->st) == cudaSuccess && cudaStreamSynchronize(t->st) == cudaSuccess;
+    if (!ok) {
+        snprintf(g_err, sizeof g_err, "tx_create: %s", cudaGetErrorString(cudaGetLastError()));
+        delete t;
+        return nullptr;
+    }
+    return t;
+}
+
+void solo_b200_tx_destroy(solo_b200_tx* q) {
+    if (!q) return;
+    cudaSetDevice(q->device);
+    delete q;
+}
+
+// the scalars of a pack: cap a multiple of 16 (aligned rows), every offset within int32, room for the worst case
+static int tx_pack_args_ok(solo_b200_tx* q, const void* bits, int cap, const void* nbytes, const TxOut& o, int64_t payload_cap) {
+    if (!q || !bits || !nbytes || !o.payload || !o.stream || !o.index || !o.desc || !o.off || !o.len || !o.count || !o.total) {
+        snprintf(g_err, sizeof g_err, "tx_pack: bad argument");
+        return 0;
+    }
+    const long long worst = (long long)q->q.n * cap;
+    if (cap < 16 || cap % 16 || worst > 0x7FFFFFFFll) {
+        snprintf(g_err, sizeof g_err, "tx_pack: cap %d must be a multiple of 16 with n * cap <= 2^31 - 1 (n %d)", cap, q->q.n);
+        return 0;
+    }
+    if (payload_cap < worst) {
+        snprintf(g_err, sizeof g_err, "tx_pack: payload_cap %lld is below n * cap = %lld", (long long)payload_cap, worst);
+        return 0;
+    }
+    return 1;
+}
+static int tx_pack_launch(solo_b200_tx* t, const u8* bits, int cap, const i16* nbytes, const TxOut& o, cudaStream_t st) {
+    const int nblk = tx_blocks(t->q.n);
+    sb_tx_sizes_kernel<<<nblk, SB_TX_BLOCK, 0, st>>>(t->q, nbytes, cap);
+    count_launch();
+    CK(cudaGetLastError());
+    sb_tx_scan_kernel<<<1, SB_TX_SCAN_THREADS, 0, st>>>(t->q, nblk, o.count, o.total);
+    count_launch();
+    CK(cudaGetLastError());
+    sb_tx_pack_kernel<<<(t->q.n + SB_TX_PACK_WARPS - 1) / SB_TX_PACK_WARPS, SB_TX_PACK_WARPS * 32, 0, st>>>(t->q, bits, cap, nbytes, o);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int solo_b200_tx_pack_device(solo_b200_tx* q, const uint8_t* d_bits, int cap, const int16_t* d_nbytes, uint8_t* d_payload,
+                             int64_t payload_cap, int32_t* d_stream, uint32_t* d_index, uint8_t* d_desc, int32_t* d_off,
+                             int32_t* d_len, int32_t* d_count, int64_t* d_total, void* cuda_stream) {
+    const TxOut o = {d_payload, d_stream, d_index, d_desc, d_off, d_len, d_count, d_total};
+    if (!tx_pack_args_ok(q, d_bits, cap, d_nbytes, o, payload_cap)) return -1;
+    if (((uintptr_t)d_bits | (uintptr_t)d_payload) & 15) {
+        snprintf(g_err, sizeof g_err, "tx_pack_device: d_bits and d_payload must be 16-byte aligned");
+        return -1;
+    }
+    CK(cudaSetDevice(q->device));
+    return tx_pack_launch(q, d_bits, cap, d_nbytes, o, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_tx_pack_host(solo_b200_tx* q, const uint8_t* bits, int cap, const int16_t* nbytes, uint8_t* payload,
+                           int64_t payload_cap, int32_t* stream, uint32_t* index, uint8_t* desc, int32_t* off, int32_t* len,
+                           int64_t* total) {
+    i32 count = 0;              // host copies of the call's datagram count and byte total
+    i64 tot = 0;
+    const TxOut h = {payload, stream, index, desc, off, len, &count, total};
+    if (!tx_pack_args_ok(q, bits, cap, nbytes, h, payload_cap)) return -1;
+    CK(cudaSetDevice(q->device));
+    const size_t n = (size_t)q->q.n, rows = n * (size_t)cap, e = 2 * n;
+    cudaStream_t st = q->st;
+    // bits [n][cap] | payload [n * cap] | stream, index, off, len [2n] each | count, total | nbytes [n][2] | desc [2n]
+    const size_t o_pay = rows, o_ent = 2 * rows, o_cnt = o_ent + 16 * e, o_nb = o_cnt + 16, o_desc = o_nb + 4 * n;
+    u8* d = nullptr;
+    int r = 0;
+    auto ok = [&](cudaError_t err, const char* what) { if (!r && err != cudaSuccess) r = fail(what, err); return !r; };
+    if (ok(cudaMallocAsync(&d, o_desc + e, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d, bits, rows, cudaMemcpyHostToDevice, st), "copy bits") &&
+        ok(cudaMemcpyAsync(d + o_nb, nbytes, 4 * n, cudaMemcpyHostToDevice, st), "copy nbytes")) {
+        const TxOut o = {d + o_pay, (i32*)(d + o_ent), (u32*)(d + o_ent + 4 * e), d + o_desc, (i32*)(d + o_ent + 8 * e),
+                         (i32*)(d + o_ent + 12 * e), (i32*)(d + o_cnt), (i64*)(d + o_cnt + 8)};
+        if (!(r = tx_pack_launch(q, d, cap, (const i16*)(d + o_nb), o, st)) &&
+            ok(cudaMemcpyAsync(&count, o.count, 4, cudaMemcpyDeviceToHost, st), "copy count") &&
+            ok(cudaMemcpyAsync(&tot, o.total, 8, cudaMemcpyDeviceToHost, st), "copy total") &&
+            ok(cudaStreamSynchronize(st), "tx_pack")) {
+            const size_t c = (size_t)count;
+            (tot == 0 || ok(cudaMemcpyAsync(payload, o.payload, (size_t)tot, cudaMemcpyDeviceToHost, st), "copy payload")) &&
+                ok(cudaMemcpyAsync(stream, o.stream, 4 * c, cudaMemcpyDeviceToHost, st), "copy stream") &&
+                ok(cudaMemcpyAsync(index, o.index, 4 * c, cudaMemcpyDeviceToHost, st), "copy index") &&
+                ok(cudaMemcpyAsync(desc, o.desc, c, cudaMemcpyDeviceToHost, st), "copy desc") &&
+                ok(cudaMemcpyAsync(off, o.off, 4 * c, cudaMemcpyDeviceToHost, st), "copy off") &&
+                ok(cudaMemcpyAsync(len, o.len, 4 * c, cudaMemcpyDeviceToHost, st), "copy len");
+        }
+    }
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "tx_pack");
+    if (r) return r;
+    *total = tot;
+    return count;
+}
+
+int solo_b200_tx_reset(solo_b200_tx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
+    if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "tx_reset: bad argument"); return -1; }
+    {
+        std::vector<u8> seen((size_t)q->q.n, 0);
+        for (int i = 0; i < n; i++) {
+            if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "tx_reset: stream %d outside [0, %d)", streams[i], q->q.n); return -1; }
+            if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "tx_reset: stream %d is listed twice", streams[i]); return -1; }
+        }
+    }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    u8* d = nullptr;
+    int r = 0;
+    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
+    if (ok(cudaMallocAsync(&d, 8 * (size_t)n, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d, streams, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy streams") &&
+        ok(cudaMemcpyAsync(d + 4 * (size_t)n, start, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy start")) {
+        sb_tx_reset_kernel<<<(n + SB_TX_BLOCK - 1) / SB_TX_BLOCK, SB_TX_BLOCK, 0, st>>>(q->q, (const i32*)d, (const u32*)(d + 4 * (size_t)n), n);
+        count_launch();
+        ok(cudaGetLastError(), "sb_tx_reset_kernel");
+    }
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "tx_reset");
+    return r;
+}
+
+int solo_b200_tx_stats(solo_b200_tx* q, uint32_t* counters, void* cuda_stream) {
+    if (!q || !counters) { snprintf(g_err, sizeof g_err, "tx_stats: bad argument"); return -1; }
+    CK(cudaSetDevice(q->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaMemcpyAsync(counters, q->q.cnt, 4 * TX_NCOUNT * (size_t)q->q.n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// ---- downlink contributor lists (sb_tx.cuh) ----------------------------------------------------------------------------------
+static int contributors_scalars_ok(int n, int n_rooms, int k) {
+    if (n > 0 && n_rooms >= 0 && k >= 1 && k <= SB_MIX_KMAX) return 1;
+    snprintf(g_err, sizeof g_err, "mix_contributors: bad argument (n %d, n_rooms %d, k %d)", n, n_rooms, k);
+    return 0;
+}
+// every row -1 / 127 (the rows of streams in no room keep that), then one kernel for the members' rows; no kernel without rooms
+static int contributors_launch(const i32* room_start, const i32* members, int R, int k, const i32* talkers, const u8* level,
+                               int n, i32* csrc, u8* csrc_level, cudaStream_t st) {
+    const size_t e = (size_t)n * (size_t)k;
+    CK(cudaMemsetAsync(csrc, 0xFF, 4 * e, st));
+    CK(cudaMemsetAsync(csrc_level, SB_TX_LVL_NONE, e, st));
+    if (R == 0) return 0;
+    sb_mix_contributors_kernel<<<(n + SB_CONTRIB_THREADS - 1) / SB_CONTRIB_THREADS, SB_CONTRIB_THREADS, 0, st>>>(
+        room_start, members, R, k, talkers, level, n, csrc, csrc_level);
+    count_launch();
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int solo_b200_mix_contributors_device(const int32_t* d_room_start, const int32_t* d_members, int n_rooms, int k,
+                                      const int32_t* d_talkers, const uint8_t* d_level, int n, int32_t* d_csrc,
+                                      uint8_t* d_csrc_level, void* cuda_stream) {
+    if (!d_room_start || !d_members || !d_talkers || !d_level || !d_csrc || !d_csrc_level) { snprintf(g_err, sizeof g_err, "mix_contributors: bad argument"); return -1; }
+    if (!contributors_scalars_ok(n, n_rooms, k)) return -1;
+    return contributors_launch(d_room_start, d_members, n_rooms, k, d_talkers, d_level, n, d_csrc, d_csrc_level, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_mix_contributors_host(const int32_t* room_start, const int32_t* members, int n_rooms, int k, const int32_t* talkers,
+                                    const uint8_t* level, int n, int32_t* csrc, uint8_t* csrc_level) {
+    if (!room_start || !level || !csrc || !csrc_level || (n_rooms > 0 && !talkers)) { snprintf(g_err, sizeof g_err, "mix_contributors: bad argument"); return -1; }
+    if (!contributors_scalars_ok(n, n_rooms, k)) return -1;
+    if (room_start[0] != 0) { snprintf(g_err, sizeof g_err, "mix_contributors: room_start[0] is %d, not 0", room_start[0]); return -1; }
+    for (int r = 0; r < n_rooms; r++)
+        if (room_start[r + 1] < room_start[r]) { snprintf(g_err, sizeof g_err, "mix_contributors: room_start decreases at room %d", r); return -1; }
+    const i32 M = room_start[n_rooms];
+    if (M > 0 && !members) { snprintf(g_err, sizeof g_err, "mix_contributors: bad argument (members NULL)"); return -1; }
+    {
+        std::vector<u8> seen((size_t)n, 0);
+        for (i32 m = 0; m < M; m++) {
+            const i32 j = members[m];
+            if (j < 0 || j >= n) { snprintf(g_err, sizeof g_err, "mix_contributors: member %d is stream %d, outside [0, %d)", m, j, n); return -1; }
+            if (seen[j]++) { snprintf(g_err, sizeof g_err, "mix_contributors: stream %d is listed twice", j); return -1; }
+        }
+    }
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    if (int e = require_gpu(dev)) return e;
+    const size_t e = (size_t)n * (size_t)k, tk = 4 * (size_t)n_rooms * (size_t)k, rs = 4 * ((size_t)n_rooms + 1 + (size_t)M);
+    cudaStream_t st;
+    CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    u8* d = nullptr;            // csrc [n][k] | room_start, members | talkers | level | csrc_level [n][k]
+    const size_t o_rs = 4 * e, o_tk = o_rs + rs, o_lv = o_tk + tk, o_cl = o_lv + (size_t)n;
+    int r = 0;
+    auto ok = [&](cudaError_t err, const char* what) { if (!r && err != cudaSuccess) r = fail(what, err); return !r; };
+    ok(cudaMallocAsync(&d, o_cl + e, st), "cudaMallocAsync") &&
+        ok(cudaMemcpyAsync(d + o_rs, room_start, 4 * ((size_t)n_rooms + 1), cudaMemcpyHostToDevice, st), "copy room_start") &&
+        (M == 0 || ok(cudaMemcpyAsync(d + o_rs + 4 * ((size_t)n_rooms + 1), members, 4 * (size_t)M, cudaMemcpyHostToDevice, st), "copy members")) &&
+        (tk == 0 || ok(cudaMemcpyAsync(d + o_tk, talkers, tk, cudaMemcpyHostToDevice, st), "copy talkers")) &&
+        ok(cudaMemcpyAsync(d + o_lv, level, (size_t)n, cudaMemcpyHostToDevice, st), "copy level");
+    if (!r) r = contributors_launch((const i32*)(d + o_rs), (const i32*)(d + o_rs + 4 * ((size_t)n_rooms + 1)), n_rooms, k,
+                                    (const i32*)(d + o_tk), d + o_lv, n, (i32*)d, d + o_cl, st);
+    ok(cudaStreamSynchronize(st), "mix_contributors") && ok(cudaMemcpyAsync(csrc, d, 4 * e, cudaMemcpyDeviceToHost, st), "copy csrc") &&
+        ok(cudaMemcpyAsync(csrc_level, d + o_cl, e, cudaMemcpyDeviceToHost, st), "copy csrc_level");
+    if (d) cudaFreeAsync(d, st);
+    ok(cudaStreamSynchronize(st), "mix_contributors");
+    cudaStreamDestroy(st);
+    return r;
 }
 
 // ---- multi-GPU ingest through peer memory --------------------------------------------------------------------------------
