@@ -152,6 +152,14 @@ def _activity_device(fn, h, d_pcm, d_level, d_flags, stream):
         raise SoloError("activity_device failed (%d): %s" % (r, _err()))
 
 
+def _queue_reset(fn, name, h, streams, start, stream):
+    streams = np.ascontiguousarray(streams, np.int32).ravel()
+    start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
+    r = fn(h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
+    if r:
+        raise SoloError("%s failed (%d): %s" % (name, r, _err()))
+
+
 def profile_enable(on=True):
     lib().solo_b200_profile_enable(1 if on else 0)
 
@@ -613,11 +621,7 @@ class RxQueue:
 
     def reset(self, streams, start, stream=0):
         """Empty the listed streams' slots, zero their counters, and play packet start[i] next on stream streams[i]."""
-        streams = np.ascontiguousarray(streams, np.int32).ravel()
-        start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
-        r = lib().solo_b200_rx_reset(self.h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
-        if r:
-            raise SoloError("rx_reset failed (%d): %s" % (r, _err()))
+        _queue_reset(lib().solo_b200_rx_reset, "rx_reset", self.h, streams, start, stream)
 
     def stats(self, stream=0):
         """(counters uint32 [N, 8] in the order of RX_COUNTERS, arrivals for streams outside [0, N))."""
@@ -681,11 +685,7 @@ class TxQueue:
 
     def reset(self, streams, start, stream=0):
         """Give the listed streams' next rows index start[i] and zero their counters."""
-        streams = np.ascontiguousarray(streams, np.int32).ravel()
-        start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
-        r = lib().solo_b200_tx_reset(self.h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
-        if r:
-            raise SoloError("tx_reset failed (%d): %s" % (r, _err()))
+        _queue_reset(lib().solo_b200_tx_reset, "tx_reset", self.h, streams, start, stream)
 
     def stats(self, stream=0):
         """counters uint32 [N, 4] in the order of TX_COUNTERS."""

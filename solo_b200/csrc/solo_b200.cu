@@ -31,6 +31,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <mutex>
 #include <vector>
 
@@ -817,6 +818,53 @@ static void count_launch() {
     std::lock_guard<std::mutex> lk(g_mu);
     g_launches++;
 }
+// right after one kernel launch: count it and report a launch error under the kernel's name
+static int launched(const char* kernel) {
+    count_launch();
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(kernel, e);
+}
+
+// The device staging of one call of the mixer and queue *_host entry points, on the call's stream.  span() lays out the
+// call's arrays: each gets a 16-byte-aligned place in one allocation, is copied in from `in` and back to `out` where those
+// are not NULL, and its device address is written to `dev` when run() has allocated.  Copies back happen only when every
+// earlier step succeeded, the launch's execution included.  finish() always frees, synchronises and returns the first error.
+struct Staging {
+    struct Span { void** dev; const void* in; void* out; size_t bytes, off; };
+    cudaStream_t st;
+    const char* who;            // names the entry point in errors
+    std::vector<Span> spans;
+    size_t size = 0;
+    u8* d = nullptr;
+    int r = 0;
+
+    Staging(cudaStream_t stream, const char* name) : st(stream), who(name) {}
+    bool ok(cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; }
+    template <class T> void span(T*& dev, const void* in, void* out, size_t bytes) {
+        spans.push_back({(void**)&dev, in, out, bytes, size});
+        size += (bytes + 15) / 16 * 16;
+    }
+    bool sync() { return ok(cudaStreamSynchronize(st), who); }
+    bool back(void* host, const void* dev, size_t bytes) { return !bytes || ok(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st), who); }
+    // allocate, copy in, launch() (0 or the error it reported), then wait and copy back; false after any failure
+    template <class F> bool run(F launch) {
+        if (!ok(cudaMallocAsync(&d, size, st), who)) return false;
+        for (Span& p : spans) *p.dev = d + p.off;
+        for (Span& p : spans)
+            if (p.in && p.bytes && !ok(cudaMemcpyAsync(d + p.off, p.in, p.bytes, cudaMemcpyHostToDevice, st), who)) return false;
+        if ((r = launch())) return false;
+        if (std::none_of(spans.begin(), spans.end(), [](const Span& p) { return p.out; })) return true;
+        if (!sync()) return false;
+        for (Span& p : spans)
+            if (p.out && !back(p.out, d + p.off, p.bytes)) return false;
+        return true;
+    }
+    int finish() {
+        if (d) cudaFreeAsync(d, st);
+        sync();
+        return r;
+    }
+};
 
 // A packet wave of a *_host call is cut into chunks of streams that run on the batch's CUDA streams: the copies of one chunk
 // overlap the kernels of another, and the blocks of one chunk's kernel fill the SMs that the tail of another chunk's kernel
@@ -991,16 +1039,12 @@ template <class B> static int state_copy(B* b, int idx, void* host, int to_host,
 static int activity_launch(const solo_b200_enc_batch* b, int lo, int n, const i16* pcm, u8* level, u8* flags, cudaStream_t st) {
     sb_activity_kernel<<<(n + SB_ACT_WARPS - 1) / SB_ACT_WARPS, SB_ACT_WARPS * 32, 0, st>>>(pcm + (size_t)lo * b->spp, b->spp, b->nf, b->d_scratch + lo,
                                                                                          nullptr, nullptr, level, flags, n);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_activity_kernel");
 }
 static int activity_launch(const solo_b200_dec_batch* b, int lo, int n, const i16* pcm, u8* level, u8* flags, cudaStream_t st) {
     sb_activity_kernel<<<(n + SB_ACT_WARPS - 1) / SB_ACT_WARPS, SB_ACT_WARPS * 32, 0, st>>>(pcm + (size_t)lo * b->spp, b->spp, b->nf, nullptr,
                                                                                          b->d_act_flags + lo, b->d_ret_int + lo, level, flags, n);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_activity_kernel");
 }
 // the report of streams [lo, lo + n) from the staged PCM rows into host arrays of n entries, on the batch's first CUDA
 // stream; returns when the arrays are filled
@@ -1151,9 +1195,7 @@ static bool control_in_range(const i32* rate, const i32* dtx, const i32* loss, i
 // the control kernel for streams [lo, lo + n); the arrays hold those n streams' entries
 static int enc_control_launch(solo_b200_enc_batch* b, int lo, int n, const i32* d_rate, const i32* d_dtx, const i32* d_loss, cudaStream_t st) {
     sb_enc_control_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(b->d_states + lo, n, d_rate, d_dtx, d_loss);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_enc_control_kernel");
 }
 // host arrays of streams [lo, lo + n) through the batch's staging into the control kernel on st; returns when it is done
 static int enc_control_host(solo_b200_enc_batch* b, int lo, int n, const i32* rate, const i32* dtx, const i32* loss, cudaStream_t st) {
@@ -1370,9 +1412,7 @@ int solo_b200_apply_loss_device(const uint8_t* d_bits_in, const int16_t* d_nbyte
                                 int16_t* d_nbytes_out, int cap, int n, void* cuda_stream) {
     if (!d_bits_in || !d_nbytes_in || !d_lostflag || !d_bits_out || !d_nbytes_out || cap < 16 || n <= 0) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
     sb_apply_loss_kernel<<<(n + 7) / 8, 256, 0, (cudaStream_t)cuda_stream>>>(d_bits_in, d_nbytes_in, d_lostflag, d_bits_out, d_nbytes_out, cap, n);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_apply_loss_kernel");
 }
 
 // ---- conference mixer (sb_mix.cuh) ---------------------------------------------------------------------------------------
@@ -1386,12 +1426,25 @@ static int mix_launch(const i16* in, i16* out, int spp, int n, const u8* level, 
                       const i32* members, int R, int k, i32* talkers, cudaStream_t st) {
     if (R == 0) return 0;
     sb_mix_select_kernel<<<(R + SB_MIX_WARPS - 1) / SB_MIX_WARPS, SB_MIX_WARPS * 32, 0, st>>>(level, flags, room_start, members, n, R, k, talkers);
-    count_launch();
-    CK(cudaGetLastError());
+    if (int e = launched("sb_mix_select_kernel")) return e;
     sb_mix_kernel<<<(n + SB_MIX_WARPS - 1) / SB_MIX_WARPS, SB_MIX_WARPS * 32, 0, st>>>(in, out, spp, n, room_start, members, R, k, talkers);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_mix_kernel");
+}
+// the room layout a *_host call of the mixer or the contributor lists takes: room_start[0] == 0 and non-decreasing,
+// members in [0, n), no stream listed twice; `who` prefixes the error text
+static int rooms_ok(const i32* room_start, const i32* members, int n_rooms, int n, const char* who) {
+    if (room_start[0] != 0) { snprintf(g_err, sizeof g_err, "%s: room_start[0] is %d, not 0", who, room_start[0]); return 0; }
+    for (int r = 0; r < n_rooms; r++)
+        if (room_start[r + 1] < room_start[r]) { snprintf(g_err, sizeof g_err, "%s: room_start decreases at room %d", who, r); return 0; }
+    const i32 M = room_start[n_rooms];
+    if (M > 0 && !members) { snprintf(g_err, sizeof g_err, "%s: bad argument (members NULL)", who); return 0; }
+    std::vector<u8> seen((size_t)n, 0);
+    for (i32 m = 0; m < M; m++) {
+        const i32 j = members[m];
+        if (j < 0 || j >= n) { snprintf(g_err, sizeof g_err, "%s: member %d is stream %d, outside [0, %d)", who, m, j, n); return 0; }
+        if (seen[j]++) { snprintf(g_err, sizeof g_err, "%s: stream %d is listed twice", who, j); return 0; }
+    }
+    return 1;
 }
 
 int solo_b200_mix_device(const int16_t* d_in, int16_t* d_out, int spp, int n, const uint8_t* d_level, const uint8_t* d_flags,
@@ -1409,49 +1462,25 @@ int solo_b200_mix_host(const int16_t* in, int16_t* out, int spp, int n, const ui
                        const int32_t* room_start, const int32_t* members, int n_rooms, int k, int32_t* talkers) {
     if (!in || !out || !level || !flags || !room_start || !talkers) { snprintf(g_err, sizeof g_err, "mix: bad argument"); return -1; }
     if (!mix_scalars_ok(spp, n, n_rooms, k)) return -1;
-    if (room_start[0] != 0) { snprintf(g_err, sizeof g_err, "mix: room_start[0] is %d, not 0", room_start[0]); return -1; }
-    for (int r = 0; r < n_rooms; r++)
-        if (room_start[r + 1] < room_start[r]) { snprintf(g_err, sizeof g_err, "mix: room_start decreases at room %d", r); return -1; }
-    const i32 M = room_start[n_rooms];
-    if (M > 0 && !members) { snprintf(g_err, sizeof g_err, "mix: bad argument (members NULL)"); return -1; }
-    {
-        std::vector<u8> seen((size_t)n, 0);
-        for (i32 m = 0; m < M; m++) {
-            const i32 j = members[m];
-            if (j < 0 || j >= n) { snprintf(g_err, sizeof g_err, "mix: member %d is stream %d, outside [0, %d)", m, j, n); return -1; }
-            if (seen[j]++) { snprintf(g_err, sizeof g_err, "mix: stream %d is listed twice", j); return -1; }
-        }
-    }
+    if (!rooms_ok(room_start, members, n_rooms, n, "mix")) return -1;
     if (n_rooms == 0) return 0;
     int dev = 0;
     CK(cudaGetDevice(&dev));
     if (int e = require_gpu(dev)) return e;
-    // `out` goes to the device too: rows of streams in no room come back as they were
-    const size_t bytes = sizeof(i16) * (size_t)spp * (size_t)n, tk = sizeof(i32) * (size_t)n_rooms * (size_t)k;
     cudaStream_t st;
     CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    i16 *d_in = nullptr, *d_out = nullptr;
-    u8* d_lf = nullptr;
-    i32 *d_rs = nullptr, *d_tk = nullptr;
-    int r = 0;
-    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
-    ok(cudaMallocAsync(&d_in, bytes, st), "cudaMallocAsync") && ok(cudaMallocAsync(&d_out, bytes, st), "cudaMallocAsync") &&
-        ok(cudaMallocAsync(&d_lf, 2 * (size_t)n, st), "cudaMallocAsync") &&
-        ok(cudaMallocAsync(&d_rs, sizeof(i32) * ((size_t)n_rooms + 1 + (size_t)M), st), "cudaMallocAsync") &&
-        ok(cudaMallocAsync(&d_tk, tk, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, st), "copy in") &&
-        ok(cudaMemcpyAsync(d_out, out, bytes, cudaMemcpyHostToDevice, st), "copy out") &&
-        ok(cudaMemcpyAsync(d_lf, level, (size_t)n, cudaMemcpyHostToDevice, st), "copy level") &&
-        ok(cudaMemcpyAsync(d_lf + n, flags, (size_t)n, cudaMemcpyHostToDevice, st), "copy flags") &&
-        ok(cudaMemcpyAsync(d_rs, room_start, sizeof(i32) * ((size_t)n_rooms + 1), cudaMemcpyHostToDevice, st), "copy room_start") &&
-        (M == 0 || ok(cudaMemcpyAsync(d_rs + n_rooms + 1, members, sizeof(i32) * (size_t)M, cudaMemcpyHostToDevice, st), "copy members"));
-    if (!r) r = mix_launch(d_in, d_out, spp, n, d_lf, d_lf + n, d_rs, d_rs + n_rooms + 1, n_rooms, k, d_tk, st);
-    // the results go to the caller's arrays only when every step succeeded
-    ok(cudaStreamSynchronize(st), "mix") && ok(cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, st), "copy out") &&
-        ok(cudaMemcpyAsync(talkers, d_tk, tk, cudaMemcpyDeviceToHost, st), "copy talkers");
-    for (void* p : {(void*)d_in, (void*)d_out, (void*)d_lf, (void*)d_rs, (void*)d_tk})
-        if (p) cudaFreeAsync(p, st);
-    ok(cudaStreamSynchronize(st), "mix");
+    const size_t bytes = sizeof(i16) * (size_t)spp * (size_t)n;
+    const i16* d_in; i16* d_out; const u8 *d_level, *d_flags; const i32 *d_rs, *d_members; i32* d_tk;
+    Staging s(st, "mix");
+    s.span(d_in, in, nullptr, bytes);
+    s.span(d_out, out, out, bytes);     // `out` goes in too: rows of streams in no room come back as they were
+    s.span(d_level, level, nullptr, (size_t)n);
+    s.span(d_flags, flags, nullptr, (size_t)n);
+    s.span(d_rs, room_start, nullptr, sizeof(i32) * ((size_t)n_rooms + 1));
+    s.span(d_members, members, nullptr, sizeof(i32) * (size_t)room_start[n_rooms]);
+    s.span(d_tk, nullptr, talkers, sizeof(i32) * (size_t)n_rooms * (size_t)k);
+    s.run([&] { return mix_launch(d_in, d_out, spp, n, d_level, d_flags, d_rs, d_members, n_rooms, k, d_tk, st); });
+    const int r = s.finish();
     cudaStreamDestroy(st);
     return r;
 }
@@ -1510,15 +1539,11 @@ static int rx_insert_launch(solo_b200_rx* r, const RxArrivals& A, cudaStream_t s
     const unsigned g = (unsigned)(((long long)A.n + SB_RX_THREADS - 1) / SB_RX_THREADS);
     const unsigned g2 = (unsigned)(((long long)A.n * SB_RX_TEAM + SB_RX_THREADS - 1) / SB_RX_THREADS);
     sb_rx_elect_kernel<<<g, SB_RX_THREADS, 0, st>>>(r->q, A);
-    count_launch();
-    CK(cudaGetLastError());
+    if (int e = launched("sb_rx_elect_kernel")) return e;
     sb_rx_classify_kernel<<<g2, SB_RX_THREADS, 0, st>>>(r->q, A);
-    count_launch();
-    CK(cudaGetLastError());
+    if (int e = launched("sb_rx_classify_kernel")) return e;
     sb_rx_commit_kernel<<<g, SB_RX_THREADS, 0, st>>>(r->q, A);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_rx_commit_kernel");
 }
 static int rx_insert_args_ok(solo_b200_rx* q, const void* stream, const void* index, const void* desc, const void* off,
                              const void* len, int n_arrivals, const void* payload, int64_t payload_bytes) {
@@ -1544,25 +1569,17 @@ int solo_b200_rx_insert_host(solo_b200_rx* q, const int32_t* stream, const uint3
     if (!rx_insert_args_ok(q, stream, index, desc, off, len, n_arrivals, payload, payload_bytes)) return -1;
     if (n_arrivals == 0) return 0;
     CK(cudaSetDevice(q->device));
-    const size_t na = (size_t)n_arrivals, pb = (size_t)payload_bytes;
-    cudaStream_t st = q->st;
-    u8* d = nullptr;            // [stream | index | off | len] int32 x n, desc x n, payload
-    int r = 0;
-    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
-    if (ok(cudaMallocAsync(&d, 17 * na + pb, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d, stream, 4 * na, cudaMemcpyHostToDevice, st), "copy stream") &&
-        ok(cudaMemcpyAsync(d + 4 * na, index, 4 * na, cudaMemcpyHostToDevice, st), "copy index") &&
-        ok(cudaMemcpyAsync(d + 8 * na, off, 4 * na, cudaMemcpyHostToDevice, st), "copy off") &&
-        ok(cudaMemcpyAsync(d + 12 * na, len, 4 * na, cudaMemcpyHostToDevice, st), "copy len") &&
-        ok(cudaMemcpyAsync(d + 16 * na, desc, na, cudaMemcpyHostToDevice, st), "copy desc") &&
-        (pb == 0 || ok(cudaMemcpyAsync(d + 17 * na, payload, pb, cudaMemcpyHostToDevice, st), "copy payload"))) {
-        const RxArrivals A = {(const i32*)d, (const u32*)(d + 4 * na), d + 16 * na, (const i32*)(d + 8 * na),
-                              (const i32*)(d + 12 * na), n_arrivals, d + 17 * na, payload_bytes};
-        r = rx_insert_launch(q, A, st);
-    }
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "rx_insert");
-    return r;
+    const size_t na = (size_t)n_arrivals;
+    RxArrivals A = {nullptr, nullptr, nullptr, nullptr, nullptr, n_arrivals, nullptr, payload_bytes};
+    Staging s(q->st, "rx_insert");
+    s.span(A.stream, stream, nullptr, 4 * na);
+    s.span(A.index, index, nullptr, 4 * na);
+    s.span(A.desc, desc, nullptr, na);
+    s.span(A.off, off, nullptr, 4 * na);
+    s.span(A.len, len, nullptr, 4 * na);
+    s.span(A.payload, payload, nullptr, (size_t)payload_bytes);
+    s.run([&] { return rx_insert_launch(q, A, q->st); });
+    return s.finish();
 }
 
 static int rx_pull_args_ok(solo_b200_rx* q, const void* bits, int cap, const void* nbytes, const void* lostflag) {
@@ -1572,9 +1589,7 @@ static int rx_pull_args_ok(solo_b200_rx* q, const void* bits, int cap, const voi
 }
 static int rx_pull_launch(solo_b200_rx* r, const u32* play, u8* bits, int cap, i16* nbytes, i32* lostflag, cudaStream_t st) {
     sb_rx_pull_kernel<<<(r->q.n + SB_RX_PULL_WARPS - 1) / SB_RX_PULL_WARPS, SB_RX_PULL_WARPS * 32, 0, st>>>(r->q, play, bits, cap, nbytes, lostflag);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_rx_pull_kernel");
 }
 
 int solo_b200_rx_pull_device(solo_b200_rx* q, const uint32_t* d_play, uint8_t* d_bits, int cap, int16_t* d_nbytes,
@@ -1588,49 +1603,45 @@ int solo_b200_rx_pull_device(solo_b200_rx* q, const uint32_t* d_play, uint8_t* d
 int solo_b200_rx_pull_host(solo_b200_rx* q, const uint32_t* play, uint8_t* bits, int cap, int16_t* nbytes, int32_t* lostflag) {
     if (!rx_pull_args_ok(q, bits, cap, nbytes, lostflag)) return -1;
     CK(cudaSetDevice(q->device));
-    const size_t n = (size_t)q->q.n, rows = n * (size_t)cap;
-    cudaStream_t st = q->st;
-    u8* d = nullptr;            // bits [n][cap] (the caller's rows go in, so bytes past nbytes[0] come back unchanged), nbytes,
-    int r = 0;                  // lostflag, play
-    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
-    const size_t o_nb = (rows + 15) / 16 * 16, o_lf = o_nb + 4 * n, o_play = o_lf + 4 * n;
-    if (ok(cudaMallocAsync(&d, o_play + 4 * n, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d, bits, rows, cudaMemcpyHostToDevice, st), "copy bits") &&
-        (!play || ok(cudaMemcpyAsync(d + o_play, play, 4 * n, cudaMemcpyHostToDevice, st), "copy play")) &&
-        !(r = rx_pull_launch(q, play ? (const u32*)(d + o_play) : nullptr, d, cap, (i16*)(d + o_nb), (i32*)(d + o_lf), st)))
-        ok(cudaMemcpyAsync(bits, d, rows, cudaMemcpyDeviceToHost, st), "copy bits") &&
-            ok(cudaMemcpyAsync(nbytes, d + o_nb, 4 * n, cudaMemcpyDeviceToHost, st), "copy nbytes") &&
-            ok(cudaMemcpyAsync(lostflag, d + o_lf, 4 * n, cudaMemcpyDeviceToHost, st), "copy lostflag");
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "rx_pull");
-    return r;
+    const size_t n = (size_t)q->q.n;
+    u8* d_bits; i16* d_nbytes; i32* d_lostflag; const u32* d_play;
+    Staging s(q->st, "rx_pull");
+    s.span(d_bits, bits, bits, n * (size_t)cap);    // the caller's rows go in too: bytes past nbytes[0] come back unchanged
+    s.span(d_nbytes, nullptr, nbytes, 4 * n);
+    s.span(d_lostflag, nullptr, lostflag, 4 * n);
+    s.span(d_play, play, nullptr, 4 * n);
+    s.run([&] { return rx_pull_launch(q, play ? d_play : nullptr, d_bits, cap, d_nbytes, d_lostflag, q->st); });
+    return s.finish();
 }
 
-int solo_b200_rx_reset(solo_b200_rx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
-    if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "rx_reset: bad argument"); return -1; }
-    {
-        std::vector<u8> seen((size_t)q->q.n, 0);
-        for (int i = 0; i < n; i++) {
-            if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "rx_reset: stream %d outside [0, %d)", streams[i], q->q.n); return -1; }
-            if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "rx_reset: stream %d is listed twice", streams[i]); return -1; }
-        }
+// The reset of either queue (Q solo_b200_rx or solo_b200_tx): a list of distinct streams of the queue, nothing done when it
+// is refused, then `kernel` (block threads per block) on the caller's stream, which the call synchronises.
+extern "C++" {
+template <class Q, class D>
+static int queue_reset(Q* q, const i32* streams, const u32* start, int n, cudaStream_t st,
+                       void (*kernel)(D, const i32*, const u32*, int), int block, const char* who) {
+    if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "%s: bad argument", who); return -1; }
+    std::vector<u8> seen((size_t)q->q.n, 0);
+    for (int i = 0; i < n; i++) {
+        if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "%s: stream %d outside [0, %d)", who, streams[i], q->q.n); return -1; }
+        if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "%s: stream %d is listed twice", who, streams[i]); return -1; }
     }
     if (n == 0) return 0;
     CK(cudaSetDevice(q->device));
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    u8* d = nullptr;
-    int r = 0;
-    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
-    if (ok(cudaMallocAsync(&d, 8 * (size_t)n, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d, streams, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy streams") &&
-        ok(cudaMemcpyAsync(d + 4 * (size_t)n, start, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy start")) {
-        sb_rx_reset_kernel<<<(n + SB_RX_THREADS - 1) / SB_RX_THREADS, SB_RX_THREADS, 0, st>>>(q->q, (const i32*)d, (const u32*)(d + 4 * (size_t)n), n);
-        count_launch();
-        ok(cudaGetLastError(), "sb_rx_reset_kernel");
-    }
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "rx_reset");
-    return r;
+    const i32* d_streams; const u32* d_start;
+    Staging s(st, who);
+    s.span(d_streams, streams, nullptr, 4 * (size_t)n);
+    s.span(d_start, start, nullptr, 4 * (size_t)n);
+    s.run([&] {
+        kernel<<<(n + block - 1) / block, block, 0, st>>>(q->q, d_streams, d_start, n);
+        return launched(who);
+    });
+    return s.finish();
+}
+}  // extern "C++"
+
+int solo_b200_rx_reset(solo_b200_rx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
+    return queue_reset(q, streams, start, n, (cudaStream_t)cuda_stream, sb_rx_reset_kernel, SB_RX_THREADS, "rx_reset");
 }
 
 int solo_b200_rx_stats(solo_b200_rx* q, uint32_t* counters, uint64_t* bad_stream, void* cuda_stream) {
@@ -1702,15 +1713,11 @@ static int tx_pack_args_ok(solo_b200_tx* q, const void* bits, int cap, const voi
 static int tx_pack_launch(solo_b200_tx* t, const u8* bits, int cap, const i16* nbytes, const TxOut& o, cudaStream_t st) {
     const int nblk = tx_blocks(t->q.n);
     sb_tx_sizes_kernel<<<nblk, SB_TX_BLOCK, 0, st>>>(t->q, nbytes, cap);
-    count_launch();
-    CK(cudaGetLastError());
+    if (int e = launched("sb_tx_sizes_kernel")) return e;
     sb_tx_scan_kernel<<<1, SB_TX_SCAN_THREADS, 0, st>>>(t->q, nblk, o.count, o.total);
-    count_launch();
-    CK(cudaGetLastError());
+    if (int e = launched("sb_tx_scan_kernel")) return e;
     sb_tx_pack_kernel<<<(t->q.n + SB_TX_PACK_WARPS - 1) / SB_TX_PACK_WARPS, SB_TX_PACK_WARPS * 32, 0, st>>>(t->q, bits, cap, nbytes, o);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_tx_pack_kernel");
 }
 
 int solo_b200_tx_pack_device(solo_b200_tx* q, const uint8_t* d_bits, int cap, const int16_t* d_nbytes, uint8_t* d_payload,
@@ -1735,62 +1742,31 @@ int solo_b200_tx_pack_host(solo_b200_tx* q, const uint8_t* bits, int cap, const 
     if (!tx_pack_args_ok(q, bits, cap, nbytes, h, payload_cap)) return -1;
     CK(cudaSetDevice(q->device));
     const size_t n = (size_t)q->q.n, rows = n * (size_t)cap, e = 2 * n;
-    cudaStream_t st = q->st;
-    // bits [n][cap] | payload [n * cap] | stream, index, off, len [2n] each | count, total | nbytes [n][2] | desc [2n]
-    const size_t o_pay = rows, o_ent = 2 * rows, o_cnt = o_ent + 16 * e, o_nb = o_cnt + 16, o_desc = o_nb + 4 * n;
-    u8* d = nullptr;
-    int r = 0;
-    auto ok = [&](cudaError_t err, const char* what) { if (!r && err != cudaSuccess) r = fail(what, err); return !r; };
-    if (ok(cudaMallocAsync(&d, o_desc + e, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d, bits, rows, cudaMemcpyHostToDevice, st), "copy bits") &&
-        ok(cudaMemcpyAsync(d + o_nb, nbytes, 4 * n, cudaMemcpyHostToDevice, st), "copy nbytes")) {
-        const TxOut o = {d + o_pay, (i32*)(d + o_ent), (u32*)(d + o_ent + 4 * e), d + o_desc, (i32*)(d + o_ent + 8 * e),
-                         (i32*)(d + o_ent + 12 * e), (i32*)(d + o_cnt), (i64*)(d + o_cnt + 8)};
-        if (!(r = tx_pack_launch(q, d, cap, (const i16*)(d + o_nb), o, st)) &&
-            ok(cudaMemcpyAsync(&count, o.count, 4, cudaMemcpyDeviceToHost, st), "copy count") &&
-            ok(cudaMemcpyAsync(&tot, o.total, 8, cudaMemcpyDeviceToHost, st), "copy total") &&
-            ok(cudaStreamSynchronize(st), "tx_pack")) {
-            const size_t c = (size_t)count;
-            (tot == 0 || ok(cudaMemcpyAsync(payload, o.payload, (size_t)tot, cudaMemcpyDeviceToHost, st), "copy payload")) &&
-                ok(cudaMemcpyAsync(stream, o.stream, 4 * c, cudaMemcpyDeviceToHost, st), "copy stream") &&
-                ok(cudaMemcpyAsync(index, o.index, 4 * c, cudaMemcpyDeviceToHost, st), "copy index") &&
-                ok(cudaMemcpyAsync(desc, o.desc, c, cudaMemcpyDeviceToHost, st), "copy desc") &&
-                ok(cudaMemcpyAsync(off, o.off, 4 * c, cudaMemcpyDeviceToHost, st), "copy off") &&
-                ok(cudaMemcpyAsync(len, o.len, 4 * c, cudaMemcpyDeviceToHost, st), "copy len");
-        }
+    const u8* d_bits; const i16* d_nbytes; TxOut o;
+    Staging s(q->st, "tx_pack");
+    s.span(d_bits, bits, nullptr, rows);
+    s.span(d_nbytes, nbytes, nullptr, 4 * n);
+    s.span(o.payload, nullptr, nullptr, rows);
+    s.span(o.stream, nullptr, nullptr, 4 * e);
+    s.span(o.index, nullptr, nullptr, 4 * e);
+    s.span(o.desc, nullptr, nullptr, e);
+    s.span(o.off, nullptr, nullptr, 4 * e);
+    s.span(o.len, nullptr, nullptr, 4 * e);
+    s.span(o.count, nullptr, &count, 4);
+    s.span(o.total, nullptr, &tot, 8);
+    // the count and the total first, then only the datagrams they cover
+    if (s.run([&] { return tx_pack_launch(q, d_bits, cap, d_nbytes, o, q->st); }) && s.sync()) {
+        const size_t c = (size_t)count;
+        s.back(payload, o.payload, (size_t)tot) && s.back(stream, o.stream, 4 * c) && s.back(index, o.index, 4 * c) &&
+            s.back(desc, o.desc, c) && s.back(off, o.off, 4 * c) && s.back(len, o.len, 4 * c);
     }
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "tx_pack");
-    if (r) return r;
+    if (int r = s.finish()) return r;
     *total = tot;
     return count;
 }
 
 int solo_b200_tx_reset(solo_b200_tx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
-    if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "tx_reset: bad argument"); return -1; }
-    {
-        std::vector<u8> seen((size_t)q->q.n, 0);
-        for (int i = 0; i < n; i++) {
-            if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "tx_reset: stream %d outside [0, %d)", streams[i], q->q.n); return -1; }
-            if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "tx_reset: stream %d is listed twice", streams[i]); return -1; }
-        }
-    }
-    if (n == 0) return 0;
-    CK(cudaSetDevice(q->device));
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    u8* d = nullptr;
-    int r = 0;
-    auto ok = [&](cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; };
-    if (ok(cudaMallocAsync(&d, 8 * (size_t)n, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d, streams, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy streams") &&
-        ok(cudaMemcpyAsync(d + 4 * (size_t)n, start, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "copy start")) {
-        sb_tx_reset_kernel<<<(n + SB_TX_BLOCK - 1) / SB_TX_BLOCK, SB_TX_BLOCK, 0, st>>>(q->q, (const i32*)d, (const u32*)(d + 4 * (size_t)n), n);
-        count_launch();
-        ok(cudaGetLastError(), "sb_tx_reset_kernel");
-    }
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "tx_reset");
-    return r;
+    return queue_reset(q, streams, start, n, (cudaStream_t)cuda_stream, sb_tx_reset_kernel, SB_TX_BLOCK, "tx_reset");
 }
 
 int solo_b200_tx_stats(solo_b200_tx* q, uint32_t* counters, void* cuda_stream) {
@@ -1817,9 +1793,7 @@ static int contributors_launch(const i32* room_start, const i32* members, int R,
     if (R == 0) return 0;
     sb_mix_contributors_kernel<<<(n + SB_CONTRIB_THREADS - 1) / SB_CONTRIB_THREADS, SB_CONTRIB_THREADS, 0, st>>>(
         room_start, members, R, k, talkers, level, n, csrc, csrc_level);
-    count_launch();
-    CK(cudaGetLastError());
-    return 0;
+    return launched("sb_mix_contributors_kernel");
 }
 
 int solo_b200_mix_contributors_device(const int32_t* d_room_start, const int32_t* d_members, int n_rooms, int k,
@@ -1834,40 +1808,23 @@ int solo_b200_mix_contributors_host(const int32_t* room_start, const int32_t* me
                                     const uint8_t* level, int n, int32_t* csrc, uint8_t* csrc_level) {
     if (!room_start || !level || !csrc || !csrc_level || (n_rooms > 0 && !talkers)) { snprintf(g_err, sizeof g_err, "mix_contributors: bad argument"); return -1; }
     if (!contributors_scalars_ok(n, n_rooms, k)) return -1;
-    if (room_start[0] != 0) { snprintf(g_err, sizeof g_err, "mix_contributors: room_start[0] is %d, not 0", room_start[0]); return -1; }
-    for (int r = 0; r < n_rooms; r++)
-        if (room_start[r + 1] < room_start[r]) { snprintf(g_err, sizeof g_err, "mix_contributors: room_start decreases at room %d", r); return -1; }
-    const i32 M = room_start[n_rooms];
-    if (M > 0 && !members) { snprintf(g_err, sizeof g_err, "mix_contributors: bad argument (members NULL)"); return -1; }
-    {
-        std::vector<u8> seen((size_t)n, 0);
-        for (i32 m = 0; m < M; m++) {
-            const i32 j = members[m];
-            if (j < 0 || j >= n) { snprintf(g_err, sizeof g_err, "mix_contributors: member %d is stream %d, outside [0, %d)", m, j, n); return -1; }
-            if (seen[j]++) { snprintf(g_err, sizeof g_err, "mix_contributors: stream %d is listed twice", j); return -1; }
-        }
-    }
+    if (!rooms_ok(room_start, members, n_rooms, n, "mix_contributors")) return -1;
     int dev = 0;
     CK(cudaGetDevice(&dev));
     if (int e = require_gpu(dev)) return e;
-    const size_t e = (size_t)n * (size_t)k, tk = 4 * (size_t)n_rooms * (size_t)k, rs = 4 * ((size_t)n_rooms + 1 + (size_t)M);
     cudaStream_t st;
     CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    u8* d = nullptr;            // csrc [n][k] | room_start, members | talkers | level | csrc_level [n][k]
-    const size_t o_rs = 4 * e, o_tk = o_rs + rs, o_lv = o_tk + tk, o_cl = o_lv + (size_t)n;
-    int r = 0;
-    auto ok = [&](cudaError_t err, const char* what) { if (!r && err != cudaSuccess) r = fail(what, err); return !r; };
-    ok(cudaMallocAsync(&d, o_cl + e, st), "cudaMallocAsync") &&
-        ok(cudaMemcpyAsync(d + o_rs, room_start, 4 * ((size_t)n_rooms + 1), cudaMemcpyHostToDevice, st), "copy room_start") &&
-        (M == 0 || ok(cudaMemcpyAsync(d + o_rs + 4 * ((size_t)n_rooms + 1), members, 4 * (size_t)M, cudaMemcpyHostToDevice, st), "copy members")) &&
-        (tk == 0 || ok(cudaMemcpyAsync(d + o_tk, talkers, tk, cudaMemcpyHostToDevice, st), "copy talkers")) &&
-        ok(cudaMemcpyAsync(d + o_lv, level, (size_t)n, cudaMemcpyHostToDevice, st), "copy level");
-    if (!r) r = contributors_launch((const i32*)(d + o_rs), (const i32*)(d + o_rs + 4 * ((size_t)n_rooms + 1)), n_rooms, k,
-                                    (const i32*)(d + o_tk), d + o_lv, n, (i32*)d, d + o_cl, st);
-    ok(cudaStreamSynchronize(st), "mix_contributors") && ok(cudaMemcpyAsync(csrc, d, 4 * e, cudaMemcpyDeviceToHost, st), "copy csrc") &&
-        ok(cudaMemcpyAsync(csrc_level, d + o_cl, e, cudaMemcpyDeviceToHost, st), "copy csrc_level");
-    if (d) cudaFreeAsync(d, st);
-    ok(cudaStreamSynchronize(st), "mix_contributors");
+    const size_t e = (size_t)n * (size_t)k;
+    const i32 *d_rs, *d_members, *d_talkers; const u8* d_level; i32* d_csrc; u8* d_csrc_level;
+    Staging s(st, "mix_contributors");
+    s.span(d_rs, room_start, nullptr, 4 * ((size_t)n_rooms + 1));
+    s.span(d_members, members, nullptr, 4 * (size_t)room_start[n_rooms]);
+    s.span(d_talkers, talkers, nullptr, 4 * (size_t)n_rooms * (size_t)k);
+    s.span(d_level, level, nullptr, (size_t)n);
+    s.span(d_csrc, nullptr, csrc, 4 * e);
+    s.span(d_csrc_level, nullptr, csrc_level, e);
+    s.run([&] { return contributors_launch(d_rs, d_members, n_rooms, k, d_talkers, d_level, n, d_csrc, d_csrc_level, st); });
+    const int r = s.finish();
     cudaStreamDestroy(st);
     return r;
 }

@@ -218,8 +218,8 @@ def test_malformed_device_inputs_do_not_spread(sb):
 
 
 def test_launch_budget_and_existing_calls(sb):
-    """insert: three launches (none for no arrivals); pull: one.  A decode_device call launches the same number of kernels
-    with a queue alive as without."""
+    """insert: three launches (none for no arrivals); pull: one; reset: one.  A decode_device call launches the same number
+    of kernels with a queue alive as without."""
     import torch
     n = 64
     dec = sb.DecoderBatch(n)
@@ -244,11 +244,13 @@ def test_launch_budget_and_existing_calls(sb):
     one = np.ones(1, np.int32)
     assert launches(lambda: q.insert(one, one.astype(np.uint32), one.astype(np.uint8), 0 * one, one, np.ones(4, np.uint8))) == 3
     assert launches(lambda: q.pull()) == 1
+    assert launches(lambda: q.q.reset([1, 2], [5, 6])) == 1
     assert launches(lambda: dec.decode_device(d_pcm.data_ptr(), d_bits.data_ptr(), 256, d_nb.data_ptr(), d_lf.data_ptr(), 0, st)) == before
     with pytest.raises(sb.SoloError):
         q.q.pull(cap=255)                               # below 2 * desc_cap
-    with pytest.raises(sb.SoloError):
-        q.q.reset([0, 0], [1, 1])                       # listed twice
+    for streams in ([0, 0], [-1], [n]):                 # listed twice, outside [0, n)
+        with pytest.raises(sb.SoloError):
+            q.q.reset(streams, [1] * len(streams))
     dec.close()
 
 
