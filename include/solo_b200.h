@@ -272,6 +272,49 @@ int solo_b200_rx_pull_device(solo_b200_rx *q, const uint32_t *d_play, uint8_t *d
 int solo_b200_rx_reset(solo_b200_rx *q, const int32_t *streams, const uint32_t *start, int n, void *cuda_stream);
 int solo_b200_rx_stats(solo_b200_rx *q, uint32_t *counters, uint64_t *bad_stream, void *cuda_stream);
 
+/* Receive queue timing: what an RTCP receiver report (RFC 3550 6.4.1) needs beyond the counters, and how early packets
+   arrive, from each datagram's arrival time.  Opt-in per queue; the calls above keep their behaviour and kernels.
+   enable_timing: ts_per_index is the number of RTP timestamp units per packet index (640 for 16 kHz streams with 40 ms
+     packets); max_arrivals bounds n_arrivals of a timed insert.  Allocates 52 B per stream plus 16.5 B per arrival of
+     scratch.  -1 for ts_per_index = 0, max_arrivals < 1, or when timing is already enabled.  Per stream it keeps:
+       transit  : uint32, transit time of the previous valid arrival;
+       jitter   : uint32, RFC 3550 A.8 interarrival jitter in 1/16 timestamp units;
+       highest  : uint64, extended highest index received, cycles << 32 | index;
+       received : uint32, valid arrivals since the last reset (mod 2^32);
+       margin   : 8 uint32, the playout-margin histogram.
+   insert_timed: the insert's arrays plus arrival[a], arrival a's receive time in RTP timestamp units of the receiver's
+     clock (mod 2^32).  It leaves exactly the slots, stored payload, counters and bad_stream count that insert leaves
+     for the same arrays, and also:
+     - A VALID arrival has its stream in [0, N) and is not malformed; late and duplicate arrivals are valid.  Only valid
+       arrivals touch the timing state.
+     - Over a stream's valid arrivals in ARRAY ORDER (the arrival order), with uint32 arithmetic: transit
+       t = arrival - index * ts_per_index.  If received > 0: d = |(int32)(t - transit)| (2^31 for INT_MIN) and
+       jitter += d - ((jitter + 8) >> 4); highest moves to index p when (p - (uint32)highest) mod 2^32 lies in [1, 2^31),
+       with one more cycle when p < (uint32)highest.  If received = 0, highest = p (cycle 0).  Then transit = t and
+       received += 1.
+     - Each valid arrival whose index is current adds one to margin bin min(index - last - 1, 7): bin 0 plays at the
+       next pull, bin 7 seven or more pulls later.  Late arrivals count in `late` only.
+     The result does not depend on thread scheduling.  The running time is linear in n_arrivals whatever the arrays hold,
+     including every arrival on one stream.
+   timing: jitter (reported as jitter >> 4, RFC 3550), highest and received [N], margin [N][8]; any may be NULL.  Ordered
+     on `cuda_stream`; returns after synchronising it.  -1 when timing is not enabled.
+   reset also zeroes the listed streams' timing state (highest restarts from the next valid arrival).  insert never
+   touches it.
+   Entry points: *_host and *_device as for insert; the device form checks the scalars (-1 also when timing is not
+   enabled or n_arrivals > max_arrivals) and never reads or writes out of bounds whatever the arrays hold.
+   Launches: a timed insert of n_arrivals > 0 launches insert's three kernels, then 2 + 3 * ceil(log2(N) / 8); a reset
+   of a timed queue two kernels. */
+int solo_b200_rx_enable_timing(solo_b200_rx *q, uint32_t ts_per_index, int max_arrivals);
+int solo_b200_rx_insert_timed_host(solo_b200_rx *q, const int32_t *stream, const uint32_t *index, const uint8_t *desc,
+                                   const int32_t *off, const int32_t *len, const uint32_t *arrival, int n_arrivals,
+                                   const uint8_t *payload, int64_t payload_bytes);
+int solo_b200_rx_insert_timed_device(solo_b200_rx *q, const int32_t *d_stream, const uint32_t *d_index,
+                                     const uint8_t *d_desc, const int32_t *d_off, const int32_t *d_len,
+                                     const uint32_t *d_arrival, int n_arrivals, const uint8_t *d_payload,
+                                     int64_t payload_bytes, void *cuda_stream);
+int solo_b200_rx_timing(solo_b200_rx *q, uint32_t *jitter, uint64_t *highest, uint32_t *received, uint32_t *margin,
+                        void *cuda_stream);
+
 /* Send queue: turns a wave of the encoder's rows into numbered datagrams, two per row (solo_b200_split_packet), packed
    back to back in one buffer in the receive queue's arrival format, for N streams on the device.  It is independent of
    the codec batches: a pack takes the rows of any encoder batch with the same N.

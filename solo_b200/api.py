@@ -104,6 +104,10 @@ def lib():
         L.solo_b200_rx_pull_device.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
         L.solo_b200_rx_reset.argtypes = [vp, vp, vp, C.c_int, vp]
         L.solo_b200_rx_stats.argtypes = [vp, vp, vp, vp]
+        L.solo_b200_rx_enable_timing.argtypes = [vp, C.c_uint32, C.c_int]
+        L.solo_b200_rx_insert_timed_host.argtypes = [vp] * 7 + [C.c_int, vp, C.c_int64]
+        L.solo_b200_rx_insert_timed_device.argtypes = [vp] * 7 + [C.c_int, vp, C.c_int64, vp]
+        L.solo_b200_rx_timing.argtypes = [vp] * 6
         L.solo_b200_tx_create.restype = vp
         L.solo_b200_tx_create.argtypes = [C.c_int, C.c_int]
         L.solo_b200_tx_destroy.argtypes = [vp]
@@ -571,9 +575,18 @@ class RxQueue:
         if not self.h:
             raise SoloError("solo_b200_rx_create failed: " + _err())
 
-    def insert(self, streams, index, desc, payloads):
+    def enable_timing(self, ts_per_index, max_arrivals):
+        """Keep per-stream arrival timing from now on (RFC 3550 jitter, extended highest index, valid arrivals and the
+        playout-margin histogram; see solo_b200_rx_enable_timing): ts_per_index RTP timestamp units per packet index,
+        at most max_arrivals arrivals per timed insert."""
+        r = lib().solo_b200_rx_enable_timing(self.h, int(ts_per_index), int(max_arrivals))
+        if r:
+            raise SoloError("rx_enable_timing failed (%d): %s" % (r, _err()))
+
+    def insert(self, streams, index, desc, payloads, arrival=None):
         """Arrival a is description desc[a] (1 or 2) of packet index[a] of stream streams[a], bytes payloads[a]; the
-        payloads are laid out back to back for the call."""
+        payloads are laid out back to back for the call.  arrival (uint32 receive times in RTP timestamp units, one
+        per arrival) makes it a timed insert, which needs enable_timing first; None is the untimed insert."""
         streams = np.ascontiguousarray(streams, np.int32)
         index = np.ascontiguousarray(np.asarray(index, np.int64) & 0xFFFFFFFF, np.uint32)
         desc = np.ascontiguousarray(desc, np.uint8)
@@ -584,17 +597,35 @@ class RxQueue:
         flat = np.frombuffer(b"".join(bytes(p) for p in payloads), np.uint8).copy()
         if not (len(streams) == len(index) == len(desc) == len(lens)):
             raise SoloError("RxQueue.insert: streams, index, desc and payloads differ in length")
-        r = lib().solo_b200_rx_insert_host(self.h, streams.ctypes.data, index.ctypes.data, desc.ctypes.data, off.ctypes.data,
-                                           lens.ctypes.data, len(streams), flat.ctypes.data, flat.size)
+        if arrival is None:
+            r = lib().solo_b200_rx_insert_host(self.h, streams.ctypes.data, index.ctypes.data, desc.ctypes.data,
+                                               off.ctypes.data, lens.ctypes.data, len(streams), flat.ctypes.data, flat.size)
+            if r:
+                raise SoloError("rx_insert_host failed (%d): %s" % (r, _err()))
+            return
+        arrival = np.ascontiguousarray(np.asarray(arrival, np.int64) & 0xFFFFFFFF, np.uint32)
+        if arrival.shape != (len(streams),):
+            raise SoloError("RxQueue.insert: arrival must have one entry per arrival")
+        r = lib().solo_b200_rx_insert_timed_host(self.h, streams.ctypes.data, index.ctypes.data, desc.ctypes.data,
+                                                 off.ctypes.data, lens.ctypes.data, arrival.ctypes.data, len(streams),
+                                                 flat.ctypes.data, flat.size)
         if r:
-            raise SoloError("rx_insert_host failed (%d): %s" % (r, _err()))
+            raise SoloError("rx_insert_timed_host failed (%d): %s" % (r, _err()))
 
-    def insert_device(self, d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes, stream=0):
-        """insert on device arrays (addresses), enqueued on `stream`: three kernel launches, none for n_arrivals = 0."""
-        r = lib().solo_b200_rx_insert_device(self.h, d_stream, d_index, d_desc, d_off, d_len, int(n_arrivals), d_payload,
-                                             int(payload_bytes), stream)
+    def insert_device(self, d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes, stream=0,
+                      d_arrival=None):
+        """insert on device arrays (addresses), enqueued on `stream`: three kernel launches, none for n_arrivals = 0.
+        d_arrival (uint32 receive times) makes it a timed insert: 2 + 3 * ceil(log2(N) / 8) launches more."""
+        if d_arrival is None:
+            r = lib().solo_b200_rx_insert_device(self.h, d_stream, d_index, d_desc, d_off, d_len, int(n_arrivals), d_payload,
+                                                 int(payload_bytes), stream)
+            if r:
+                raise SoloError("rx_insert_device failed (%d): %s" % (r, _err()))
+            return
+        r = lib().solo_b200_rx_insert_timed_device(self.h, d_stream, d_index, d_desc, d_off, d_len, d_arrival,
+                                                   int(n_arrivals), d_payload, int(payload_bytes), stream)
         if r:
-            raise SoloError("rx_insert_device failed (%d): %s" % (r, _err()))
+            raise SoloError("rx_insert_timed_device failed (%d): %s" % (r, _err()))
 
     def pull(self, play=None, cap=256):
         """One tick: -> (bits uint8 [N, cap], nbytes int16 [N, 2], lostflag int32 [N]) of packet play[s] (None: each
@@ -631,6 +662,17 @@ class RxQueue:
         if r:
             raise SoloError("rx_stats failed (%d): %s" % (r, _err()))
         return cnt, int(bad.value)
+
+    def timing(self, stream=0):
+        """(jitter uint32 [N] in RTP timestamp units (RFC 3550: the kept value >> 4), highest uint64 [N] (cycles << 32 |
+        index), received uint32 [N], margin uint32 [N, 8]) of a timed queue."""
+        jitter, received = np.zeros(self.n, np.uint32), np.zeros(self.n, np.uint32)
+        highest, margin = np.zeros(self.n, np.uint64), np.zeros((self.n, 8), np.uint32)
+        r = lib().solo_b200_rx_timing(self.h, jitter.ctypes.data, highest.ctypes.data, received.ctypes.data,
+                                      margin.ctypes.data, stream)
+        if r:
+            raise SoloError("rx_timing failed (%d): %s" % (r, _err()))
+        return jitter, highest, received, margin
 
     def close(self):
         if getattr(self, "h", None):

@@ -1,6 +1,6 @@
 // solo_b200 -- receive queue of descriptions (include/solo_b200.h, solo_b200_rx_*).  The per-arrival and per-slot rules,
-// written once for the queue's kernels (solo_b200.cu) and the host model (tests/hostsim/rx.cpp), and the per-row merge rule
-// that solo_b200_merge_packets and the pull kernel share.
+// written once for the queue's kernels (solo_b200.cu) and the host models (tests/hostsim/rx.cpp and rx_timing.cpp), and
+// the per-row merge rule that solo_b200_merge_packets and the pull kernel share.
 //   current : packet index p is current for a stream whose last played index is `last` when (p - last) mod 2^32 lies in
 //             [1, 2^31); "newer" is a larger distance p - last.  A slot keeps the newest current index among its held one
 //             and the call's valid arrivals; per description of it a held one stays, otherwise the first arrival in array
@@ -9,6 +9,10 @@
 //             so the newest index and, for it, the first arrival win; per slot an atomic min of position picks the one
 //             arrival that commits the slot), classify (count every arrival, copy the stored ones), commit (the slot's new
 //             index and lengths, the held descriptions it discards, and the election words back to empty).
+//   timing  : (solo_b200_rx_enable_timing, solo_b200_rx_insert_timed_*) per stream transit, RFC 3550 A.8 jitter, the
+//             extended highest index, the count of valid arrivals and a playout-margin histogram, from each arrival's
+//             receive time.  Jitter and highest follow the stream's valid arrivals in array order (rx_timing_step); the
+//             margin bin of an arrival depends only on it and `last` (rx_margin_bin).
 #pragma once
 #include "sb_common.cuh"
 
@@ -102,6 +106,43 @@ SB_HD int rx_after_play(u32 t, u32 idx, u16* len) {
     const int stale = idx != t ? (len[0] != 0) + (len[1] != 0) : 0;
     len[0] = len[1] = 0;
     return stale;
+}
+
+// ---- timing ------------------------------------------------------------------------------------------------------------
+#define RX_MARGIN_BINS 8
+
+// an arrival the timing counts: its stream is in range and it is not malformed (late and duplicate arrivals count, as
+// RFC 3550 updates the jitter for every packet received)
+SB_HD bool rx_timed(int n, int desc_cap, i32 s, int desc, i32 off, i32 len, i64 payload_bytes) {
+    return (u32)s < (u32)n && !rx_malformed(desc, off, len, desc_cap, payload_bytes);
+}
+
+// margin bin of a valid arrival of index p for a stream whose last played index is `last`: min(p - last - 1, 7) when p is
+// current (bin 0 plays at the next pull), -1 when it is late
+SB_HD int rx_margin_bin(u32 p, u32 last) {
+    if (!rx_current(p, last)) return -1;
+    const u32 m = p - last - 1u;
+    return m < RX_MARGIN_BINS - 1 ? (int)m : RX_MARGIN_BINS - 1;
+}
+
+// One valid arrival of index p at receive time `arrival` (RTP timestamp units, mod 2^32) into its stream's timing state.
+// Transit t = arrival - p * ts_per_index.  From the second valid arrival since the reset on, RFC 3550 A.8:
+// d = |(int32)(t - transit)| (2^31 for INT_MIN), jitter += d - ((jitter + 8) >> 4), all in uint32; and highest
+// (cycles << 32 | index) moves to p when p is ahead of its low word by [1, 2^31), one cycle up when p wrapped below it.
+// The first valid arrival sets highest = p.
+SB_HD void rx_timing_step(u32 p, u32 arrival, u32 ts_per_index, u32* transit, u32* jitter, u64* highest, u32* received) {
+    const u32 t = arrival - p * ts_per_index;
+    if (*received) {
+        const u32 diff = t - *transit;
+        const u32 d = (diff & 0x80000000u) ? 0u - diff : diff;
+        *jitter += d - ((*jitter + 8u) >> 4);
+        const u32 lo = (u32)*highest;
+        if (p - lo - 1u < 0x7FFFFFFFu) *highest = (((*highest >> 32) + (p < lo ? 1u : 0u)) << 32) | p;
+    } else {
+        *highest = p;
+    }
+    *transit = t;
+    (*received)++;
 }
 
 }  // namespace sb

@@ -20,7 +20,9 @@
 // each room's loudest talkers, sb_mix_kernel (warp per member) writes each member's mix-minus row.
 // The receive queue (solo_b200_rx_*, sb_rx.cuh) pairs, reorders and screens the two descriptions of each stream's packets:
 // an insert is sb_rx_elect_kernel, sb_rx_classify_kernel and sb_rx_commit_kernel over the arrivals, a pull is
-// sb_rx_pull_kernel (warp per stream), which writes the decoder's input rows.
+// sb_rx_pull_kernel (warp per stream), which writes the decoder's input rows.  A timed insert of a queue with timing
+// enabled adds sb_rx_timing_keys_kernel, a stable radix sort of the arrivals by stream (sb_rx_sort_hist / scan / scatter
+// per 8-bit digit) and sb_rx_timing_walk_kernel, which runs each stream's jitter recurrence in array order.
 // The send queue (solo_b200_tx_*, sb_tx.cuh) turns the encoder's rows into numbered datagrams packed back to back: a pack
 // is sb_tx_sizes_kernel (thread per stream), sb_tx_scan_kernel (one block) and sb_tx_pack_kernel (warp per stream).
 // sb_mix_contributors_kernel (thread per member) writes each downlink's CSRC list and RFC 6465 levels.
@@ -603,6 +605,160 @@ __global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_reset_kernel(RxDev q, con
     q.last[s] = start[i] - 1u;
     for (int k = 0; k < RX_NCOUNT; k++) q.cnt[(size_t)s * RX_NCOUNT + k] = 0;
     for (int j = 0; j < 2 * q.depth; j++) q.len[(size_t)s * 2 * q.depth + j] = 0;
+}
+
+// ---- receive queue timing (sb_rx.cuh, solo_b200_rx_insert_timed_*) ------------------------------------------------------
+// A timed insert runs the three insert passes unchanged, then its own kernels.  The margin histogram is order-free (an
+// atomicAdd per arrival; it reads `last`, which no insert changes).  Jitter and highest are a recurrence over each stream's
+// valid arrivals in array order: the call's arrivals are grouped by stream with a stable LSD radix sort of their positions
+// (8-bit digits of the stream, ceil(log2 N / 8) passes of histogram, scan and scatter), then one thread per stream runs the
+// recurrence over its group.  Arrivals the timing does not count are keyed to stream 0 with RX_KEY_SKIP set and skipped
+// there.  Every step's result is fixed by the arrays alone, so nothing depends on scheduling.
+struct RxTiming {
+    u32 ts_per_index;
+    int max_arrivals, passes;   // passes: 8-bit digits of the largest stream index
+    u32* transit;               // [n] transit of the last valid arrival
+    u32* jitter;                // [n] RFC 3550 jitter, 1/16 units
+    unsigned long long* highest;// [n] cycles << 32 | highest index
+    u32* received;              // [n] valid arrivals since the reset
+    u32* margin;                // [n][RX_MARGIN_BINS]
+    u32* key[2];                // [max_arrivals] sort keys (stream, or RX_KEY_SKIP), double-buffered
+    u32* pos[2];                // [max_arrivals] arrival positions, double-buffered
+    u32* hist;                  // [256][tiles] per tile digit counts, then their exclusive prefix in digit-major order
+};
+#define RX_KEY_SKIP 0x80000000u
+#define SB_RX_SORT_THREADS 256  // one thread per digit value in the histogram and rank bookkeeping
+#define SB_RX_SORT_ITEMS 8      // rounds of 256 arrivals per tile
+#define SB_RX_SORT_TILE (SB_RX_SORT_THREADS * SB_RX_SORT_ITEMS)
+__device__ __forceinline__ u32 rx_sort_digit(u32 key, int shift) { return ((key & ~RX_KEY_SKIP) >> shift) & 255u; }
+__device__ __forceinline__ unsigned long long tx_warp_scan(unsigned long long v, int lane);   // send queue, below
+
+// timed insert, pass 1 (thread per arrival): the sort key and position of each arrival, and its margin bin
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_timing_keys_kernel(RxDev q, RxTiming T, RxArrivals A) {
+    const int a = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (a >= A.n) return;
+    const i32 s = A.stream[a];
+    const bool ok = rx_timed(q.n, q.desc_cap, s, A.desc[a], A.off[a], A.len[a], A.payload_bytes);
+    T.key[0][a] = ok ? (u32)s : RX_KEY_SKIP;
+    T.pos[0][a] = (u32)a;
+    if (!ok) return;
+    const int b = rx_margin_bin(A.index[a], q.last[s]);
+    if (b >= 0) atomicAdd(&T.margin[(size_t)s * RX_MARGIN_BINS + b], 1u);
+}
+
+// sort pass, step 1 (block per tile): the tile's count of each digit, stored digit-major
+__global__ void __launch_bounds__(SB_RX_SORT_THREADS) sb_rx_sort_hist_kernel(const u32* __restrict__ key, u32* __restrict__ hist, int n, int shift) {
+    __shared__ u32 h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int base = blockIdx.x * SB_RX_SORT_TILE + threadIdx.x;
+    for (int r = 0; r < SB_RX_SORT_ITEMS; r++) {
+        const int i = base + r * SB_RX_SORT_THREADS;
+        if (i < n) atomicAdd(&h[rx_sort_digit(key[i], shift)], 1u);
+    }
+    __syncthreads();
+    hist[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
+}
+
+// sort pass, step 2 (one block): the exclusive prefix of the `total` digit-major counts, in place.  Each thread sums a
+// contiguous run of counts; the runs' sums are scanned as the send queue scans its block totals.
+#define SB_RX_SCAN_THREADS 1024
+__global__ void __launch_bounds__(SB_RX_SCAN_THREADS) sb_rx_sort_scan_kernel(u32* __restrict__ hist, int total) {
+    __shared__ unsigned long long warp_total[SB_RX_SCAN_THREADS / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int per = (total + SB_RX_SCAN_THREADS - 1) / SB_RX_SCAN_THREADS;
+    const int lo = imin((int)threadIdx.x * per, total), hi = imin(lo + per, total);
+    unsigned long long x = 0;
+    for (int i = lo; i < hi; i++) x += hist[i];
+    const unsigned long long v = tx_warp_scan(x, lane);
+    if (lane == 31) warp_total[w] = v;
+    __syncthreads();
+    unsigned long long base = 0;
+    for (int i = 0; i < w; i++) base += warp_total[i];
+    u32 run = (u32)(base + v - x);
+    for (int i = lo; i < hi; i++) {
+        const u32 c = hist[i];
+        hist[i] = run;
+        run += c;
+    }
+}
+
+// sort pass, step 3 (block per tile): stable scatter of the tile's keys and positions to their digit's place.  Within a
+// round of 256 arrivals, an arrival's rank among equal digits is the count in the warps before its own plus, from
+// __match_any_sync, the count of lower lanes; the rounds run in order and carry each digit's running place.
+__global__ void __launch_bounds__(SB_RX_SORT_THREADS) sb_rx_sort_scatter_kernel(const u32* __restrict__ kin, const u32* __restrict__ pin,
+                                                                            u32* __restrict__ kout, u32* __restrict__ pout,
+                                                                            const u32* __restrict__ hist, int n, int shift) {
+    __shared__ u32 place[256];
+    __shared__ u32 wcount[SB_RX_SORT_THREADS / 32][256];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    place[threadIdx.x] = hist[(size_t)threadIdx.x * gridDim.x + blockIdx.x];
+    for (int k = 0; k < SB_RX_SORT_THREADS / 32; k++) wcount[k][threadIdx.x] = 0;
+    __syncthreads();
+    for (int r = 0; r < SB_RX_SORT_ITEMS; r++) {
+        const int r0 = blockIdx.x * SB_RX_SORT_TILE + r * SB_RX_SORT_THREADS;
+        if (r0 >= n) break;                       // uniform over the block
+        const int i = r0 + threadIdx.x;
+        const bool ok = i < n;
+        const u32 key = ok ? kin[i] : 0u, p = ok ? pin[i] : 0u;
+        const u32 dig = ok ? rx_sort_digit(key, shift) : 256u;
+        const u32 peers = __match_any_sync(0xffffffffu, dig);
+        const u32 below = __popc(peers & ((1u << lane) - 1u));
+        if (ok && below == 0) wcount[w][dig] = __popc(peers);
+        __syncthreads();
+        if (ok) {
+            u32 dst = place[dig] + below;
+            for (int k = 0; k < w; k++) dst += wcount[k][dig];
+            kout[dst] = key;
+            pout[dst] = p;
+        }
+        __syncthreads();
+        u32 t = 0;
+        for (int k = 0; k < SB_RX_SORT_THREADS / 32; k++) {
+            t += wcount[k][threadIdx.x];
+            wcount[k][threadIdx.x] = 0;
+        }
+        place[threadIdx.x] += t;
+        __syncthreads();
+    }
+}
+
+// timed insert, last pass (thread per sorted arrival; the first of each stream's group works): the stream's valid
+// arrivals in array order through rx_timing_step
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_timing_walk_kernel(RxTiming T, const u32* __restrict__ K, const u32* __restrict__ P,
+                                                                           RxArrivals A, const u32* __restrict__ arrival) {
+    const int i = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (i >= A.n) return;
+    const u32 s = K[i] & ~RX_KEY_SKIP;
+    if (i > 0 && (K[i - 1] & ~RX_KEY_SKIP) == s) return;
+    u32 transit = T.transit[s], jitter = T.jitter[s], received = T.received[s];
+    u64 highest = T.highest[s];
+    bool any = false;
+    for (int j = i; j < A.n; j++) {
+        const u32 k = K[j];
+        if ((k & ~RX_KEY_SKIP) != s) break;
+        if (k & RX_KEY_SKIP) continue;
+        const u32 a = P[j];
+        rx_timing_step(A.index[a], arrival[a], T.ts_per_index, &transit, &jitter, &highest, &received);
+        any = true;
+    }
+    if (!any) return;
+    T.transit[s] = transit;
+    T.jitter[s] = jitter;
+    T.highest[s] = highest;
+    T.received[s] = received;
+}
+
+// reset of the timing state (thread per listed stream; the host has checked the list)
+__global__ void __launch_bounds__(SB_RX_THREADS) sb_rx_timing_reset_kernel(RxTiming T, const i32* __restrict__ streams, int n) {
+    const int i = blockIdx.x * SB_RX_THREADS + threadIdx.x;
+    if (i >= n) return;
+    const i32 s = streams[i];
+    T.transit[s] = 0;
+    T.jitter[s] = 0;
+    T.highest[s] = 0;
+    T.received[s] = 0;
+    for (int k = 0; k < RX_MARGIN_BINS; k++) T.margin[(size_t)s * RX_MARGIN_BINS + k] = 0;
 }
 
 // ---- send queue (sb_tx.cuh) ----------------------------------------------------------------------------------------------
@@ -1490,10 +1646,13 @@ struct solo_b200_rx {
     int device;
     cudaStream_t st;            // the _host forms' stream
     RxDev q;
+    RxTiming t;                 // all zero until solo_b200_rx_enable_timing
     ~solo_b200_rx() {
         if (st) cudaStreamDestroy(st);
         cudaFree(q.last); cudaFree(q.idx); cudaFree(q.len); cudaFree(q.elect); cudaFree(q.rep); cudaFree(q.cnt);
         cudaFree(q.bad); cudaFree(q.store);
+        cudaFree(t.transit); cudaFree(t.jitter); cudaFree(t.highest); cudaFree(t.received); cudaFree(t.margin);
+        cudaFree(t.key[0]); cudaFree(t.key[1]); cudaFree(t.pos[0]); cudaFree(t.pos[1]); cudaFree(t.hist);
     }
 };
 
@@ -1582,6 +1741,119 @@ int solo_b200_rx_insert_host(solo_b200_rx* q, const int32_t* stream, const uint3
     return s.finish();
 }
 
+static int rx_sort_tiles(int n_arrivals) { return (n_arrivals + SB_RX_SORT_TILE - 1) / SB_RX_SORT_TILE; }
+
+int solo_b200_rx_enable_timing(solo_b200_rx* q, uint32_t ts_per_index, int max_arrivals) {
+    if (!q || ts_per_index == 0 || max_arrivals < 1 || q->t.transit) {
+        snprintf(g_err, sizeof g_err, "rx_enable_timing: bad argument (ts_per_index %u, max_arrivals %d%s)", ts_per_index,
+                 max_arrivals, q && q->t.transit ? ", timing already enabled" : "");
+        return -1;
+    }
+    CK(cudaSetDevice(q->device));
+    RxTiming t = {};
+    t.ts_per_index = ts_per_index;
+    t.max_arrivals = max_arrivals;
+    for (u32 top = (u32)(q->q.n - 1); top; top >>= 8) t.passes++;
+    const size_t n = (size_t)q->q.n, na = (size_t)max_arrivals, nh = 256 * (size_t)rx_sort_tiles(max_arrivals);
+    bool ok = cudaMalloc(&t.transit, 4 * n) == cudaSuccess && cudaMalloc(&t.jitter, 4 * n) == cudaSuccess &&
+              cudaMalloc(&t.highest, 8 * n) == cudaSuccess && cudaMalloc(&t.received, 4 * n) == cudaSuccess &&
+              cudaMalloc(&t.margin, 4 * RX_MARGIN_BINS * n) == cudaSuccess;
+    for (int b = 0; b < 2; b++) ok = ok && cudaMalloc(&t.key[b], 4 * na) == cudaSuccess && cudaMalloc(&t.pos[b], 4 * na) == cudaSuccess;
+    ok = ok && cudaMalloc(&t.hist, 4 * nh) == cudaSuccess;
+    ok = ok && cudaMemsetAsync(t.transit, 0, 4 * n, q->st) == cudaSuccess && cudaMemsetAsync(t.jitter, 0, 4 * n, q->st) == cudaSuccess &&
+         cudaMemsetAsync(t.highest, 0, 8 * n, q->st) == cudaSuccess && cudaMemsetAsync(t.received, 0, 4 * n, q->st) == cudaSuccess &&
+         cudaMemsetAsync(t.margin, 0, 4 * RX_MARGIN_BINS * n, q->st) == cudaSuccess && cudaStreamSynchronize(q->st) == cudaSuccess;
+    if (!ok) {
+        snprintf(g_err, sizeof g_err, "rx_enable_timing: %s", cudaGetErrorString(cudaGetLastError()));
+        cudaFree(t.transit); cudaFree(t.jitter); cudaFree(t.highest); cudaFree(t.received); cudaFree(t.margin);
+        cudaFree(t.key[0]); cudaFree(t.key[1]); cudaFree(t.pos[0]); cudaFree(t.pos[1]); cudaFree(t.hist);
+        return -1;
+    }
+    q->t = t;
+    return 0;
+}
+
+// the timed insert on st: the three insert passes, the keys pass, the sort passes and the walk; nothing for no arrivals
+static int rx_insert_timed_launch(solo_b200_rx* r, const RxArrivals& A, const u32* arrival, cudaStream_t st) {
+    if (A.n == 0) return 0;
+    if (int e = rx_insert_launch(r, A, st)) return e;
+    RxTiming& T = r->t;
+    const unsigned g = (unsigned)(((long long)A.n + SB_RX_THREADS - 1) / SB_RX_THREADS), tiles = (unsigned)rx_sort_tiles(A.n);
+    sb_rx_timing_keys_kernel<<<g, SB_RX_THREADS, 0, st>>>(r->q, T, A);
+    if (int e = launched("sb_rx_timing_keys_kernel")) return e;
+    int src = 0;
+    for (int p = 0; p < T.passes; p++, src ^= 1) {
+        sb_rx_sort_hist_kernel<<<tiles, SB_RX_SORT_THREADS, 0, st>>>(T.key[src], T.hist, A.n, 8 * p);
+        if (int e = launched("sb_rx_sort_hist_kernel")) return e;
+        sb_rx_sort_scan_kernel<<<1, SB_RX_SCAN_THREADS, 0, st>>>(T.hist, 256 * (int)tiles);
+        if (int e = launched("sb_rx_sort_scan_kernel")) return e;
+        sb_rx_sort_scatter_kernel<<<tiles, SB_RX_SORT_THREADS, 0, st>>>(T.key[src], T.pos[src], T.key[src ^ 1], T.pos[src ^ 1],
+                                                                         T.hist, A.n, 8 * p);
+        if (int e = launched("sb_rx_sort_scatter_kernel")) return e;
+    }
+    sb_rx_timing_walk_kernel<<<g, SB_RX_THREADS, 0, st>>>(T, T.key[src], T.pos[src], A, arrival);
+    return launched("sb_rx_timing_walk_kernel");
+}
+static int rx_insert_timed_args_ok(solo_b200_rx* q, const void* arrival, int n_arrivals) {
+    if (!q->t.transit) { snprintf(g_err, sizeof g_err, "rx_insert_timed: timing is not enabled"); return 0; }
+    if (n_arrivals > q->t.max_arrivals || (n_arrivals > 0 && !arrival)) {
+        snprintf(g_err, sizeof g_err, "rx_insert_timed: bad argument (n_arrivals %d, max_arrivals %d)", n_arrivals, q->t.max_arrivals);
+        return 0;
+    }
+    return 1;
+}
+
+int solo_b200_rx_insert_timed_device(solo_b200_rx* q, const int32_t* d_stream, const uint32_t* d_index, const uint8_t* d_desc,
+                                     const int32_t* d_off, const int32_t* d_len, const uint32_t* d_arrival, int n_arrivals,
+                                     const uint8_t* d_payload, int64_t payload_bytes, void* cuda_stream) {
+    if (!rx_insert_args_ok(q, d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes) ||
+        !rx_insert_timed_args_ok(q, d_arrival, n_arrivals))
+        return -1;
+    if (n_arrivals == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    const RxArrivals A = {d_stream, d_index, d_desc, d_off, d_len, n_arrivals, d_payload, payload_bytes};
+    return rx_insert_timed_launch(q, A, d_arrival, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_rx_insert_timed_host(solo_b200_rx* q, const int32_t* stream, const uint32_t* index, const uint8_t* desc,
+                                   const int32_t* off, const int32_t* len, const uint32_t* arrival, int n_arrivals,
+                                   const uint8_t* payload, int64_t payload_bytes) {
+    if (!rx_insert_args_ok(q, stream, index, desc, off, len, n_arrivals, payload, payload_bytes) ||
+        !rx_insert_timed_args_ok(q, arrival, n_arrivals))
+        return -1;
+    if (n_arrivals == 0) return 0;
+    CK(cudaSetDevice(q->device));
+    const size_t na = (size_t)n_arrivals;
+    RxArrivals A = {nullptr, nullptr, nullptr, nullptr, nullptr, n_arrivals, nullptr, payload_bytes};
+    const u32* d_arrival;
+    Staging s(q->st, "rx_insert_timed");
+    s.span(A.stream, stream, nullptr, 4 * na);
+    s.span(A.index, index, nullptr, 4 * na);
+    s.span(A.desc, desc, nullptr, na);
+    s.span(A.off, off, nullptr, 4 * na);
+    s.span(A.len, len, nullptr, 4 * na);
+    s.span(d_arrival, arrival, nullptr, 4 * na);
+    s.span(A.payload, payload, nullptr, (size_t)payload_bytes);
+    s.run([&] { return rx_insert_timed_launch(q, A, d_arrival, q->st); });
+    return s.finish();
+}
+
+int solo_b200_rx_timing(solo_b200_rx* q, uint32_t* jitter, uint64_t* highest, uint32_t* received, uint32_t* margin,
+                        void* cuda_stream) {
+    if (!q || !q->t.transit) { snprintf(g_err, sizeof g_err, "rx_timing: %s", q ? "timing is not enabled" : "bad argument"); return -1; }
+    CK(cudaSetDevice(q->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const size_t n = (size_t)q->q.n;
+    if (jitter) CK(cudaMemcpyAsync(jitter, q->t.jitter, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (highest) CK(cudaMemcpyAsync(highest, q->t.highest, 8 * n, cudaMemcpyDeviceToHost, st));
+    if (received) CK(cudaMemcpyAsync(received, q->t.received, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (margin) CK(cudaMemcpyAsync(margin, q->t.margin, 4 * RX_MARGIN_BINS * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (jitter)
+        for (size_t s = 0; s < n; s++) jitter[s] >>= 4;     // the state keeps 1/16 units (RFC 3550 A.8)
+    return 0;
+}
+
 static int rx_pull_args_ok(solo_b200_rx* q, const void* bits, int cap, const void* nbytes, const void* lostflag) {
     if (!q || !bits || !nbytes || !lostflag) { snprintf(g_err, sizeof g_err, "rx_pull: bad argument"); return 0; }
     if (cap < 2 * q->q.desc_cap) { snprintf(g_err, sizeof g_err, "rx_pull: cap %d is below 2 * desc_cap = %d", cap, 2 * q->q.desc_cap); return 0; }
@@ -1615,11 +1887,13 @@ int solo_b200_rx_pull_host(solo_b200_rx* q, const uint32_t* play, uint8_t* bits,
 }
 
 // The reset of either queue (Q solo_b200_rx or solo_b200_tx): a list of distinct streams of the queue, nothing done when it
-// is refused, then `kernel` (block threads per block) on the caller's stream, which the call synchronises.
+// is refused, then `kernel` (block threads per block) on the caller's stream, which the call synchronises.  `also`, when
+// given, launches more work on the same device list of streams after it.
 extern "C++" {
 template <class Q, class D>
 static int queue_reset(Q* q, const i32* streams, const u32* start, int n, cudaStream_t st,
-                       void (*kernel)(D, const i32*, const u32*, int), int block, const char* who) {
+                       void (*kernel)(D, const i32*, const u32*, int), int block, const char* who,
+                       int (*also)(Q*, const i32*, int, cudaStream_t) = nullptr) {
     if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "%s: bad argument", who); return -1; }
     std::vector<u8> seen((size_t)q->q.n, 0);
     for (int i = 0; i < n; i++) {
@@ -1634,14 +1908,23 @@ static int queue_reset(Q* q, const i32* streams, const u32* start, int n, cudaSt
     s.span(d_start, start, nullptr, 4 * (size_t)n);
     s.run([&] {
         kernel<<<(n + block - 1) / block, block, 0, st>>>(q->q, d_streams, d_start, n);
-        return launched(who);
+        if (int e = launched(who)) return e;
+        return also ? also(q, d_streams, n, st) : 0;
     });
     return s.finish();
 }
 }  // extern "C++"
 
+// a timed queue's reset also clears the listed streams' timing state: one more launch
+static int rx_reset_timing(solo_b200_rx* q, const i32* d_streams, int n, cudaStream_t st) {
+    if (!q->t.transit) return 0;
+    sb_rx_timing_reset_kernel<<<(n + SB_RX_THREADS - 1) / SB_RX_THREADS, SB_RX_THREADS, 0, st>>>(q->t, d_streams, n);
+    return launched("sb_rx_timing_reset_kernel");
+}
+
 int solo_b200_rx_reset(solo_b200_rx* q, const int32_t* streams, const uint32_t* start, int n, void* cuda_stream) {
-    return queue_reset(q, streams, start, n, (cudaStream_t)cuda_stream, sb_rx_reset_kernel, SB_RX_THREADS, "rx_reset");
+    return queue_reset(q, streams, start, n, (cudaStream_t)cuda_stream, sb_rx_reset_kernel, SB_RX_THREADS, "rx_reset",
+                       rx_reset_timing);
 }
 
 int solo_b200_rx_stats(solo_b200_rx* q, uint32_t* counters, uint64_t* bad_stream, void* cuda_stream) {
