@@ -32,6 +32,15 @@ def lib(emu=None):
         L.hs_nsq_run.argtypes = [C.c_int] * 4 + [C.c_void_p] * 4
         L.hs_level.argtypes = [C.c_longlong, C.c_int]
         L.hs_row_level.argtypes = [C.c_void_p, C.c_int]
+        vp, ci = C.c_void_p, C.c_int
+        L.mix_model.argtypes = [vp, vp, ci, ci] + [vp] * 4 + [ci, ci, vp]
+        L.rx_model_insert.argtypes = [ci, ci, ci] + [vp] * 13 + [ci, vp, C.c_int64]
+        L.rx_model_pull.argtypes = [ci, ci, ci] + [vp] * 6 + [vp, ci, vp, vp]
+        L.rx_model_merge.argtypes = [ci, ci, vp, vp]
+        L.rx_model_timing.argtypes = [ci, ci, C.c_uint32] + [vp] * 12 + [ci, C.c_int64]
+        L.tx_model_pack.argtypes = [ci, vp, ci, vp] + [vp] * 9
+        L.tx_model_pack.restype = ci
+        L.tx_model_contributors.argtypes = [vp, vp, ci, ci, vp, vp, ci, vp, vp]
         if emu:
             L.hs_set_emu_nsq.argtypes = [C.c_int]
             L.hs_enc_encode_pair.argtypes = [C.c_void_p] * 6 + [C.c_int] + [C.c_void_p] * 3
@@ -152,3 +161,138 @@ class SimDecoder:
         if self.h:
             self.L.hs_dec_destroy(self.h)
             self.h = None
+
+
+# ---- the server side: mixer, receive queue, send queue (server.cpp) -----------------------------------------------------
+M32 = 1 << 32
+
+
+def _ptrs(*arrays):
+    return [x.ctypes.data for x in arrays]
+
+
+def mix_model(pcm, level, flags, room_start, members, k, out):
+    """The two mix kernels over rows pcm int16 [n, spp] into out (rows of streams in no room are left as they are).
+    Returns (out, talkers int32 [rooms, k])."""
+    R = len(room_start) - 1
+    talkers = np.full((R, k), 12345, np.int32)
+    n, spp = pcm.shape
+    lib().mix_model(*_ptrs(pcm, out), spp, n, *_ptrs(level, flags, room_start, members), R, k, talkers.ctypes.data)
+    return out, talkers
+
+
+def contributors(room_start, members, k, talkers, level, n):
+    """sb_mix_contributors_kernel's lists: (csrc int32 [n, k], csrc_level uint8 [n, k])."""
+    csrc, lvl = np.zeros((n, k), np.int32), np.zeros((n, k), np.uint8)
+    rs, mb, tk, lv = (np.ascontiguousarray(x, t) for x, t in ((room_start, np.int32), (members, np.int32),
+                                                                 (talkers, np.int32), (level, np.uint8)))
+    lib().tx_model_contributors(*_ptrs(rs, mb), len(rs) - 1, k, *_ptrs(tk, lv), n, *_ptrs(csrc, lvl))
+    return csrc, lvl
+
+
+def merge(n1, n2):
+    """The shared merge rule of descriptions of n1 / n2 bytes (0 = missing): (row length, nbytes int16 [2], lostflag)."""
+    nb, lf = np.zeros(2, np.int16), np.zeros(1, np.int32)
+    row = lib().rx_model_merge(n1, n2, *_ptrs(nb, lf))
+    return row, nb, int(lf[0])
+
+
+class SimRx:
+    """A receive queue of n streams (solo_b200_rx) in the device layout of solo_b200.cu's RxDev, and of RxTiming once
+    timing is enabled, advanced by the host build of sb_rx.cuh.  Same call shapes as solo_b200.RxQueue."""
+
+    def __init__(self, n, depth, desc_cap):
+        self.L, self.n, self.depth, self.desc_cap = lib(), n, depth, desc_cap
+        self.last = np.full(n, M32 - 1, np.uint32)
+        self.idx = np.zeros(n * depth, np.uint32)
+        self.len = np.zeros(n * depth * 2, np.uint16)
+        self.elect = np.zeros(n * depth * 2, np.uint64)
+        self.rep = np.full(n * depth, 0xFFFFFFFF, np.uint32)
+        self.cnt = np.zeros((n, 8), np.uint32)
+        self.bad = np.zeros(1, np.uint64)
+        self.store = np.zeros(n * depth * 2 * desc_cap + 16, np.uint8)
+        self.ts = None
+
+    def enable_timing(self, ts_per_index):
+        self.ts = int(ts_per_index)
+        self.transit = np.zeros(self.n, np.uint32)
+        self.jitter = np.zeros(self.n, np.uint32)          # 1/16 units, as the device keeps it
+        self.highest = np.zeros(self.n, np.uint64)
+        self.received = np.zeros(self.n, np.uint32)
+        self.margin = np.zeros((self.n, 8), np.uint32)
+
+    def insert(self, stream, index, desc, off, lens, payload, arrival=None):
+        """arrival (receive times) makes it a timed insert, which needs enable_timing first."""
+        a = [np.ascontiguousarray(x, t) for x, t in ((stream, np.int32), (index, np.uint32), (desc, np.uint8),
+                                                     (off, np.int32), (lens, np.int32), (payload, np.uint8))]
+        na, pay = len(a[0]), a[5]
+        self.L.rx_model_insert(self.n, self.depth, self.desc_cap, *_ptrs(self.last, self.idx, self.len, self.elect, self.rep,
+                                                                         self.cnt, self.bad, self.store),
+                               *_ptrs(*a[:5]), na, pay.ctypes.data, pay.size)
+        if arrival is not None:     # as rx_insert_timed_launch: the insert passes, then the timing of the same arrays
+            assert self.ts is not None, "timing is not enabled"
+            ar = np.ascontiguousarray(arrival, np.uint32)
+            assert ar.shape == (na,)
+            self.L.rx_model_timing(self.n, self.desc_cap, self.ts, *_ptrs(self.last, self.transit, self.jitter, self.highest,
+                                                                          self.received, self.margin),
+                                   *_ptrs(*a[:5], ar), na, pay.size)
+
+    def pull(self, play=None, cap=None):
+        """-> (bits uint8 [n, cap], nbytes int16 [n, 2], lostflag int32 [n]); cap defaults to 2 * desc_cap."""
+        cap = 2 * self.desc_cap if cap is None else cap
+        bits = np.zeros((self.n, cap), np.uint8)
+        nb = np.zeros((self.n, 2), np.int16)
+        lf = np.zeros(self.n, np.int32)
+        p = np.ascontiguousarray(play, np.uint32) if play is not None else None
+        self.L.rx_model_pull(self.n, self.depth, self.desc_cap, *_ptrs(self.last, self.idx, self.len, self.cnt, self.store),
+                             p.ctypes.data if p is not None else None, bits.ctypes.data, cap, *_ptrs(nb, lf))
+        return bits, nb, lf
+
+    def reset(self, streams, start):
+        """As solo_b200_rx_reset: the listed streams play start[i] next, with empty slots, zero counters and, on a timed
+        queue, cleared timing."""
+        for s, t in zip(streams, start):
+            self.last[s] = (int(t) - 1) % M32
+            self.cnt[s] = 0
+            self.len[s * 2 * self.depth:(s + 1) * 2 * self.depth] = 0
+        if self.ts is not None:
+            for x in (self.transit, self.jitter, self.highest, self.received, self.margin):
+                x[np.asarray(streams, np.int64)] = 0
+
+    def stats(self):
+        """(counters uint32 [n, 8], arrivals for streams outside [0, n))."""
+        return self.cnt.copy(), int(self.bad[0])
+
+    def timing(self):
+        """(jitter >> 4, highest, received, margin), as solo_b200_rx_timing reports them."""
+        return self.jitter >> 4, self.highest.copy(), self.received.copy(), self.margin.copy()
+
+
+class SimTx:
+    """A send queue of n streams (solo_b200_tx) in the device layout of solo_b200.cu's TxDev, advanced by the host build
+    of sb_tx.cuh."""
+
+    def __init__(self, n):
+        self.L, self.n = lib(), n
+        self.next = np.zeros(n, np.uint32)
+        self.cnt = np.zeros((n, 4), np.uint32)
+
+    def pack(self, bits, nbytes):
+        """-> (payload bytes, [(stream, index, desc, off, len)])."""
+        bits = np.ascontiguousarray(bits, np.uint8)
+        nbytes = np.ascontiguousarray(nbytes, np.int16)
+        e = 2 * self.n
+        payload = np.zeros(self.n * bits.shape[1], np.uint8)
+        ent = [np.zeros(e, t) for t in (np.int32, np.uint32, np.uint8, np.int32, np.int32)]
+        total = C.c_int64()
+        c = self.L.tx_model_pack(self.n, bits.ctypes.data, bits.shape[1], *_ptrs(nbytes, self.next, self.cnt, payload, *ent),
+                                 C.byref(total))
+        return bytes(payload[:total.value]), list(zip(*(x[:c].tolist() for x in ent)))
+
+    def reset(self, streams, start):
+        for s, t in zip(streams, start):
+            self.next[s] = int(t) % M32
+            self.cnt[s] = 0
+
+    def stats(self):
+        return self.cnt.copy()

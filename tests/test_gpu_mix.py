@@ -1,5 +1,5 @@
 """The conference mixer on the GPU (sb_mix_select_kernel + sb_mix_kernel through solo_b200_mix_host / _device), at 0
-tolerance against the numpy restatement of tests/test_mix.py: random layouts at every row length, a 65 536-stream layout,
+tolerance against the numpy restatement of tests/server_ref.py: random layouts at every row length, a 65 536-stream layout,
 argument checking, out-of-range members on the device path, 32 kHz rows, and a whole MCU tick (decode, activity, mix,
 downlink encode) on the device against the same tick through host calls and numpy mixing."""
 import os
@@ -9,7 +9,7 @@ import pytest
 
 from tests.golden import make_golden_32k as mk
 from tests.parity import sb  # noqa: F401  (fixture)
-from tests.test_mix import POISON, csr, numpy_mix
+from tests.server_ref import POISON, csr, mixed_layout, numpy_mix, to_dev
 from tests.util import GOLDEN, load_clip, loss_flags, receive, signal_classes
 
 pytestmark = pytest.mark.gpu
@@ -19,11 +19,6 @@ CAP = 256
 def dev():
     import torch
     return torch.device("cuda", 0)
-
-
-def to_dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev())
 
 
 def mix_on_device(sb, pcm, level, flags, room_start, members, n_rooms, k, out_init):
@@ -67,18 +62,6 @@ def test_random_layouts_host_and_device(sb, spp):
         rs, mb = csr(rooms)
         out, t = mix_on_device(sb, pcm, level, flags, rs, mb, len(rooms), k, np.full((n, spp), POISON, np.int16))
         assert np.array_equal(t, wt) and np.array_equal(out, want), k
-
-
-def mixed_layout(n=65536, seed=1):
-    """8 192 rooms of 4, 64 rooms of 256 and one room of 12 000 over a permutation of the streams; 4 384 in no room."""
-    perm = np.random.Generator(np.random.PCG64(seed)).permutation(n).astype(np.int32)
-    sizes = [4] * 8192 + [256] * 64 + [12000]
-    rooms, o = [], 0
-    for s in sizes:
-        rooms.append(perm[o:o + s])
-        o += s
-    assert n - o == 4384
-    return rooms, perm[o:]
 
 
 def test_65536_streams(sb):

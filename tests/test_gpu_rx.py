@@ -1,83 +1,22 @@
 """The receive queue on the GPU (sb_rx_elect / classify / commit / pull kernels through solo_b200_rx_*), at 0 tolerance
-against the restatement of tests/test_rx.py: seeded arrival processes at N = 257 and at N = 65 536 (a 1 024-stream sample
+against the restatement of tests/server_ref.py: seeded arrival processes at N = 257 and at N = 65 536 (a 1 024-stream sample
 modelled), both entry-point forms, NULL and explicit play, arrival order, malformed device inputs, the launch budget, and a
 whole receive -> decode run on the device that reproduces the reference decoder's PCM under golden.npz's 50 % loss."""
 import numpy as np
 import pytest
 
 from tests.parity import sb  # noqa: F401  (fixture)
-from tests.test_rx import M32, PyRx, make_ops
+from tests.server_ref import DeviceForm, HostForm, M32, PyRx, check_pull, make_ops, replay, run_model, to_dev
 from tests.util import load_golden
 
 pytestmark = pytest.mark.gpu
 
 
-def to_dev(a):
-    import torch
-    return torch.from_numpy(np.array(a)).to(torch.device("cuda", 0))
-
-
-class DeviceForm:
-    """RxQueue driven through insert_device / pull_device on the current torch stream."""
-
-    def __init__(self, sb, n, depth, desc_cap):
-        self.q, self.n, self.cap = sb.RxQueue(n, depth, desc_cap), n, 2 * desc_cap
-
-    def insert(self, stream, index, desc, off, lens, payload):
-        import torch
-        a = [to_dev(x) for x in (stream, index.view(np.int32), desc, off, lens, payload)]
-        self.q.insert_device(*(x.data_ptr() for x in a[:5]), len(stream), a[5].data_ptr(), payload.size,
-                             torch.cuda.current_stream().cuda_stream)
-
-    def pull(self, play=None):
-        import torch
-        d_bits = torch.zeros((self.n, self.cap), dtype=torch.uint8, device="cuda")
-        d_nb = torch.zeros((self.n, 2), dtype=torch.int16, device="cuda")
-        d_lf = torch.zeros(self.n, dtype=torch.int32, device="cuda")
-        d_play = to_dev(np.asarray(play, np.uint32).view(np.int32)) if play is not None else None
-        self.q.pull_device(d_play.data_ptr() if d_play is not None else 0, d_bits.data_ptr(), self.cap, d_nb.data_ptr(),
-                           d_lf.data_ptr(), torch.cuda.current_stream().cuda_stream)
-        return d_bits.cpu().numpy(), d_nb.cpu().numpy(), d_lf.cpu().numpy()
-
-    def reset(self, streams, start):
-        self.q.reset(streams, start)
-
-    def stats(self):
-        import torch
-        torch.cuda.synchronize()
-        return self.q.stats()
-
-
-class HostForm(DeviceForm):
-    """The same through solo_b200_rx_insert_host (raw arrays, so malformed offsets reach it) and pull_host."""
-
-    def insert(self, stream, index, desc, off, lens, payload):
-        a = [np.ascontiguousarray(x) for x in (stream, index, desc, off, lens, payload)]
-        from solo_b200.api import lib
-        r = lib().solo_b200_rx_insert_host(self.q.h, *(x.ctypes.data for x in a[:5]), len(stream), a[5].ctypes.data,
-                                           a[5].size)
-        assert r == 0
-
-    def pull(self, play=None):
-        return self.q.pull(play, cap=self.cap)
-
-
 def check_against_model(impl, ops, n, depth, desc_cap):
     """Replay ops on impl; rows (up to nbytes[0]), nbytes, lostflag and counters must equal the restatement's."""
-    m = PyRx(n, depth, desc_cap)
-    for op in ops:
-        if op[0] == "insert":
-            impl.insert(*op[1:])
-            m.insert(*op[1:])
-        elif op[0] == "reset":
-            impl.reset(op[1], op[2])
-            m.reset(op[1], op[2])
-        else:
-            bits, nb, lf = impl.pull(op[1])
-            rows, wnb, wlf = m.pull(op[1])
-            assert np.array_equal(nb, wnb) and np.array_equal(lf, wlf)
-            for s, row in enumerate(rows):
-                assert bytes(bits[s, :len(row)]) == row, s
+    m, want = run_model(ops, n, depth, desc_cap)
+    for got, w in zip(replay(impl, ops), want):
+        check_pull(got, w)
     cnt, bad = impl.stats()
     assert np.array_equal(cnt.astype(np.int64), m.cnt) and bad == m.bad
     return m

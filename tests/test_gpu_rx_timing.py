@@ -1,95 +1,69 @@
 """Receive-queue timing on the GPU (sb_rx_timing_keys / sort / walk kernels through solo_b200_rx_insert_timed_* and
-solo_b200_rx_timing), at 0 tolerance against the host model (sim.SimRxTiming, the same sb_rx.cuh rules in array order):
-seeded arrival processes at N = 257 through both entry points, the rx_time.py traffic at N = 65 536, every arrival on
+solo_b200_rx_timing), at 0 tolerance against the host model (a timed sim.SimRx, the same sb_rx.cuh rules in array
+order): seeded arrival processes at N = 257 through both entry points, the rx_time.py traffic at N = 65 536, every arrival on
 one stream at n = max_arrivals, garbage arrays, repeatability, reset, and a send queue -> network -> receive queue
 loopback with known delays whose jitter has a closed form.  A timed queue and an untimed one fed the same arrays must
 pull the same rows and report the same counters."""
 import numpy as np
 import pytest
 
-from tests.hostsim.rx_timing import SimRxTiming
+from tests.hostsim.sim import SimRx
 from tests.parity import sb  # noqa: F401  (fixture)
-from tests.test_rx import M32, PyRx, make_ops
-from tests.test_rx_timing import add_arrivals
+from tests.server_ref import DeviceForm, HostForm, M32, PyRx, add_arrivals, make_ops, replay, rx_time_traffic
 from tests.util import load_golden
 
 pytestmark = pytest.mark.gpu
 
 
-def to_dev(a):
-    import torch
-    a = np.ascontiguousarray(a)
-    if a.dtype == np.uint32:
-        a = a.view(np.int32)
-    return torch.from_numpy(a).to(torch.device("cuda", 0))
-
-
-def insert_device(q, stream, index, desc, off, lens, payload, arrival=None):
-    import torch
-    d = [to_dev(x) for x in (stream, index, desc, off, lens, payload)]
-    da = to_dev(arrival) if arrival is not None else None
-    q.insert_device(*(x.data_ptr() for x in d[:5]), len(stream), d[5].data_ptr(), payload.size,
-                    torch.cuda.current_stream().cuda_stream, d_arrival=da.data_ptr() if da is not None else None)
-    torch.cuda.synchronize()
-
-
-def insert_host(q, stream, index, desc, off, lens, payload, arrival=None):
-    """The raw host entry points, so that malformed offsets reach them."""
-    from solo_b200.api import lib
-    a = [np.ascontiguousarray(x) for x in (stream, index, desc, off, lens, payload)]
-    if arrival is None:
-        r = lib().solo_b200_rx_insert_host(q.h, *(x.ctypes.data for x in a[:5]), len(stream), a[5].ctypes.data, a[5].size)
-    else:
-        ar = np.ascontiguousarray(arrival, np.uint32)
-        r = lib().solo_b200_rx_insert_timed_host(q.h, *(x.ctypes.data for x in a[:5]), ar.ctypes.data, len(stream),
-                                                 a[5].ctypes.data, a[5].size)
-    assert r == 0
-
-
 def check_timing(q, m):
-    for got, want in zip(q.timing(), m.read()):
+    for got, want in zip(q.timing(), m.timing()):
         assert got.dtype == want.dtype and np.array_equal(got, want)
 
 
-def run_pair(sb, ops, n, depth, desc_cap, ts, insert, max_arrivals):
-    """Replay timed ops on a timed queue, an untimed queue and the model.  Pulls and counters of the two queues must
-    agree, and the timed queue's timing must equal the model's after every insert.  Returns the timed queue."""
-    timed, plain = sb.RxQueue(n, depth, desc_cap), sb.RxQueue(n, depth, desc_cap)
+def timed_model(n, depth, desc_cap, ts):
+    m = SimRx(n, depth, desc_cap)
+    m.enable_timing(ts)
+    return m
+
+
+def run_pair(sb, ops, n, depth, desc_cap, ts, form, max_arrivals):
+    """Replay timed ops on a timed queue, an untimed queue and the host model.  Pulls and counters of the two queues must
+    agree and equal the restatement's counters, and the timed queue's timing must equal the model's after every insert.
+    Returns the timed queue."""
+    timed, plain = form(sb, n, depth, desc_cap), form(sb, n, depth, desc_cap)
     timed.enable_timing(ts, max_arrivals)
-    q, m = PyRx(n, depth, desc_cap), SimRxTiming(n, desc_cap, ts)
+    q, m = PyRx(n, depth, desc_cap), timed_model(n, depth, desc_cap, ts)
     for op in ops:
         if op[0] == "insert":
-            stream, index, desc, off, lens, payload, arrival = op[1:]
-            m.insert(np.array(q.last, np.uint32), stream, index, desc, off, lens, arrival, payload.size)
-            q.insert(stream, index, desc, off, lens, payload)
-            insert(timed, stream, index, desc, off, lens, payload, arrival)
-            insert(plain, stream, index, desc, off, lens, payload)
+            q.insert(*op[1:7])
+            m.insert(*op[1:])
+            timed.insert(*op[1:])
+            plain.insert(*op[1:7])
             check_timing(timed, m)
         elif op[0] == "reset":
-            for x in (timed, plain):
+            for x in (timed, plain, q, m):
                 x.reset(op[1], op[2])
-            q.reset(op[1], op[2])
-            m.reset(op[1])
             check_timing(timed, m)
         else:
-            a, b = timed.pull(op[1], cap=2 * desc_cap), plain.pull(op[1], cap=2 * desc_cap)
+            a, b = timed.pull(op[1]), plain.pull(op[1])
             q.pull(op[1])
+            m.pull(op[1])
             assert all(np.array_equal(x, y) for x, y in zip(a, b))
     ca, cb = timed.stats(), plain.stats()
     assert np.array_equal(ca[0], cb[0]) and ca[1] == cb[1]
     assert np.array_equal(ca[0].astype(np.int64), q.cnt)
     plain.close()
-    return timed, m
+    return timed
 
 
-@pytest.mark.parametrize("insert", [insert_device, insert_host])
+@pytest.mark.parametrize("form", [DeviceForm, HostForm], ids=["insert_device", "insert_host"])
 @pytest.mark.parametrize("explicit_play", [False, True])
-def test_timed_queue_equals_model_257(sb, insert, explicit_play):
+def test_timed_queue_equals_model_257(sb, form, explicit_play):
     n, depth, desc_cap, ts = 257, 8, 128, 640
     rng = np.random.Generator(np.random.PCG64(257 + explicit_play))
     ops, _ = make_ops(rng, n, depth, desc_cap, 16, explicit_play=explicit_play)
     ops = add_arrivals(rng, ops, ts, M32 - 7000)
-    q, m = run_pair(sb, ops, n, depth, desc_cap, ts, insert, 4096)
+    q = run_pair(sb, ops, n, depth, desc_cap, ts, form, 4096)
     jitter, highest, received, margin = q.timing()
     assert (highest >> np.uint64(32)).max() >= 1 and (margin.sum(0) > 0).all() and received.sum() > 0
     q.close()
@@ -102,64 +76,36 @@ def test_host_and_device_forms_agree_and_repeat(sb):
     ops, _ = make_ops(rng, n, depth, desc_cap, 8)
     ops = add_arrivals(rng, ops, ts, 5)
     res = []
-    for insert in (insert_host, insert_device, insert_device):
-        q = sb.RxQueue(n, depth, desc_cap)
+    for form in (HostForm, DeviceForm, DeviceForm):
+        q = form(sb, n, depth, desc_cap)
         q.enable_timing(ts, 8192)
-        for op in ops:
-            if op[0] == "insert":
-                insert(q, *op[1:7], op[7])
-            elif op[0] == "reset":
-                q.reset(op[1], op[2])
-            else:
-                q.pull(op[1], cap=2 * desc_cap)
+        replay(q, ops)
         res.append(q.timing())
         q.close()
     for r in res[1:]:
         assert all(np.array_equal(x, y) for x, y in zip(r, res[0]))
 
 
-def rx_time_traffic(N, rng):
-    """tools/rx_time.py's tick: both descriptions of every stream's golden-sized packet, 1 % duplicated, 10 % one tick
-    early, shuffled.  Returns (stream, desc, lens, payload, off, early)."""
-    g = load_golden()
-    P = g["fix_nbytes"].shape[0]
-    s = np.repeat(np.arange(N, dtype=np.int32), 2)
-    d = np.tile(np.array([1, 2], np.uint8), N)
-    p = s % P
-    n0, n1 = g["fix_nbytes"][p, 0].astype(np.int32), g["fix_nbytes"][p, 1].astype(np.int32)
-    lens = np.where(d == 1, n0 - n1, n1).astype(np.int32)
-    src = np.where(d == 1, 0, n0 - n1)
-    dup = rng.choice(2 * N, 2 * N // 100, replace=False)
-    s, d, lens, src, p = (np.concatenate([x, x[dup]]) for x in (s, d, lens, src, p))
-    early = rng.random(len(s)) < 0.10
-    order = rng.permutation(len(s))
-    s, d, lens, src, p, early = (x[order] for x in (s, d, lens, src, p, early))
-    off = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int32)
-    payload = np.concatenate([g["fix_bits"][pi, si:si + li] for pi, si, li in zip(p, src, lens)]).astype(np.uint8)
-    return s, d, lens, payload, off, early.astype(np.int64)
-
-
 def test_timed_queue_equals_model_65536(sb):
     """65 536 streams and about 132 k arrivals per tick (the rx_time.py traffic) with receive times: index * 640 plus a
     per-arrival delay, the clock wrapping during the run.  Every stream's timing is compared."""
-    N, depth, desc_cap, cap, ts = 65536, 8, 128, 256, 640
+    N, depth, desc_cap, ts = 65536, 8, 128, 640
     rng = np.random.Generator(np.random.PCG64(65536))
     s, d, lens, payload, off, early = rx_time_traffic(N, rng)
     A = len(s)
-    timed, plain = sb.RxQueue(N, depth, desc_cap), sb.RxQueue(N, depth, desc_cap)
+    timed, plain = DeviceForm(sb, N, depth, desc_cap), DeviceForm(sb, N, depth, desc_cap)
     timed.enable_timing(ts, A)
-    m = SimRxTiming(N, desc_cap, ts)
-    last = np.full(N, M32 - 1, np.uint32)
+    m = timed_model(N, depth, desc_cap, ts)
     for t in range(4):
         index = ((t + early) % M32).astype(np.uint32)
         arrival = ((M32 - 2 * ts + index.astype(np.int64) * ts + rng.integers(0, 2 * ts, A)) % M32).astype(np.uint32)
-        m.insert(last, s, index, d, off, lens, arrival, payload.size)
-        insert_device(timed, s, index, d, off, lens, payload, arrival)
-        insert_device(plain, s, index, d, off, lens, payload)
+        m.insert(s, index, d, off, lens, payload, arrival)
+        timed.insert(s, index, d, off, lens, payload, arrival)
+        plain.insert(s, index, d, off, lens, payload)
         check_timing(timed, m)
-        a, b = timed.pull(cap=cap), plain.pull(cap=cap)
+        a, b = timed.pull(), plain.pull()
+        m.pull()
         assert all(np.array_equal(x, y) for x, y in zip(a, b))
-        last = last + np.uint32(1)
     ca, cb = timed.stats(), plain.stats()
     assert np.array_equal(ca[0], cb[0]) and ca[1] == cb[1]
     jitter, highest, received, margin = timed.timing()
@@ -172,9 +118,9 @@ def test_all_arrivals_on_one_stream(sb, N, target):
     the sort holds every arrival, and its walk follows array order."""
     desc_cap, ts, A = 64, 640, 140000
     rng = np.random.Generator(np.random.PCG64(N))
-    q = sb.RxQueue(N, 32, desc_cap)
+    q = DeviceForm(sb, N, 32, desc_cap)
     q.enable_timing(ts, A)
-    m = SimRxTiming(N, desc_cap, ts)
+    m = timed_model(N, 32, desc_cap, ts)
     stream = np.full(A, target, np.int32)
     index = (np.arange(A) // 2 + rng.integers(-40, 40, A)) % M32
     index = index.astype(np.uint32)
@@ -183,8 +129,8 @@ def test_all_arrivals_on_one_stream(sb, N, target):
     off = rng.integers(0, 60, A).astype(np.int32)
     payload = rng.integers(0, 256, 64).astype(np.uint8)
     arrival = ((index.astype(np.int64) * ts + rng.integers(0, 3000, A)) % M32).astype(np.uint32)
-    m.insert(np.full(N, M32 - 1, np.uint32), stream, index, desc, off, lens, arrival, payload.size)
-    insert_device(q, stream, index, desc, off, lens, payload, arrival)
+    m.insert(stream, index, desc, off, lens, payload, arrival)
+    q.insert(stream, index, desc, off, lens, payload, arrival)
     check_timing(q, m)
     assert int(q.timing()[2][target]) == A
 
@@ -194,10 +140,9 @@ def test_garbage_arrays(sb):
     arrival.  The timing still equals the model, and the counters equal an untimed queue's."""
     N, depth, desc_cap, ts = 1000, 8, 32, 0x9E3779B1
     rng = np.random.Generator(np.random.PCG64(77))
-    timed, plain = sb.RxQueue(N, depth, desc_cap), sb.RxQueue(N, depth, desc_cap)
+    timed, plain = DeviceForm(sb, N, depth, desc_cap), DeviceForm(sb, N, depth, desc_cap)
     timed.enable_timing(ts, 50000)
-    m = SimRxTiming(N, desc_cap, ts)
-    last = np.full(N, M32 - 1, np.uint32)
+    m = timed_model(N, depth, desc_cap, ts)
     for t in range(3):
         A = 50000
         w = rng.integers(0, M32, (6, A), dtype=np.uint64).astype(np.uint32)
@@ -209,13 +154,13 @@ def test_garbage_arrays(sb):
         index = np.where(w[4] % 2 == 0, t + w[4] % 12, w[4]).astype(np.uint32)
         arrival = w[5]
         payload = rng.integers(0, 256, 256).astype(np.uint8)
-        m.insert(last, stream, index, desc, off, lens, arrival, payload.size)
-        insert_device(timed, stream, index, desc, off, lens, payload, arrival)
-        insert_device(plain, stream, index, desc, off, lens, payload)
+        m.insert(stream, index, desc, off, lens, payload, arrival)
+        timed.insert(stream, index, desc, off, lens, payload, arrival)
+        plain.insert(stream, index, desc, off, lens, payload)
         check_timing(timed, m)
-        a, b = timed.pull(cap=2 * desc_cap), plain.pull(cap=2 * desc_cap)
+        a, b = timed.pull(), plain.pull()
+        m.pull()
         assert all(np.array_equal(x, y) for x, y in zip(a, b))
-        last = last + np.uint32(1)
     ca, cb = timed.stats(), plain.stats()
     assert np.array_equal(ca[0], cb[0]) and ca[1] == cb[1] and ca[1] > 0
     assert m.received.sum() > 0
@@ -226,7 +171,7 @@ def test_reset_clears_listed_streams_and_launches(sb):
     device call refuses n_arrivals > max_arrivals and a queue without timing."""
     import torch
     n, desc_cap, ts = 40, 32, 640
-    q = sb.RxQueue(n, 8, desc_cap)
+    q = DeviceForm(sb, n, 8, desc_cap)
     k = 2 * n
     stream = np.repeat(np.arange(n, dtype=np.int32), 2)
     index = np.tile(np.array([0, 3], np.uint32), n)
@@ -236,15 +181,15 @@ def test_reset_clears_listed_streams_and_launches(sb):
     with pytest.raises(sb.SoloError):
         q.timing()
     with pytest.raises(sb.SoloError):
-        insert_device(q, *args, arrival)
+        q.insert(*args, arrival)
     q.enable_timing(ts, k)
     with pytest.raises(sb.SoloError):
         q.enable_timing(ts, k)
     with pytest.raises(sb.SoloError):
-        insert_device(q, *(np.concatenate([x, x[:1]]) for x in args[:5]), args[5], np.concatenate([arrival, arrival[:1]]))
-    insert_device(q, *args, arrival)
+        q.insert(*(np.concatenate([x, x[:1]]) for x in args[:5]), args[5], np.concatenate([arrival, arrival[:1]]))
+    q.insert(*args, arrival)
     before = q.timing()
-    insert_device(q, *args)                                   # untimed: timing unchanged
+    q.insert(*args)                                           # untimed: timing unchanged
     assert all(np.array_equal(x, y) for x, y in zip(q.timing(), before))
     listed = np.array([3, 17, 39], np.int32)
     l0 = sb.kernel_launches()
@@ -255,7 +200,7 @@ def test_reset_clears_listed_streams_and_launches(sb):
     for x, y in zip(after, before):
         assert not x[listed].any() and np.array_equal(x[keep], y[keep])
     l0 = sb.kernel_launches()
-    insert_device(q, *args, arrival)
+    q.insert(*args, arrival)
     assert sb.kernel_launches() - l0 == 3 + 2 + 3 * 1     # N = 40: one 8-bit digit
     torch.cuda.synchronize()
     assert int(q.timing()[1][3]) == 3 and int(q.timing()[2][3]) == 2
@@ -279,7 +224,7 @@ def test_loopback_jitter_has_closed_form(sb):
     k = (np.arange(N) * 37) % 300
     k[::9] = 0
     tx = sb.TxQueue(N)
-    rx = sb.RxQueue(N, 8, 128)
+    rx = HostForm(sb, N, 8, 128)
     rx.enable_timing(ts, 2 * N)
     sent = np.zeros(N, np.int64)
     for t in range(ticks):
@@ -287,8 +232,8 @@ def test_loopback_jitter_has_closed_form(sb):
         arrival = (index.astype(np.int64) * ts + 1000 + np.where(desc == 2, k[stream], 0)) % M32
         order = np.lexsort((np.arange(len(stream)), arrival))          # the network delivers in arrival order
         stream, index, desc, off, lens, arrival = (x[order] for x in (stream, index, desc, off, lens, arrival))
-        insert_host(rx, stream, index, desc, off, lens, payload, arrival.astype(np.uint32))
-        rx.pull(cap=cap)
+        rx.insert(stream, index, desc, off, lens, payload, arrival.astype(np.uint32))
+        rx.pull()
         np.add.at(sent, stream, 1)
     jitter, highest, received, margin = rx.timing()
     assert np.array_equal(jitter, np.maximum(k - 1, 0).astype(np.uint32))

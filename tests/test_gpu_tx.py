@@ -1,5 +1,5 @@
 """The send queue and the downlink contributor lists on the GPU (sb_tx_sizes / scan / pack kernels through solo_b200_tx_*,
-sb_mix_contributors_kernel), at 0 tolerance against the restatements of tests/test_tx.py: random rows at N = 257 and at
+sb_mix_contributors_kernel), at 0 tolerance against the restatements of tests/server_ref.py: random rows at N = 257 and at
 N = 65 536 (a 1 024-stream sample modelled, count, offsets and byte total checked in full), both entry-point forms, a real
 encode_device wave against split_packet, malformed nbytes, repeatability, the launch budget and the scalar refusals;
 then a loopback on the device: encode -> pack -> a seeded network -> receive queue -> decode reproduces encode ->
@@ -8,55 +8,11 @@ import numpy as np
 import pytest
 
 from tests.parity import sb  # noqa: F401  (fixture)
-from tests.test_tx import (BAD, DTX, M32, OCTETS, SENT, PyTx, contributors_literal, layout, random_rows,
-                           select_talkers, split_row)
+from tests.server_ref import (BAD, DTX, M32, OCTETS, SENT, DevicePack, HostPack, PyTx, contributors_literal, csr_rooms,
+                              random_rows, select_talkers, split_row, to_dev)
 from tests.util import load_clip, speech_replay
 
 pytestmark = pytest.mark.gpu
-
-
-def to_dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", 0))
-
-
-class DevicePack:
-    """TxQueue driven through pack_device on torch buffers, on the current torch stream."""
-
-    def __init__(self, sb, n):
-        import torch
-        self.q, self.n = sb.TxQueue(n), n
-        self.ent = [torch.zeros(2 * n, dtype=t, device="cuda") for t in (torch.int32, torch.int32, torch.uint8, torch.int32,
-                                                                          torch.int32)]
-        self.ct = torch.zeros(1, dtype=torch.int32, device="cuda")
-        self.tot = torch.zeros(1, dtype=torch.int64, device="cuda")
-
-    def pack(self, bits, nbytes):
-        import torch
-        d_bits, d_nb = to_dev(bits), to_dev(nbytes)
-        cap = bits.shape[1]
-        d_pay = torch.full((self.n * cap,), 0xA5, dtype=torch.uint8, device="cuda")
-        self.q.pack_device(d_bits.data_ptr(), cap, d_nb.data_ptr(), d_pay.data_ptr(), d_pay.numel(),
-                           *(x.data_ptr() for x in self.ent), self.ct.data_ptr(), self.tot.data_ptr(),
-                           torch.cuda.current_stream().cuda_stream)
-        c, t = int(self.ct.item()), int(self.tot.item())
-        st, ix, de, of, ln = (x[:c].cpu().numpy() for x in self.ent)
-        return bytes(d_pay[:t].cpu().numpy()), list(zip(st.tolist(), (ix.view(np.uint32)).tolist(), de.tolist(), of.tolist(),
-                                                       ln.tolist()))
-
-    def reset(self, streams, start):
-        self.q.reset(streams, start)
-
-    def stats(self):
-        import torch
-        torch.cuda.synchronize()
-        return self.q.stats()
-
-
-class HostPack(DevicePack):
-    def pack(self, bits, nbytes):
-        payload, st, ix, de, of, ln = self.q.pack(bits, nbytes)
-        return bytes(payload), list(zip(st.tolist(), ix.tolist(), de.tolist(), of.tolist(), ln.tolist()))
 
 
 @pytest.mark.parametrize("form", [DevicePack, HostPack])
@@ -229,7 +185,7 @@ def test_contributors_equal_literal_loop(sb):
     sizes = [1] * 1000 + [4] * 8192 + [256] * 64 + [12000]
     st = torch.cuda.current_stream().cuda_stream
     for k in (1, 3, 8):
-        room_start, members = layout(rng, n, sizes)
+        room_start, members = csr_rooms(rng, n, sizes)
         level = rng.integers(0, 256, n).astype(np.uint8)
         flags = np.where(rng.random(n) < 0.4, rng.integers(1, 16, n), 0).astype(np.uint8)
         tk = select_talkers(room_start, members, level, flags, k, n)

@@ -6,7 +6,7 @@ downlink encode_device against decode_device + encode_device alone, at 16 384 ro
 
     python tools/mix_time.py [--reps 50] [--warmup 5] [--tick-reps 8]
 
-Layouts: 16 384 rooms of 4; 256 rooms of 256; one room of 65 536; the mixed layout of tests/test_gpu_mix.py (8 192 rooms
+Layouts: 16 384 rooms of 4; 256 rooms of 256; one room of 65 536; the mixed layout of tests/server_ref.py (8 192 rooms
 of 4, 64 of 256, one of 12 000, 4 384 streams in no room).  Rows, levels and flags are seeded random (about 60 % of the
 streams eligible).  Prints one JSON line with the card's name and power limit beside the numbers."""
 import argparse
@@ -31,7 +31,7 @@ def main():
     import numpy as np
     import torch
     import solo_b200
-    from tests.test_gpu_mix import mixed_layout
+    from tests.server_ref import mixed_layout
     from tests.util import load_golden
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: the mix kernels have no CPU implementation to time")

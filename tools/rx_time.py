@@ -31,32 +31,18 @@ def main():
     import numpy as np
     import torch
     import solo_b200
+    from tests.server_ref import rx_time_traffic
     from tests.util import load_golden
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: the receive-queue kernels have no CPU implementation to time")
     N, depth, desc_cap, cap, dev = 65536, 8, 128, 256, torch.device("cuda", 0)
     stream = torch.cuda.current_stream().cuda_stream
     rng = np.random.Generator(np.random.PCG64(1))
-    g = load_golden()
-    P = g["fix_nbytes"].shape[0]
-    s = np.repeat(np.arange(N, dtype=np.int32), 2)
-    d = np.tile(np.array([1, 2], np.uint8), N)
-    p = s % P
-    n0, n1 = g["fix_nbytes"][p, 0].astype(np.int32), g["fix_nbytes"][p, 1].astype(np.int32)
-    lens = np.where(d == 1, n0 - n1, n1).astype(np.int32)
-    src = np.where(d == 1, 0, n0 - n1)                          # the description's first byte in its packet row
-    dup = rng.choice(2 * N, 2 * N // 100, replace=False)        # 1 % sent twice
-    s, d, lens, src, p = (np.concatenate([x, x[dup]]) for x in (s, d, lens, src, p))
-    early = rng.random(2 * N) < 0.10
-    early = np.concatenate([early, early[dup]]).astype(np.uint32)
-    order = rng.permutation(len(s))
-    s, d, lens, src, p, early = (x[order] for x in (s, d, lens, src, p, early))
-    off = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int32)
-    payload = np.concatenate([g["fix_bits"][pi, si:si + li] for pi, si, li in zip(p, src, lens)]).astype(np.uint8)
+    s, d, lens, payload, off, early = rx_time_traffic(N, rng)
     A = len(s)
     td = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
     d_s, d_d, d_off, d_len, d_pay = td(s), td(d), td(off), td(lens), td(payload)
-    d_early = td(early.view(np.int32))
+    d_early = td(early.astype(np.int32))
     d_idx = torch.zeros(A, dtype=torch.int32, device=dev)
     d_bits = torch.zeros((N, cap), dtype=torch.uint8, device=dev)
     d_nb = torch.zeros((N, 2), dtype=torch.int16, device=dev)
@@ -91,7 +77,9 @@ def main():
     # bytes the tick must move, from the shapes: payload read and stored, the arrival arrays read by the three passes
     # (17 B each), the touched slots' metadata (index 4, lengths 4, election words 16, commit word 4) read and written,
     # per stream last / counters / nbytes / lostflag, and the rows: read from the store and written
-    rows = int(n0.sum())
+    g = load_golden()
+    p = np.repeat(np.arange(N), 2) % g["fix_nbytes"].shape[0]      # the packet of each original arrival
+    rows = int(g["fix_nbytes"][p, 0].astype(np.int32).sum())
     slot_meta = N * 28 * 2
     nbytes = 2 * payload.size + 3 * 17 * A + slot_meta + N * (4 + 32 + 4 + 4) + 2 * rows
     res = {"streams": N, "depth": depth, "desc_cap": desc_cap, "cap": cap, "arrivals_per_tick": A, "reps": a.reps,

@@ -28,7 +28,7 @@ def main():
     import numpy as np
     import torch
     import solo_b200
-    from tests.test_gpu_rx_timing import rx_time_traffic
+    from tests.server_ref import rx_time_traffic
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: the receive-queue kernels have no CPU implementation to time")
     N, depth, desc_cap, cap, ts, dev = 65536, 8, 128, 256, 640, torch.device("cuda", 0)
