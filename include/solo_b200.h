@@ -25,6 +25,8 @@
  *     for the user rates that keep the 16 kHz core.  A frame that codes another core rate (8 or 12 kHz, which the reference
  *     would resample to 16 kHz) is that stream's error, ret = -12, exactly like a corrupted packet; the other streams of the
  *     batch are not affected.
+ *   - A decoder batch of 32 kHz streams may instead output their 16 kHz core (solo_b200_dec_batch_create_out): rows of
+ *     16 * framesize_ms samples, which mix with 16 kHz streams' rows.
  *   - There is no 32 kHz ENCODER yet: solo_b200_enc_batch_create and AGR_Sate_Encoder_Init return NULL for samplerate 32000,
  *     with solo_b200_last_error() saying so.
  *
@@ -95,6 +97,21 @@ solo_b200_dec_batch *solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_d
 /* The same with the arithmetic: NULL, with solo_b200_last_error() set, for an unknown value or SOLO_B200_DEC_FIX with 20 ms
    packets. */
 solo_b200_dec_batch *solo_b200_dec_batch_create_arith(int n_streams, const USER_Ctrl_dec *ctrl, int device, int arith);
+/* The same with the output rate of the batch's PCM rows.  out_samplerate = ctrl->samplerate gives the batch of
+   solo_b200_dec_batch_create_arith.  out_samplerate = 16000 with ctrl->samplerate = 32000 is core output: every packet of a
+   32 kHz stream is decoded to its 16 kHz SILK core (0-8 kHz) only, rows of 16 * framesize_ms samples (640 or 320), the
+   layout of a 16 kHz batch, so that a 32 kHz uplink is an ordinary row of a 16 kHz room (mixer, downlink encoder).
+     - The row is exactly the int16 low band the reference hands to its synthesis filter bank (AGR_Sate_qmf_synth) for the
+       same packets: band-limited to what a 16 kHz stream carries, with no resampling.  The 8-16 kHz band is not decoded
+       and the synthesis filter bank does not run: a wave is one launch instead of two.
+     - Return codes (including -12 for frames coded at an 8 or 12 kHz core), concealment, DTX / comfort noise, lostflag 2 / 3
+       and the activity flags are those of a full 32 kHz batch fed the same packets; the activity level is that of the
+       640- or 320-sample row.
+     - State blobs record the mode: the sized import refuses a blob of the other mode (a core-output stream's high-band and
+       filter-bank memories have not followed its packets, so it cannot continue as a full-band stream, nor the reverse).
+   Any other out_samplerate returns NULL with solo_b200_last_error() set. */
+solo_b200_dec_batch *solo_b200_dec_batch_create_out(int n_streams, const USER_Ctrl_dec *ctrl, int device, int arith,
+                                                    int out_samplerate);
 int solo_b200_dec_batch_decode_host(solo_b200_dec_batch *b, int16_t *pcm, const uint8_t *bits, int cap,
                                     const int16_t *nbytes, const int32_t *lostflag, int32_t *ret);
 int solo_b200_dec_batch_decode_device(solo_b200_dec_batch *b, int16_t *d_pcm, const uint8_t *d_bits, int cap,
@@ -109,8 +126,9 @@ int solo_b200_enc_batch_import_state(solo_b200_enc_batch *b, int idx, const void
 int solo_b200_dec_batch_export_state(solo_b200_dec_batch *b, int idx, void *blob);
 int solo_b200_dec_batch_import_state(solo_b200_dec_batch *b, int idx, const void *blob);
 /* The decoder forms with the blob's size: -1 (nothing copied, solo_b200_last_error() set) when blob_bytes is not the batch's
-   solo_b200_dec_state_bytes_rate(samplerate), i.e. for a blob of a stream of the other sample rate.  The unsized forms
-   above trust the caller's blob to be of the batch's rate. */
+   solo_b200_dec_state_bytes_rate(samplerate), i.e. for a blob of a stream of the other sample rate, and on import when a
+   32 kHz blob is of the other output mode (core output or full band, see solo_b200_dec_batch_create_out).  The unsized
+   forms above trust the caller's blob to be of the batch's rate and mode. */
 int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch *b, int idx, void *blob, int blob_bytes);
 int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch *b, int idx, const void *blob, int blob_bytes);
 

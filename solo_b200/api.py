@@ -57,6 +57,8 @@ def lib():
         L.solo_b200_dec_batch_create.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int]
         L.solo_b200_dec_batch_create_arith.restype = vp
         L.solo_b200_dec_batch_create_arith.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int, C.c_int]
+        L.solo_b200_dec_batch_create_out.restype = vp
+        L.solo_b200_dec_batch_create_out.argtypes = [C.c_int, C.POINTER(DecCtrl), C.c_int, C.c_int, C.c_int]
         L.solo_b200_dec_batch_decode_host.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
         L.solo_b200_dec_batch_decode_device.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp, vp]
         L.solo_b200_dec_batch_destroy.argtypes = [vp]
@@ -351,18 +353,22 @@ DEC_ARITH = {"flp": 0, "fix": 1}   # SOLO_B200_DEC_FLP / SOLO_B200_DEC_FIX
 class DecoderBatch:
     """N decoder streams resident on one GPU."""
 
-    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000):
+    def __init__(self, n, use_md_index=0, device=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000, out_samplerate=None):
         """arith: "flp" decodes to the reference float build's PCM, "fix" to its fixed-point build's (40 ms packets and
         joint mode 1 only; see solo_b200_dec_batch_create_arith in include/solo_b200.h).  samplerate: 16000, or 32000 for
-        streams of the reference's 32 kHz API (16 kHz SILK core; PCM rows of 32 * framesize_ms samples)."""
+        streams of the reference's 32 kHz API (16 kHz SILK core; PCM rows of 32 * framesize_ms samples).
+        out_samplerate: the rate of the PCM rows, samplerate by default; 16000 with samplerate 32000 decodes the streams to
+        their 16 kHz core only (rows of 16 * framesize_ms samples that mix with 16 kHz streams' rows; see
+        solo_b200_dec_batch_create_out)."""
         if arith not in DEC_ARITH:
             raise SoloError("arith must be one of %s, not %r" % (sorted(DEC_ARITH), arith))
         self.n = int(n)
         self.samplerate = int(samplerate)
-        self.samples = self.samplerate // 1000 * framesize_ms
+        self.out_samplerate = self.samplerate if out_samplerate is None else int(out_samplerate)
+        self.samples = self.out_samplerate // 1000 * framesize_ms
         self.arith = arith
         self.ctrl = DecCtrl(0, self.samplerate, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
-        self.h = lib().solo_b200_dec_batch_create_arith(self.n, C.byref(self.ctrl), device, DEC_ARITH[arith])
+        self.h = lib().solo_b200_dec_batch_create_out(self.n, C.byref(self.ctrl), device, DEC_ARITH[arith], self.out_samplerate)
         if not self.h:
             raise SoloError("solo_b200_dec_batch_create failed: " + _err())
 
@@ -394,7 +400,8 @@ class DecoderBatch:
         return blob
 
     def import_state(self, idx, blob):
-        """A blob of export_state from a batch of the same sample rate (another rate's blob is refused)."""
+        """A blob of export_state from a batch of the same sample rate and output rate (a blob of another rate, or of a
+        32 kHz batch of the other output rate, is refused)."""
         blob = np.ascontiguousarray(blob, np.uint8)
         if lib().solo_b200_dec_batch_import_state_sized(self.h, int(idx), blob.ctypes.data, blob.size):
             raise SoloError("import_state: " + _err())

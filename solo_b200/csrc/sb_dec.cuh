@@ -68,6 +68,10 @@ template <int KHZ> struct DecStateT {
     i32 plc_pitchL_Q8, plc_last_frame_lost, plc_rand_seed, plc_conc_energy, plc_conc_energy_shift;
     i32 plc_prevGain_Q16[NB_SUBFR];
     i16 plc_LTPCoef_Q14[LTP_ORDER], plc_prevLPC_Q12[LPC_ORDER], plc_randScale_Q14, plc_prevLTP_scale_Q14;
+    // 1: the stream decodes to its SILK core only (core output of a 32 kHz stream, dec_packet<KHZ, true>), so its high-band
+    // and filter-bank memories never advance.  Kept in the state so that an exported blob records it.  It sits in what was
+    // the padding after the int16 fields above: the state's size and every other field's offset are as without it.
+    i16 core_only;
     // CNG (structs.h:283-290)
     i32 cng_exc_buf_Q10[FRAME];
     i32 cng_smth_NLSF_Q15[LPC_ORDER];
@@ -98,10 +102,12 @@ template <int KHZ> struct DecCtrlT {
 
 // SKP_Silk_init_decoder + AGR_Sate_Decoder_Init, expressed for the core the first good frame selects (the PLC and CNG
 // reset themselves to it on their first call, PLC.c:52-55, CNG.c:89-94).
-template <int KHZ> SB_FN void dec_state_init(DecStateT<KHZ>* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0, i32 arith = DEC_FLP) {
+template <int KHZ> SB_FN void dec_state_init(DecStateT<KHZ>* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0, i32 arith = DEC_FLP,
+                                              i32 core_only = 0) {
     SB_DEC_DIMS(KHZ);
     memset(st, 0, sizeof(DecStateT<KHZ>));
     st->useMDIndex = useMDIndex;
+    st->core_only = core_only ? 1 : 0;
     st->arith = arith == DEC_FIX ? DEC_FIX : DEC_FLP;
     st->frames_per_packet = framesize_ms == 20 ? 1 : 2;
     st->hb_frame = joint_hb ? 2 * FRAME : FRAME;
@@ -911,7 +917,11 @@ struct DecBands { i16* low; float* high; };
 // bits/cap: payload row as handed in by the caller; nb: {n0, n1} (not modified); returns the reference's return code.
 // Everything up to the synthesis filter bank: on 0 the band signals are in `bands`, and dec_synth (the synthesis kernel)
 // turns them into PCM.
-template <int KHZ>
+// CORE (core output): the SILK core's PCM is the result.  bands->low is the caller's PCM row (nf * FRAME samples, any
+// 2-byte alignment), bands->high is unused, and the high band is not decoded: it reads the core's excitation, but nothing
+// in the core reads it, so the row is the low band the reference hands to its synthesis filter bank (AGR_Sate_qmf_synth's
+// first argument) for the same packets.  Checks, return codes, concealment and activity flags are the full decoder's.
+template <int KHZ, bool CORE = false>
 SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits, int cap, const i16* nb_in, i32 lostflag, DecStale* stale,
                      const DecBands* bands) {
     SB_DEC_DIMS(KHZ);
@@ -950,7 +960,7 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
             for (int i = c1; i < c1 + 8; i++) W->pay[1][i] = 0;
         }
     }
-    for (int i = 0; i < half; i++) { W->res_Q10[i] = 0; W->lowout[i] = 0; }
+    for (int i = 0; i < half; i++) { if (!CORE) W->res_Q10[i] = 0; W->lowout[i] = 0; }
     W->act = 0;
     for (int f = 0; f < nf; f++) {
         i32 ret;
@@ -969,7 +979,7 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
         }
         if (ret < 0) return ret;
         if (lostflag != 1) W->act |= (u8)((st->vadFlag & 1) << f);
-        for (int i = 0; i < FRAME; i++) W->res_Q10[f * FRAME + i] = st->exc_Q10[i];
+        if (!CORE) for (int i = 0; i < FRAME; i++) W->res_Q10[f * FRAME + i] = st->exc_Q10[i];
     }
     if (st->moreInternalDecoderFrames) {     // the payload outlives this call
         for (int k = 0; k < 2; k++) {
@@ -977,6 +987,18 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
             st->rc_base_Q32[k] = rc[k].base_Q32; st->rc_range_Q16[k] = rc[k].range_Q16;
             st->rc_bufferIx[k] = rc[k].bufferIx; st->rc_error[k] = rc[k].error; st->rc_bufLen[k] = rc[k].bufLen;
         }
+    }
+    if (CORE) {
+#ifdef __CUDA_ARCH__
+        if ((((size_t)bands->low) & 15) == 0) {
+            const int4* sl = reinterpret_cast<const int4*>(W->lowout);
+            int4* dl = reinterpret_cast<int4*>(bands->low);
+            for (int i = 0; i < half / 8; i++) dl[i] = sl[i];
+            return 0;
+        }
+#endif
+        for (int i = 0; i < half; i++) bands->low[i] = W->lowout[i];
+        return 0;
     }
     const int hb_lost = (lostflag == 1 || lostflag == 2);
     const bool fix = st->arith == DEC_FIX;
@@ -1005,7 +1027,8 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, const u8* bits,
 }
 
 // The whole packet on one thread (host model): the decode kernel's dec_packet, then, for an accepted packet, the synthesis
-// kernel's dec_synth into vout (2 * nf * FRAME samples).  Without DecStale storage a packet that would continue in the
+// kernel's dec_synth into vout (2 * nf * FRAME samples).  A core_only stream takes the core-output decode kernel's
+// dec_packet straight into vout (nf * FRAME samples).  Without DecStale storage a packet that would continue in the
 // previous payload resynchronises on its own bytes instead.
 template <int KHZ>
 SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, i16* vout, const u8* bits, int cap, const i16* nb_in, i32 lostflag,
@@ -1013,6 +1036,10 @@ SB_FN i32 dec_packet(DecStateT<KHZ>* st, DecPacketWorkT<KHZ>* W, i16* vout, cons
     SB_DEC_DIMS(KHZ);
     DecStale discard;
     if (!stale) { st->moreInternalDecoderFrames = 0; stale = &discard; }
+    if (st->core_only) {
+        const DecBands out = {vout, nullptr};
+        return dec_packet<KHZ, true>(st, W, bits, cap, nb_in, lostflag, stale, &out);
+    }
     i16 low[2 * FRAME];
     float high[2 * FRAME];
     const DecBands bands = {low, high};

@@ -207,12 +207,16 @@ __global__ void __launch_bounds__(SB_TPB, SB_FINISH_MINB) sb_enc_finish_kernel(E
 
 static_assert(SOLO_B200_DEC_FLP == DEC_FLP && SOLO_B200_DEC_FIX == DEC_FIX, "decoder arithmetic codes");
 template <int KHZ>
-__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecStateT<KHZ>* states, int n, int mdi, int framesize_ms, int joint_hb, int arith) {
+__global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecStateT<KHZ>* states, int n, int mdi, int framesize_ms, int joint_hb, int arith,
+                                                             int core_only) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb, arith);
+    if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb, arith, core_only);
 }
 
-template <int KHZ>
+// CORE = false: band signals of `spp`-sample packets into band_low / band_high, rows of spp / 2 samples, for the synthesis
+// kernel.  CORE = true (core output): the SILK core's PCM straight into band_low = the caller's PCM rows of spp / 2 samples;
+// band_high is not used and there is no synthesis launch.
+template <int KHZ, bool CORE = false>
 __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(DecStateT<KHZ>* states, const u8* __restrict__ bits, int cap,
                                                            const i16* __restrict__ nbytes, const i32* __restrict__ lostflag,
                                                            i32* __restrict__ ret, i32* __restrict__ ret_int, u8* __restrict__ act, DecStale* stale,
@@ -221,8 +225,8 @@ __global__ void __launch_bounds__(SB_DEC_TPB, SB_DECODE_MINB) sb_decode_kernel(D
     if (s >= n) return;
     DecPacketWorkT<KHZ> W;
     i16 nb[2] = {nbytes[2 * s], nbytes[2 * s + 1]};
-    const DecBands bands = {band_low + (size_t)s * (spp / 2), band_high + (size_t)s * (spp / 2)};
-    i32 r = dec_packet(&states[s], &W, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
+    const DecBands bands = {band_low + (size_t)s * (spp / 2), CORE ? nullptr : band_high + (size_t)s * (spp / 2)};
+    i32 r = dec_packet<KHZ, CORE>(&states[s], &W, bits + (size_t)s * cap, cap, nb, lostflag[s], &stale[s], &bands);
     if (ret) ret[s] = r;
     ret_int[s] = r;
     act[s] = r < 0 ? (u8)0 : W.act;
@@ -1078,6 +1082,7 @@ struct solo_b200_enc_batch : Batch {
 };
 struct solo_b200_dec_batch : Batch {
     int khz;                    // SILK core rate: 8 (16 kHz streams, DecState) or 16 (32 kHz streams, DecState32)
+    int core_only;              // 1: 32 kHz streams decoded to their 16 kHz core (spp = the core's rows, no band buffers)
     void* d_states;             // DecStateT<khz>[n]
     DecStale* d_stale;          // payload copies that outlive a packet call (only touched after a corrupted packet, see sb_dec.cuh)
     i32* d_flags; i32* d_ret;   // staging for the *_host entry points and the arena
@@ -1400,21 +1405,29 @@ static int check_dec_arith(const USER_Ctrl_dec* c, int arith) {
 // (re)initialise streams [lo, lo + n) of a decoder batch on its first CUDA stream
 static void dec_init_launch(solo_b200_dec_batch* b, int lo, int n, int mdi, int framesize_ms, int joint_enable, int arith) {
     const int g = (n + SB_TPB - 1) / SB_TPB, joint = joint_enable ? 1 : 0;
-    if (b->khz == 16) sb_dec_init_kernel<16><<<g, SB_TPB, 0, b->st[0]>>>((DecState32*)b->d_states + lo, n, mdi, framesize_ms, joint, arith);
-    else sb_dec_init_kernel<8><<<g, SB_TPB, 0, b->st[0]>>>((DecState*)b->d_states + lo, n, mdi, framesize_ms, joint, arith);
+    if (b->khz == 16) sb_dec_init_kernel<16><<<g, SB_TPB, 0, b->st[0]>>>((DecState32*)b->d_states + lo, n, mdi, framesize_ms, joint, arith, b->core_only);
+    else sb_dec_init_kernel<8><<<g, SB_TPB, 0, b->st[0]>>>((DecState*)b->d_states + lo, n, mdi, framesize_ms, joint, arith, 0);
     count_launch();
 }
-static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst, int arith) {
+// out_samplerate: ctrl->samplerate, or 16000 for 32 kHz streams decoded to their 16 kHz core
+static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst, int arith, int out_samplerate) {
     if (n_streams <= 0 || check_dec_ctrl(ctrl)) { snprintf(g_err, sizeof g_err, "bad decoder configuration"); return nullptr; }
     if (check_dec_arith(ctrl, arith)) return nullptr;
+    const int core_only = ctrl->samplerate == 32000 && out_samplerate == 16000;
+    if (out_samplerate != ctrl->samplerate && !core_only) {
+        snprintf(g_err, sizeof g_err, "bad decoder output rate %d for %d Hz streams (the stream's rate, or 16000 for 32000)", out_samplerate, ctrl->samplerate);
+        return nullptr;
+    }
     if (require_gpu(device)) return nullptr;
     solo_b200_dec_batch* b = new solo_b200_dec_batch();
     b->khz = ctrl->samplerate == 32000 ? 16 : 8;
-    if (!batch_setup(b, n_streams, device, ctrl->samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
+    b->core_only = core_only;
+    const size_t band = core_only ? 0 : (size_t)ctrl->samplerate / 2000 * ctrl->framesize_ms;   // samples per band and packet
+    if (!batch_setup(b, n_streams, device, out_samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
         cudaMalloc(&b->d_states, state_stride(b) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_stale, sizeof(DecStale) * (size_t)n_streams) != cudaSuccess ||
-        cudaMalloc(&b->d_band_low, sizeof(i16) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
-        cudaMalloc(&b->d_band_high, sizeof(float) * (size_t)(b->spp / 2) * (size_t)n_streams) != cudaSuccess ||
+        (band && cudaMalloc(&b->d_band_low, sizeof(i16) * band * (size_t)n_streams) != cudaSuccess) ||
+        (band && cudaMalloc(&b->d_band_high, sizeof(float) * band * (size_t)n_streams) != cudaSuccess) ||
         cudaMalloc(&b->d_ret_int, sizeof(i32) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_act_flags, (size_t)n_streams) != cudaSuccess) {
         fail("dec_batch_create", cudaGetLastError());
@@ -1426,18 +1439,29 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
     return b;
 }
 solo_b200_dec_batch* solo_b200_dec_batch_create(int n_streams, const USER_Ctrl_dec* ctrl, int device) {
-    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, SOLO_B200_DEC_FLP);
+    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, SOLO_B200_DEC_FLP, ctrl ? ctrl->samplerate : 0);
 }
 solo_b200_dec_batch* solo_b200_dec_batch_create_arith(int n_streams, const USER_Ctrl_dec* ctrl, int device, int arith) {
-    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith);
+    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith, ctrl ? ctrl->samplerate : 0);
+}
+solo_b200_dec_batch* solo_b200_dec_batch_create_out(int n_streams, const USER_Ctrl_dec* ctrl, int device, int arith, int out_samplerate) {
+    return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith, out_samplerate);
 }
 
-// the two decoder kernels of core rate KHZ for streams [lo, lo + n) of b
+// the decoder kernels of core rate KHZ for streams [lo, lo + n) of b: decode and synthesis, or the core-output decode alone
 extern "C++" {
 template <int KHZ>
 static void dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
                         i32* d_ret, cudaStream_t st) {
     DecStateT<KHZ>* states = (DecStateT<KHZ>*)b->d_states + lo;
+    // core output: the PCM rows (b->spp samples) are the low band of 2 * b->spp-sample packets
+    if constexpr (KHZ == 16) if (b->core_only) {
+        sb_decode_kernel<KHZ, true><<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(states, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo,
+                                                                                    d_lostflag + lo, d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo,
+                                                                                    b->d_act_flags + lo, b->d_stale + lo, d_pcm + (size_t)lo * b->spp,
+                                                                                    nullptr, 2 * b->spp, n);
+        return;
+    }
     const size_t half = (size_t)(b->spp / 2);
     sb_decode_kernel<KHZ><<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(states, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, d_lostflag + lo,
                                                                        d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_act_flags + lo, b->d_stale + lo,
@@ -1453,7 +1477,8 @@ static int dec_launch(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u
     if (b->khz == 16) dec_kernels<16>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
     else dec_kernels<8>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
     prof_end(st, &ev);
-    count_launch(); count_launch();
+    count_launch();
+    if (!b->core_only) count_launch();      // the synthesis kernel
     CK(cudaGetLastError());
     return 0;
 }
@@ -1495,6 +1520,13 @@ int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch* b, int idx, void
     return state_copy(b, idx, blob, 1, blob_bytes < 0 ? 0 : blob_bytes);
 }
 int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch* b, int idx, const void* blob, int blob_bytes) {
+    // a blob of the batch's size but of the other output mode: a core-output stream's high-band and filter-bank memories
+    // have not followed its packets
+    if (b && blob && b->khz == 16 && blob_bytes == (int)sizeof(DecState32) && ((const DecState32*)blob)->core_only != b->core_only) {
+        snprintf(g_err, sizeof g_err, "state blob of a %s stream, this batch decodes %s", b->core_only ? "full-band 32 kHz" : "core-output (16 kHz)",
+                 b->core_only ? "to the 16 kHz core" : "the full 32 kHz band");
+        return -1;
+    }
     return state_copy(b, idx, (void*)blob, 0, blob_bytes < 0 ? 0 : blob_bytes);
 }
 
@@ -2296,7 +2328,7 @@ void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
     if (check_dec_arith(dec_Ctrl, arith)) { fprintf(stderr, "solo_b200: AGR_Sate_Decoder_Init: %s\n", g_err); return nullptr; }
     // the arithmetic is a property of the slot, not of the segment: one segment holds handles of both kinds
     return arena_open(g_dec_segs, DEC_MAGIC, dec_Ctrl->samplerate, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, "AGR_Sate_Decoder_Init", "decoder",
-                      [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1, SOLO_B200_DEC_FLP); },
+                      [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1, SOLO_B200_DEC_FLP, dec_Ctrl->samplerate); },
                       [&](solo_b200_dec_batch* b, int slot) {
                           dec_init_launch(b, slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, arith);
                       });
