@@ -43,6 +43,11 @@ def available():
     return all(os.path.exists(os.path.join(REF_DIR, f)) for f in ("libjc1_fix.so", "libjc1_flp.so"))
 
 
+def lowband_available():
+    """The decoders with a tap on their low band (oracle/lowband.mk) are built."""
+    return all(os.path.exists(os.path.join(REF_DIR, "libjc1_%s_lowband.so" % k)) for k in ("flp", "fix"))
+
+
 class RefLib:
     def __init__(self, kind="fix"):
         path = os.path.join(REF_DIR, "libjc1_%s.so" % kind)
@@ -71,19 +76,19 @@ def lib(kind):
 
 
 class RefEncoder:
-    """One reference encoder handle (kind = 'fix' | 'flp')."""
+    """One reference encoder handle (kind = 'fix' | 'flp') at the API sample rate `samplerate` (16000 or 32000)."""
 
-    def __init__(self, kind="fix", rate=13600, dtx=0, use_md_index=0, framesize_ms=40, joint_hb=0):
+    def __init__(self, kind="fix", rate=13600, dtx=0, use_md_index=0, framesize_ms=40, joint_hb=0, samplerate=16000):
         self.kind = kind
         self.L = lib(kind).lib
-        self.samples = 16 * framesize_ms
-        self.ctrl = EncCtrl(2, rate, 16000, dtx, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
+        self.samples = samplerate // 1000 * framesize_ms
+        self.ctrl = EncCtrl(2, rate, samplerate, dtx, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
         self.h = self.L.AGR_Sate_Encoder_Init(C.byref(self.ctrl))
         self._bits = (C.c_uint8 * 1024)()
         self._nb = (C.c_int16 * 6)()
 
-    def encode(self, pcm640):
-        pcm = np.ascontiguousarray(pcm640, dtype=np.int16)
+    def encode(self, pcm_packet):
+        pcm = np.ascontiguousarray(pcm_packet, dtype=np.int16)
         assert pcm.size == self.samples
         C.memset(self._nb, 0, 12)
         n = self.L.AGR_Sate_Encoder_Encode(self.h, pcm.ctypes.data, self._bits, 1024, self._nb)
@@ -120,22 +125,44 @@ class RefEncoder:
 
 
 class RefDecoder:
-    """One reference decoder handle (kind = 'flp' is the PCM parity target)."""
+    """One reference decoder handle (kind = 'flp' is the PCM parity target, 'fix' the fixed-point build) at the API sample
+    rate `samplerate` (16000 or 32000).
 
-    def __init__(self, kind="flp", use_md_index=0, framesize_ms=40, joint_hb=0):
-        self.L = lib(kind).lib
-        self.samples = 16 * framesize_ms
-        self.ctrl = DecCtrl(0, 16000, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
+    out_samplerate = 16000 for a 32 kHz stream: the same decoder in the build with a tap on its low band (oracle/lowband.mk).
+    decode() then returns the int16 low band the packet handed to the synthesis filter bank (AGR_Sate_qmf_synth's first
+    argument, 16 * framesize_ms samples), or an empty row when the filter bank did not run (a rejected packet); `full` keeps
+    that call's full-band PCM.  The tap records one low band per library, so decode calls into one tapped library must not
+    overlap."""
+
+    def __init__(self, kind="flp", use_md_index=0, framesize_ms=40, joint_hb=0, samplerate=16000, out_samplerate=None):
+        out_samplerate = samplerate if out_samplerate is None else out_samplerate
+        self.tapped = (samplerate, out_samplerate) == (32000, 16000)
+        if out_samplerate != samplerate and not self.tapped:
+            raise ValueError("no decoder of %d Hz streams with %d Hz output" % (samplerate, out_samplerate))
+        self.L = lib(kind + "_lowband" if self.tapped else kind).lib
+        self.ns_want = samplerate // 1000 * framesize_ms
+        self.samples = out_samplerate // 1000 * framesize_ms
+        self.ctrl = DecCtrl(0, samplerate, framesize_ms, 1 if joint_hb else 0, 1 if joint_hb else 0, use_md_index)
         self.h = self.L.AGR_Sate_Decoder_Init(C.byref(self.ctrl))
-        self._out = np.zeros(960, dtype=np.int16)
+        self._out = np.zeros(samplerate // 1000 * 60, dtype=np.int16)
         self._ns = C.c_int16(0)
+        if self.tapped:
+            self.L.lowband_take.argtypes = [C.c_void_p, C.c_int]
+            self._low = np.zeros(self.samples, np.int16)
+            self.L.lowband_take(self._low.ctypes.data, self._low.size)
 
     def decode(self, payload, nbytes, lostflag):
-        """payload/nbytes pre-trimmed by the caller as dec_main.c:245-307 does."""
+        """payload/nbytes pre-trimmed by the caller as dec_main.c:245-307 does; returns (PCM, return value)."""
         buf = (C.c_uint8 * 1024)(*payload) if payload else (C.c_uint8 * 1024)()
         nb = (C.c_int16 * 6)(int(nbytes[0]), int(nbytes[1]))
         ret = self.L.AGR_Sate_Decoder_Decode(self.h, self._out.ctypes.data, C.byref(self._ns), buf, nb, int(lostflag))
-        return self._out[:self.samples].copy(), ret
+        assert ret != 0 or self._ns.value == self.ns_want, (self._ns.value, self.ns_want)
+        if not self.tapped:
+            return self._out[:self.samples].copy(), ret
+        self.full = self._out[:self.ns_want].copy()
+        n = self.L.lowband_take(self._low.ctypes.data, self._low.size)
+        assert n in (0, self.samples), n
+        return self._low[:n].copy(), ret
 
     def close(self):
         if self.h:

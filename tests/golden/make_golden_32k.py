@@ -4,7 +4,7 @@ its two decoders make of them -- the parity target of the 32 kHz decoder.  Needs
 
     python tests/golden/make_golden_32k.py
 
-Inputs, made from speech_clip.npz by fixed rules (tests/ref32.py):
+Inputs, made from speech_clip.npz by fixed rules (tests/util.py):
   up   upsample2(clip): every 16 kHz sample followed by floor((x[n] + x[n+1]) / 2) -- integer-exact
   hb   with_high_band(clip): up plus white noise (sigma 400, PCG64 seed 32), so that 8-16 kHz carries a signal
 Streams (FIX encoder at 32 kHz; user rates inside the range that keeps the 16 kHz core, see INTEGRATION.md):
@@ -27,8 +27,8 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-from tests.ref32 import Ref32Decoder, Ref32Encoder, upsample2, with_high_band  # noqa: E402
-from tests.util import loss_flags, trim_payload  # noqa: E402
+from oracle.ref import RefDecoder, RefEncoder  # noqa: E402
+from tests.util import loss_flags, trim_payload, upsample2, with_high_band  # noqa: E402
 
 OUT = os.path.join(HERE, "golden_32k.npz")
 # name: (input, encoder / decoder configuration, rate, packets, loss percentage of the lossy decode or None)
@@ -43,6 +43,11 @@ STREAMS = {
 def inputs():
     clip = np.load(os.path.join(HERE, "speech_clip.npz"))["pcm"]
     return {"up": upsample2(clip), "hb": with_high_band(clip)}
+
+
+def load():
+    """The committed fixture."""
+    return np.load(OUT)
 
 
 def packet_md5(pcm_rows):
@@ -95,14 +100,14 @@ def fixture():
     x = inputs()
     f = {}
     for s, (src, cfg, rate, n, loss) in STREAMS.items():
-        e = Ref32Encoder("fix", rate=rate, **cfg)
+        e = RefEncoder("fix", rate=rate, samplerate=32000, **cfg)
         pk = [e.encode(x[src][p * e.samples:(p + 1) * e.samples]) for p in range(n)]
         e.close()
         f[s + "_bits"] = np.frombuffer(b"".join(b for b, _, _ in pk), np.uint8)
         f[s + "_nbytes"] = np.array([nb for _, nb, _ in pk], np.int16)
         f[s + "_loss_flags"] = np.array(loss_flags(n, loss if loss else 50, seed=3), np.int32)
     for key, s, kind, rule in decode_cases():
-        rows = decode(Ref32Decoder(kind, **STREAMS[s][1]), packets(f, s), flags_of(f, s, rule))
+        rows = decode(RefDecoder(kind, samplerate=32000, **STREAMS[s][1]), packets(f, s), flags_of(f, s, rule))
         f[key + "_md5"] = hashlib.md5(np.concatenate(rows).tobytes()).hexdigest()
         f[key + "_packet_md5"] = packet_md5(rows)
     return f

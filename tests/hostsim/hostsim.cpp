@@ -329,10 +329,10 @@ int hs_row_level(const short* pcm, int n) {
 
 // one decoder stream; samplerate (first, so that hs_dec_decode can read it) picks the core rate: 16000 -> KHZ 8, 32000 -> 16
 template <int KHZ> struct HsDec { int samplerate; sb::DecStateT<KHZ> st; sb::DecPacketWorkT<KHZ> w; sb::DecStale stale; };
-template <int KHZ> static void* dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate) {
+template <int KHZ> static void* dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate, int core_only) {
     HsDec<KHZ>* h = (HsDec<KHZ>*)calloc(1, sizeof(HsDec<KHZ>));
     h->samplerate = samplerate;
-    sb::dec_state_init(&h->st, mdi, framesize_ms, joint_hb, arith);
+    sb::dec_state_init(&h->st, mdi, framesize_ms, joint_hb, arith, core_only);
     return h;
 }
 template <int KHZ> static int dec_decode(void* p, short* pcm, const unsigned char* bits, int cap, const short* nb, int lostflag, unsigned char* flags) {
@@ -343,10 +343,13 @@ template <int KHZ> static int dec_decode(void* p, short* pcm, const unsigned cha
 }
 
 extern "C" {
-// arith: sb::DEC_FLP or sb::DEC_FIX; samplerate 16000 or 32000 (NULL for any other)
-void* hs_dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate) {
-    if (samplerate == 16000) return dec_create<8>(mdi, framesize_ms, joint_hb, arith, samplerate);
-    if (samplerate == 32000) return dec_create<16>(mdi, framesize_ms, joint_hb, arith, samplerate);
+// arith: sb::DEC_FLP or sb::DEC_FIX; samplerate 16000 or 32000; out_samplerate the stream's own rate, or 16000 for a 32 kHz
+// stream decoded to its 16 kHz core (the core-output decode kernel's dec_packet<16, true>).  NULL for any other pair, as
+// solo_b200_dec_batch_create_out refuses them.
+void* hs_dec_create(int mdi, int framesize_ms, int joint_hb, int arith, int samplerate, int out_samplerate) {
+    if (samplerate == 16000 && out_samplerate == 16000) return dec_create<8>(mdi, framesize_ms, joint_hb, arith, samplerate, 0);
+    if (samplerate == 32000 && (out_samplerate == 32000 || out_samplerate == 16000))
+        return dec_create<16>(mdi, framesize_ms, joint_hb, arith, samplerate, out_samplerate == 16000);
     return nullptr;
 }
 // same calling convention as AGR_Sate_Decoder_Decode (payload pre-trimmed by the caller); nb is not modified.  flags (may be

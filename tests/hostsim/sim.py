@@ -20,7 +20,7 @@ def lib(emu=None):
         L.hs_enc_create3.restype = C.c_void_p
         L.hs_enc_create3.argtypes = [C.c_int] * 5
         L.hs_dec_create.restype = C.c_void_p
-        L.hs_dec_create.argtypes = [C.c_int] * 5
+        L.hs_dec_create.argtypes = [C.c_int] * 6
         L.hs_enc_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.hs_enc_destroy.argtypes = [C.c_void_p]
         L.hs_enc_set_control.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
@@ -139,12 +139,15 @@ def row_level(x):
 
 
 class SimDecoder:
-    def __init__(self, use_md_index=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000):
-        """arith "flp" / "fix": the reference's float or fixed-point build; samplerate 16000 or 32000 (16 kHz SILK core)."""
+    def __init__(self, use_md_index=0, framesize_ms=40, joint_hb=0, arith="flp", samplerate=16000, out_samplerate=None):
+        """arith "flp" / "fix": the reference's float or fixed-point build; samplerate 16000 or 32000 (16 kHz SILK core);
+        out_samplerate the stream's rate (the default) or, for a 32 kHz stream, 16000: rows of its 16 kHz core."""
+        out_samplerate = samplerate if out_samplerate is None else out_samplerate
         self.L = lib()
-        self.h = self.L.hs_dec_create(use_md_index, framesize_ms, joint_hb, ARITH[arith], samplerate)
-        assert self.h, samplerate
-        self.pcm = np.zeros(samplerate // 1000 * framesize_ms, np.int16)
+        self.h = self.L.hs_dec_create(use_md_index, framesize_ms, joint_hb, ARITH[arith], samplerate, out_samplerate)
+        if not self.h:
+            raise ValueError("no decoder of %d Hz streams with %d Hz output" % (samplerate, out_samplerate))
+        self.pcm = np.zeros(out_samplerate // 1000 * framesize_ms, np.int16)
         self.fl = np.zeros(1, np.uint8)
         self.flags = 0      # the activity flags of the last packet: bit f VAD flag, bit 2 + f concealed; 0 if rejected
 

@@ -1,7 +1,8 @@
 """Drivers of the parity tests.
 
 lockstep runs two per-stream codecs side by side: the host model of the kernels, the drop-in handles or the reference.
-RefRows runs the reference per checked row beside a batch, and DevicePath drives a batch through its device entry points.
+RefRows runs the reference per checked row beside a batch.  DeviceDecoder drives a decoder batch through its device entry
+points, and DevicePath an encoder batch and its decoder batch.
 The fixtures sb, ref and sim are imported by the test modules that use them.
 Bar: payloads and both length fields byte-identical; return values 0; PCM within PCM_TOL."""
 import collections
@@ -82,14 +83,19 @@ def batch_packets(bits, nb):
     return [(bytes(bits[i, :max(int(nb[i, 0]), 0)]), (int(nb[i, 0]), int(nb[i, 1]))) for i in range(len(nb))]
 
 
+def batch_rows(rx, cap):
+    """(payload, nbytes, lostflag) triples as a batch decoder's input: payloads uint8 [rows, cap] (a payload longer than cap
+    cut to it), nbytes int16 [rows, 2], lostflags int32 [rows]."""
+    tb, tnb, tf = np.zeros((len(rx), cap), np.uint8), np.zeros((len(rx), 2), np.int16), np.zeros(len(rx), np.int32)
+    for i, (b, tnb[i], tf[i]) in enumerate(rx):
+        tb[i, :min(len(b), cap)] = np.frombuffer(b, np.uint8)[:cap]
+    return tb, tnb, tf
+
+
 def received(packets, flags, cap):
     """What the receiver hands a batch decoder: `receive` of each (payload, (n0, n1)) packet under its lostflag, as
-    payloads uint8 [rows, cap], nbytes int16 [rows, 2], lostflags int32 [rows]."""
-    tb, tnb, tf = np.zeros((len(packets), cap), np.uint8), np.zeros((len(packets), 2), np.int16), np.zeros(len(packets), np.int32)
-    for i, ((b, nb), f) in enumerate(zip(packets, flags)):
-        pb, tnb[i], tf[i] = receive(b, nb, f)
-        tb[i, :len(pb)] = np.frombuffer(pb, np.uint8)
-    return tb, tnb, tf
+    batch_rows."""
+    return batch_rows([receive(b, nb, f) for (b, nb), f in zip(packets, flags)], cap)
 
 
 class RefRows:
@@ -153,19 +159,59 @@ class RefRows:
         self.pool.shutdown()
 
 
+class DeviceDecoder:
+    """A decoder batch through decode_device and activity_device on torch buffers of its own (cuda:0), in order on `stream`
+    (default: the current stream).  Same call shapes as the batch's host calls, decode and activity."""
+
+    def __init__(self, db, cap=256, stream=None):
+        import torch
+        self.torch, self.db, self.cap = torch, db, cap
+        self.stream = torch.cuda.current_stream() if stream is None else stream
+        N, dev = db.n, torch.device("cuda", 0)
+        self.tb, self.tnb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
+        self.flags, self.ret = torch.zeros(N, dtype=torch.int32, device=dev), torch.full((N,), -99, dtype=torch.int32, device=dev)
+        self.pcm = torch.zeros((N, db.samples), dtype=torch.int16, device=dev)
+        self.level, self.vad = torch.zeros(N, dtype=torch.uint8, device=dev), torch.zeros(N, dtype=torch.uint8, device=dev)
+
+    def decode(self, tb=None, tnb=None, tf=None, rows=None, check=True):
+        """Decode payloads [N, cap], nbytes [N, 2] and lostflags [N]: host arrays or cuda:0 tensors, each copied into the
+        decoder's input buffer on the device, where a leading dimension of 1 is broadcast over the batch; None decodes what
+        that buffer holds.  check: every row must return 0.  Returns (pcm, ret) of rows (all rows by default) as host
+        arrays."""
+        torch = self.torch
+        with torch.cuda.stream(self.stream):
+            for buf, a in ((self.tb, tb), (self.tnb, tnb), (self.flags, tf)):
+                if a is not None:
+                    buf.copy_(torch.as_tensor(np.ascontiguousarray(a) if isinstance(a, np.ndarray) else a).to(buf.device))
+            self.db.decode_device(self.pcm.data_ptr(), self.tb.data_ptr(), self.cap, self.tnb.data_ptr(), self.flags.data_ptr(),
+                                  self.ret.data_ptr(), self.stream.cuda_stream)
+        self.stream.synchronize()
+        assert not check or int((self.ret != 0).sum().item()) == 0, "decoder return"
+        return self._rows(self.pcm, rows), self._rows(self.ret, rows)
+
+    def activity(self, rows=None):
+        """activity_device after the last decode: (level, flags) of rows (all rows by default) as host arrays."""
+        with self.torch.cuda.stream(self.stream):
+            self.db.activity_device(self.pcm.data_ptr(), self.level.data_ptr(), self.vad.data_ptr(), self.stream.cuda_stream)
+        return self._rows(self.level, rows), self._rows(self.vad, rows)
+
+    def _rows(self, t, rows):
+        self.stream.synchronize()
+        return (t if rows is None else t[self.torch.as_tensor(rows, dtype=self.torch.long, device=t.device)]).cpu().numpy()
+
+
 class DevicePath:
     """A batch through its device entry points on torch buffers of its own (cuda:0), in order on `stream` (default: the
     current stream): set_control_device, encode_device, then apply_loss_device or host-made payloads, decode_device."""
 
     def __init__(self, sb, eb, db=None, cap=256, stream=None):
         import torch
-        self.torch, self.sb, self.eb, self.db, self.cap = torch, sb, eb, db, cap
+        self.torch, self.sb, self.eb, self.cap = torch, sb, eb, cap
         self.stream = torch.cuda.current_stream() if stream is None else stream
+        self.dec = DeviceDecoder(db, cap, self.stream) if db is not None else None
         N, S, dev = eb.n, eb.samples, torch.device("cuda", 0)
-        self.x, self.pcm = torch.zeros((N, S), dtype=torch.int16, device=dev), torch.zeros((N, S), dtype=torch.int16, device=dev)
-        self.bits, self.tb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, cap), dtype=torch.uint8, device=dev)
-        self.nb, self.tnb = torch.zeros((N, 2), dtype=torch.int16, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
-        self.flags, self.ret = torch.zeros(N, dtype=torch.int32, device=dev), torch.zeros(N, dtype=torch.int32, device=dev)
+        self.x = torch.zeros((N, S), dtype=torch.int16, device=dev)
+        self.bits, self.nb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
         self.ctrl = torch.zeros((3, N), dtype=torch.int32, device=dev)
 
     def encode(self, x, control=None):
@@ -186,24 +232,21 @@ class DevicePath:
     def decode(self, flags, rx=None):
         """Decode under lostflags [N]: the encoded payloads trimmed on the device (apply_loss_device), or rx = (payloads,
         nbytes) made on the host.  Every row must return 0."""
-        torch, st = self.torch, self.stream.cuda_stream
-        with torch.cuda.stream(self.stream):
-            self.flags.copy_(torch.from_numpy(np.ascontiguousarray(flags, np.int32)))
-            if rx is None:
-                self.sb.apply_loss_device(self.bits.data_ptr(), self.nb.data_ptr(), self.flags.data_ptr(), self.tb.data_ptr(),
-                                          self.tnb.data_ptr(), self.cap, self.eb.n, st)
-            else:
-                self.tb.copy_(torch.from_numpy(rx[0]))
-                self.tnb.copy_(torch.from_numpy(rx[1]))
-            self.db.decode_device(self.pcm.data_ptr(), self.tb.data_ptr(), self.cap, self.tnb.data_ptr(), self.flags.data_ptr(),
-                                  self.ret.data_ptr(), st)
-        self.stream.synchronize()
-        assert int((self.ret != 0).sum().item()) == 0, "decoder return"
+        d = self.dec           # rows=[]: nothing comes back to the host here, rows() reads the PCM
+        if rx is not None:
+            d.decode(rx[0], rx[1], flags, rows=[])
+            return
+        with self.torch.cuda.stream(self.stream):
+            d.flags.copy_(self.torch.from_numpy(np.ascontiguousarray(flags, np.int32)))
+            self.sb.apply_loss_device(self.bits.data_ptr(), self.nb.data_ptr(), d.flags.data_ptr(), d.tb.data_ptr(),
+                                      d.tnb.data_ptr(), self.cap, self.eb.n, self.stream.cuda_stream)
+        d.decode(rows=[])
 
     def rows(self, idx=None):
-        """(payloads, length fields, PCM) of rows idx (all rows by default) as host arrays."""
+        """(payloads, length fields, PCM -- None without a decoder batch) of rows idx (all rows by default) as host
+        arrays."""
         self.stream.synchronize()
         if idx is None:
-            return self.bits.cpu().numpy(), self.nb.cpu().numpy(), self.pcm.cpu().numpy()
+            return self.bits.cpu().numpy(), self.nb.cpu().numpy(), self.dec and self.dec.pcm.cpu().numpy()
         i = self.torch.tensor(idx, device=self.bits.device)
-        return self.bits[i].cpu().numpy(), self.nb[i].cpu().numpy(), self.pcm[i].cpu().numpy()
+        return self.bits[i].cpu().numpy(), self.nb[i].cpu().numpy(), self.dec and self.dec.pcm[i].cpu().numpy()

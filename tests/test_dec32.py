@@ -6,19 +6,14 @@ tests/golden/golden_32k.npz pins the reference's PCM of 32 kHz bitstreams by per
 where oracle/_ref is built, the fixture is re-derived from it and the host model runs in lockstep with both reference
 decoders over inputs the fixture does not cover."""
 import hashlib
-import os
 
 import numpy as np
 import pytest
 
 from tests.golden import make_golden_32k as mk
 from tests.parity import ref, sim  # noqa: F401  (fixtures)
-from tests.util import GOLDEN, fuzz_decoder, load_clip, load_golden, loss_flags, loss_with_bursts, receive
-
-
-def load32():
-    return np.load(os.path.join(GOLDEN, "golden_32k.npz"))
-
+from tests.util import (chirp, fuzz_decoder, load_clip, load_golden, loss_flags, loss_with_bursts, receive, upsample2,
+                        with_high_band)
 
 CASES = mk.decode_cases()
 
@@ -26,7 +21,7 @@ CASES = mk.decode_cases()
 @pytest.mark.parametrize("key,stream,kind,rule", CASES, ids=[c[0] for c in CASES])
 def test_host_model_matches_fixture(sim, key, stream, kind, rule):
     """Every pinned 32 kHz decode, in the arithmetic of the reference build that made it: per-packet md5 equal (0 LSB)."""
-    f = load32()
+    f = mk.load()
     d = sim.SimDecoder(arith=kind, samplerate=32000, **mk.STREAMS[stream][1])
     rows = mk.decode(d, mk.packets(f, stream), mk.flags_of(f, stream, rule))
     assert all(len(y) == 32 * mk.STREAMS[stream][1]["framesize_ms"] for y in rows)
@@ -38,7 +33,7 @@ def test_host_model_matches_fixture(sim, key, stream, kind, rule):
 
 def test_fixture_rederived_from_oracle(ref):
     """The committed fixture is what the reference libraries produce now (inputs, payloads, both decoders' PCM)."""
-    f, want = mk.fixture(), load32()
+    f, want = mk.fixture(), mk.load()
     assert sorted(f) == sorted(want.files)
     for k in f:
         assert np.array_equal(np.asarray(f[k]), want[k]), k
@@ -48,7 +43,7 @@ def test_other_core_rate_is_that_streams_error(sim):
     """A frame whose sampling-rate index is not the decoder's core rate is a rejected packet (-12), as a corrupted one: 16 kHz
     streams' packets (8 kHz core) to a 32 kHz decoder and 32 kHz streams' packets to a 16 kHz decoder.  The decoder stays
     usable: a good packet after the rejected ones decodes as it does on a fresh decoder."""
-    g, f = load_golden(), load32()
+    g, f = load_golden(), mk.load()
     pk32 = mk.packets(f, "hb40")
     for arith in ("flp", "fix"):
         d = sim.SimDecoder(arith=arith, samplerate=32000)
@@ -70,9 +65,8 @@ def test_other_core_rate_is_that_streams_error(sim):
 
 def test_low_rate_handset_stream_is_rejected_not_misdecoded(ref, sim):
     """A reference 32 kHz encoder below the 16 kHz-core range (12 kb/s) codes a lower core; every such packet is -12 here."""
-    from tests.ref32 import Ref32Encoder, with_high_band
     x = with_high_band(load_clip()[:640 * 10])
-    e = Ref32Encoder("fix", rate=12000)
+    e = ref.RefEncoder("fix", rate=12000, samplerate=32000)
     d = sim.SimDecoder(samplerate=32000)
     for p in range(10):
         b, nb, n = e.encode(x[p * 1280:(p + 1) * 1280])
@@ -83,7 +77,6 @@ def test_low_rate_handset_stream_is_rejected_not_misdecoded(ref, sim):
 def signals32(n_packets, seed=11):
     """(name, int16 32 kHz signal) classes beyond the fixture: speech with noise, zeros, DC, full-scale square, a chirp over
     the whole band, loud noise, 2 kHz sine, speech fading to silence (for DTX)."""
-    from tests.ref32 import chirp, upsample2, with_high_band
     rng = np.random.Generator(np.random.PCG64(seed))
     clip = load_clip()
     L = 1280 * n_packets
@@ -128,17 +121,16 @@ def flags_for(kind, n, s):
 def test_lockstep_with_reference_decoders(ref, sim, cfg, rate, mdi, dtx, loss):
     """Reference FIX encoder at 32 kHz -> (receiver under the loss process) -> host model and the reference decoders, float
     and (40 ms packets, joint mode 1) fixed point, over eight signal classes: every packet's PCM identical (0 LSB)."""
-    from tests.ref32 import Ref32Decoder, Ref32Encoder
     n = 24 if cfg["framesize_ms"] == 40 else 40
     kinds = ["flp"] + (["fix"] if cfg["framesize_ms"] == 40 else [])
     for s, (name, x) in enumerate(signals32(n)):
-        e = Ref32Encoder("fix", rate=rate, dtx=dtx, use_md_index=mdi, **cfg)
+        e = ref.RefEncoder("fix", rate=rate, dtx=dtx, use_md_index=mdi, samplerate=32000, **cfg)
         k = e.samples
         pk = [e.encode(x[p * k:(p + 1) * k]) for p in range(n)]
         e.close()
         fl = flags_for(loss, n, s)
         for kind in kinds:
-            dr = Ref32Decoder(kind, use_md_index=mdi, **cfg)
+            dr = ref.RefDecoder(kind, use_md_index=mdi, samplerate=32000, **cfg)
             ds = sim.SimDecoder(use_md_index=mdi, arith=kind, samplerate=32000, **cfg)
             for p, (b, nb, _) in enumerate(pk):
                 rx = receive(b, nb, fl[p])
@@ -152,7 +144,7 @@ def test_32k_decoder_survives_malformed_packets_under_asan(tmp_path):
     """The ASan / UBSan fuzzer of tests/hostsim/fuzz_dec.cpp with the fixture's 32 kHz packets as its corpus: bit flips,
     garbage, lying lengths, short rows and invalid flags into the 32 kHz decoders of both arithmetics (float 40 ms, 20 ms
     and joint mode 1; fixed point 40 ms and joint mode 1).  Every mode both decodes and rejects some of them."""
-    f = load32()
+    f = mk.load()
     corpus = tmp_path / "corpus32.bit"
     with open(corpus, "wb") as out:
         for s in mk.STREAMS:

@@ -1,121 +1,105 @@
-"""Core output of 32 kHz streams on the CPU: the host build of the core-output decode (tests/hostsim, dec_packet<16, true> of
+"""Core output of 32 kHz streams on the CPU: the host model's core-output decoder (tests/hostsim, dec_packet<16, true> of
 sb_dec.cuh) against the low band the reference's decoders hand to their synthesis filter bank, at 0 LSB.
 
 The reference is tapped, not changed: oracle/lowband.mk links its untouched sources with -Wl,--wrap=AGR_Sate_qmf_synth, and
-tests.core32.Ref32LowbandDecoder reads what the wrapper recorded (the float build's `lowout`, the fixed-point build's
-`OutLow`)."""
-import os
-
+oracle.ref.RefDecoder(..., samplerate=32000, out_samplerate=16000) returns what the wrapper recorded (the float build's
+`lowout`, the fixed-point build's `OutLow`)."""
 import numpy as np
 import pytest
 
-from tests.core32 import MODE_IDS, MODES, malformed_sequence, mixed_loss, stream_of, tap  # noqa: F401  (tap: fixture)
+from tests.core32 import CORE, MODE_IDS, MODES, malformed_sequence, mixed_loss, stream_of, tap  # noqa: F401  (tap: fixture)
 from tests.golden import make_golden_32k as mk
-from tests.hostsim.core import SimCoreDecoder
 from tests.parity import ref, sim  # noqa: F401  (fixtures)
-from tests.util import GOLDEN, load_clip, load_golden, receive
+from tests.util import load_clip, load_golden, receive, upsample2
 
 
-def load32():
-    return np.load(os.path.join(GOLDEN, "golden_32k.npz"))
-
-
-def stream_cfg(stream):
-    return mk.STREAMS[stream][1]
-
-
-def rx_of(pk, flags):
-    """What the receiver hands the decoder for each packet (a DTX packet concealed as lost)."""
-    return [receive(b, nb, f) for (b, nb), f in zip(pk, flags)]
-
-
-def core_lockstep(tap, kind, cfg, rx, tag=()):
-    """The tapped reference decoder and the host model's core output over the same received packets: both return 0, and
-    every row equals the reference's low band (0 LSB).  Returns the number of rows compared."""
-    dr = tap(kind, **cfg)
-    ds = SimCoreDecoder(arith=kind, **cfg)
+def core_lockstep(ref, sim, kind, cfg, pk, flags, tag=()):
+    """The tapped reference decoder and the host model's core output over what the receiver makes of the packets pk under
+    flags: both return 0, and every row equals the reference's low band (0 LSB).  Returns the number of rows compared."""
+    dr = ref.RefDecoder(kind, **CORE, **cfg)
+    ds = sim.SimDecoder(arith=kind, **CORE, **cfg)
     assert ds.pcm.size == 16 * cfg["framesize_ms"]
-    for p, x in enumerate(rx):
-        (_, ra), (y, rb) = dr.decode(*x), ds.decode(*x)
+    for p, ((b, nb), fl) in enumerate(zip(pk, flags)):
+        x = receive(b, nb, fl)
+        (low, ra), (y, rb) = dr.decode(*x), ds.decode(*x)
         assert ra == rb == 0, (kind, p, ra, rb) + tuple(tag)
-        assert dr.low is not None and np.array_equal(y, dr.low), \
-            (kind, p, "core row differs from the reference's low band (0 LSB bar)", int(np.abs(y.astype(int) - dr.low).max())) + tuple(tag)
+        assert low.size == y.size and np.array_equal(y, low), \
+            (kind, p, "core row differs from the reference's low band (0 LSB bar)", int(np.abs(y.astype(int) - low).max())) + tuple(tag)
     dr.close(), ds.close()
-    return len(rx)
+    return len(pk)
 
 
 CASES = mk.decode_cases()
 
 
 @pytest.mark.parametrize("key,stream,kind,rule", CASES, ids=[c[0] for c in CASES])
-def test_tap_leaves_the_reference_pcm_alone(tap, key, stream, kind, rule):
+def test_tap_leaves_the_reference_pcm_alone(ref, tap, key, stream, kind, rule):
     """The tapped library decodes every pinned 32 kHz decode exactly as the untapped one (the fixture's per-packet md5),
     and records a low band of 16 * framesize_ms samples for every packet."""
-    f = load32()
-    d = tap(kind, **stream_cfg(stream))
+    f = mk.load()
+    d = ref.RefDecoder(kind, **CORE, **mk.STREAMS[stream][1])
     lows = []
 
     class Recording:
         def decode(self, *a):
-            y, r = d.decode(*a)
-            lows.append(d.low)
-            return y, r
+            low, r = d.decode(*a)
+            lows.append(low)
+            return d.full, r
 
         def close(self):
             d.close()
     rows = mk.decode(Recording(), mk.packets(f, stream), mk.flags_of(f, stream, rule))
     assert (mk.packet_md5(rows) == f[key + "_packet_md5"]).all()
-    assert all(x is not None and x.size == 16 * stream_cfg(stream)["framesize_ms"] for x in lows)
+    assert all(x.size == 16 * mk.STREAMS[stream][1]["framesize_ms"] for x in lows)
 
 
 @pytest.mark.parametrize("key,stream,kind,rule", CASES, ids=[c[0] for c in CASES])
-def test_core_rows_equal_the_reference_low_band(tap, key, stream, kind, rule):
+def test_core_rows_equal_the_reference_low_band(ref, sim, tap, key, stream, kind, rule):
     """Every stream of golden_32k.npz under each of its pinned lostflag sequences, in the arithmetic of that decode."""
-    f = load32()
+    f = mk.load()
     pk, flags = mk.packets(f, stream), mk.flags_of(f, stream, rule)
-    assert core_lockstep(tap, kind, stream_cfg(stream), rx_of(pk, flags), (key,)) == len(pk)
+    assert core_lockstep(ref, sim, kind, mk.STREAMS[stream][1], pk, flags, (key,)) == len(pk)
 
 
 @pytest.mark.parametrize("name,cfg,kind", MODES, ids=MODE_IDS)
-def test_core_rows_under_mixed_loss(tap, name, cfg, kind):
+def test_core_rows_under_mixed_loss(ref, sim, tap, name, cfg, kind):
     """Every fixture stream of the configuration under its own mixed loss process over lostflags 1 / 2 / 3 / 4."""
-    f = load32()
-    streams = [s for s in mk.STREAMS if stream_cfg(s) == cfg]
+    f = mk.load()
+    streams = [s for s in mk.STREAMS if mk.STREAMS[s][1] == cfg]
     assert streams
     for i, s in enumerate(streams):
         pk = mk.packets(f, s)
         fl = mixed_loss(len(pk), seed=40 + i)
         assert {1, 2, 3, 4} <= set(fl)
-        core_lockstep(tap, kind, cfg, rx_of(pk, fl), (s,))
+        core_lockstep(ref, sim, kind, cfg, pk, fl, (s,))
 
 
 @pytest.mark.parametrize("name,cfg,kind", MODES, ids=MODE_IDS)
-def test_core_rows_with_dtx(tap, name, cfg, kind):
+def test_core_rows_with_dtx(ref, sim, tap, name, cfg, kind):
     """The reference FIX encoder at 32 kHz with DTX on speech fading to silence (DTX packets are concealed as lost, comfort
     noise follows), clean and under the mixed loss process."""
-    from tests.ref32 import Ref32Encoder, upsample2
     clip = load_clip()
     n = 30 if cfg["framesize_ms"] == 40 else 50
     k = 32 * cfg["framesize_ms"]
     L = n * k
     t = np.arange(L)
     x = (upsample2(clip)[:L] * np.clip(1.0 - t / (0.5 * L), 0, 1)).astype(np.int16)
-    e = Ref32Encoder("fix", rate=24000, dtx=1, **cfg)
+    e = ref.RefEncoder("fix", rate=24000, dtx=1, samplerate=32000, **cfg)
     pk = [e.encode(x[p * k:(p + 1) * k])[:2] for p in range(n)]
     e.close()
     assert sum(nb[0] <= 0 for _, nb in pk) >= 3, "the signal must produce DTX packets"
-    core_lockstep(tap, kind, cfg, rx_of(pk, [4] * n), ("dtx",))
-    core_lockstep(tap, kind, cfg, rx_of(pk, mixed_loss(n, seed=77)), ("dtx", "loss"))
+    core_lockstep(ref, sim, kind, cfg, pk, [4] * n, ("dtx",))
+    core_lockstep(ref, sim, kind, cfg, pk, mixed_loss(n, seed=77), ("dtx", "loss"))
 
 
 @pytest.mark.parametrize("name,cfg,kind", MODES, ids=MODE_IDS)
 def test_return_codes_equal_the_full_band_decoders(ref, sim, name, cfg, kind):
     """Damaged and other-core packets between good ones: the core-output host model returns exactly what the full-band
     one returns for every packet (-12 for the other cores), and both reject some and decode some."""
-    f, g = load32(), load_golden()
+    f, g = mk.load(), load_golden()
     stream = stream_of(cfg)
     seq = malformed_sequence(f, g, stream, 40, seed=5)
-    core = SimCoreDecoder(arith=kind, **cfg)
+    core = sim.SimDecoder(arith=kind, **CORE, **cfg)
     full = sim.SimDecoder(arith=kind, samplerate=32000, **cfg)
     rets = []
     for p, (b, nb, fl) in enumerate(seq):

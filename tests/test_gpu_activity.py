@@ -2,15 +2,14 @@
 the PCM row it reports on, every flags byte the host model's (tests/hostsim), and the packet calls' outputs
 and launch counts are the same with and without activity calls."""
 import hashlib
-import os
 
 import numpy as np
 import pytest
 
 from solo_b200 import api
 from tests.golden import make_golden_32k as mk
-from tests.parity import sb, sim  # noqa: F401  (fixtures)
-from tests.util import GOLDEN, load_clip, load_golden, loss_flags, receive, signal_classes
+from tests.parity import DeviceDecoder, batch_rows, received, sb, sim  # noqa: F401  (fixtures)
+from tests.util import load_clip, load_golden, loss_flags, receive, signal_classes
 
 pytestmark = pytest.mark.gpu
 CAP = 256
@@ -81,7 +80,7 @@ def test_clip_payloads_with_activity_calls_equal_the_reference(sb):
 
 def dec_cases():
     """(name, samplerate, decoder kwargs, arith, packets, pinned md5 key or None, pinned flags or None)."""
-    g, f = load_golden(), np.load(os.path.join(GOLDEN, "golden_32k.npz"))
+    g, f = load_golden(), mk.load()
     pk16 = [(bytes(g["fix_bits"][p, :int(g["fix_nbytes"][p, 0])]), tuple(int(v) for v in g["fix_nbytes"][p])) for p in range(60)]
     out = [("16k-40ms-flp", 16000, dict(framesize_ms=40), "flp", pk16, None, None)]
     for s, arith in (("hb40", "flp"), ("hb40", "fix"), ("hb20", "flp"), ("joint", "flp"), ("joint", "fix")):
@@ -104,42 +103,28 @@ def test_decoder_batches_under_per_stream_loss(sb, sim, case):
     """N = 64 streams per batch, each under its own 50 % loss process (row 0: the fixture's loss flags), through decode +
     activity (host) and decode_device + activity_device: level = the host function of the output rows, flags = the host
     model's, PCM = the host model's (row 0: the fixture's md5); chunking (1 or 3) changes nothing."""
-    import torch
     cases = dec_cases()
     cases += [("16k-20ms-flp", 16000, dict(framesize_ms=20), "flp", enc16(sim, dict(framesize_ms=20)), None, None),
               ("16k-joint-fix", 16000, dict(framesize_ms=40, joint_hb=1), "fix", enc16(sim, dict(framesize_ms=40, joint_hb=1)), None, None)]
     name, sr, cfg, arith, pk, md5key, pinned = cases[case]
-    f32 = np.load(os.path.join(GOLDEN, "golden_32k.npz"))
+    f32 = mk.load()
     N, T = 64, len(pk)
     flags = np.array([loss_flags(T, 50, seed=40 + s) for s in range(N)], np.int32)
     if pinned is not None:
         flags[0] = pinned
     dh = sb.DecoderBatch(N, arith=arith, samplerate=sr, **cfg)
-    dd = sb.DecoderBatch(N, arith=arith, samplerate=sr, **cfg)
+    dd = DeviceDecoder(sb.DecoderBatch(N, arith=arith, samplerate=sr, **cfg), CAP)
     hm = [sim.SimDecoder(arith=arith, samplerate=sr, **cfg) for _ in range(N)]
-    S = dh.samples
-    dev = torch.device("cuda", 0)
-    d_pcm = torch.zeros((N, S), dtype=torch.int16, device=dev)
-    d_ret = torch.zeros(N, dtype=torch.int32, device=dev)
-    d_lv = torch.zeros(N, dtype=torch.uint8, device=dev)
-    d_fl = torch.zeros(N, dtype=torch.uint8, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
     for p in range(T):
         sb.set_chunks(1 if p % 2 else 3)
         rx = [receive(pk[p][0], pk[p][1], int(flags[s, p])) for s in range(N)]
-        tb = np.zeros((N, CAP), np.uint8)
-        for s, (b, nb, fl) in enumerate(rx):
-            tb[s, :len(b)] = np.frombuffer(b, np.uint8)
-        tnb = np.array([r[1] for r in rx], np.int16)
-        tf = np.array([r[2] for r in rx], np.int32)
+        tb, tnb, tf = batch_rows(rx, CAP)
         pcm, ret = dh.decode(tb, tnb, tf)
         lv, fl = dh.activity()
         assert (ret == 0).all()
-        t_b, t_nb, t_f = (torch.from_numpy(a).to(dev) for a in (tb, tnb, tf))
-        dd.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), d_ret.data_ptr(), st)
-        dd.activity_device(d_pcm.data_ptr(), d_lv.data_ptr(), d_fl.data_ptr(), st)
-        torch.cuda.synchronize()
-        assert np.array_equal(d_pcm.cpu().numpy(), pcm) and np.array_equal(d_lv.cpu().numpy(), lv) and np.array_equal(d_fl.cpu().numpy(), fl), (name, p)
+        d_pcm, _ = dd.decode(tb, tnb, tf)
+        d_lv, d_fl = dd.activity()
+        assert np.array_equal(d_pcm, pcm) and np.array_equal(d_lv, lv) and np.array_equal(d_fl, fl), (name, p)
         assert np.array_equal(lv, levels(sim, pcm)), (name, p)
         for s in range(N):
             y, r = hm[s].decode(*rx[s])
@@ -149,7 +134,7 @@ def test_decoder_batches_under_per_stream_loss(sb, sim, case):
         conc = 0xC if cfg["framesize_ms"] == 40 else 0x4
         assert np.array_equal(fl & conc != 0, tf == 1), (name, p)
     sb.set_chunks(0)
-    dh.close(), dd.close()
+    dh.close(), dd.db.close()
     for h in hm:
         h.close()
 
@@ -164,23 +149,12 @@ def test_sample_of_a_65536_stream_batch(sb, sim):
     lost = np.random.Generator(np.random.PCG64(67)).random((T, N)) < 0.5
     db = sb.DecoderBatch(N)
     hm = [sim.SimDecoder() for _ in rows]
-    dev = torch.device("cuda", 0)
-    d_pcm = torch.zeros((N, 640), dtype=torch.int16, device=dev)
-    d_lv = torch.zeros(N, dtype=torch.uint8, device=dev)
-    d_fl = torch.zeros(N, dtype=torch.uint8, device=dev)
-    idx = torch.from_numpy(rows).to(dev)
-    st = torch.cuda.current_stream().cuda_stream
+    dev = DeviceDecoder(db, CAP)
     for p in range(T):
         n0 = int(g["fix_nbytes"][p, 0])
-        row = np.zeros(CAP, np.uint8)
-        row[:n0] = g["fix_bits"][p, :n0]
-        t_b = torch.from_numpy(row).to(dev).expand(N, CAP).contiguous()
-        t_nb = torch.from_numpy(g["fix_nbytes"][p].astype(np.int16)).to(dev).expand(N, 2).contiguous()
-        t_f = torch.from_numpy(np.where(lost[p], 1, 4).astype(np.int32)).to(dev)
-        db.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), 0, st)
-        db.activity_device(d_pcm.data_ptr(), d_lv.data_ptr(), d_fl.data_ptr(), st)
-        torch.cuda.synchronize()
-        pcm, lv, fl = d_pcm[idx].cpu().numpy(), d_lv[idx].cpu().numpy(), d_fl[idx].cpu().numpy()
+        tb, tnb, _ = batch_rows([(bytes(g["fix_bits"][p, :n0]), g["fix_nbytes"][p], 4)], CAP)      # broadcast on the device
+        pcm, _ = dev.decode(tb, tnb, np.where(lost[p], 1, 4), rows=rows)
+        lv, fl = dev.activity(rows=rows)
         assert np.array_equal(lv, levels(sim, pcm)), p
         for i, s in enumerate(rows):
             y, r = hm[i].decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 1 if lost[p, s] else 4)
@@ -188,14 +162,14 @@ def test_sample_of_a_65536_stream_batch(sb, sim):
     db.close()
     for h in hm:
         h.close()
-    del d_pcm
+    del dev
     torch.cuda.empty_cache()
 
 
 def test_drop_in_handles_report_what_the_batch_row_reports(sb):
     """Encoder handles and 16 / 32 kHz decoder handles report, packet by packet, the level / flags of a batch row that codes
     the same stream; before their first packet, and for NULL or foreign handles, the calls fail."""
-    f = np.load(os.path.join(GOLDEN, "golden_32k.npz"))
+    f = mk.load()
     clip = load_clip()
     he = sb.SoloEncoder(rate=13600, dtx=1)
     h16, h32 = sb.SoloDecoder(), sb.SoloDecoder(samplerate=32000)
@@ -216,15 +190,11 @@ def test_drop_in_handles_report_what_the_batch_row_reports(sb):
         assert he.last_activity() == tuple(int(a[1]) for a in eb.activity()), p
         rx = receive(b, nb, fl16[p])
         y, r = h16.decode(*rx)
-        row = np.zeros((2, CAP), np.uint8)
-        row[:, :len(rx[0])] = np.frombuffer(rx[0], np.uint8)
-        d16.decode(row, np.tile(np.array(rx[1], np.int16), (2, 1)), np.full(2, rx[2], np.int32))
+        d16.decode(*batch_rows([rx] * 2, CAP))
         assert h16.last_activity() == tuple(int(a[0]) for a in d16.activity()), p
         rx = receive(pk32[p][0], pk32[p][1], fl32[p])
         y, r = h32.decode(*rx)
-        row = np.zeros((2, CAP), np.uint8)
-        row[:, :len(rx[0])] = np.frombuffer(rx[0], np.uint8)
-        d32.decode(row, np.tile(np.array(rx[1], np.int16), (2, 1)), np.full(2, rx[2], np.int32))
+        d32.decode(*batch_rows([rx] * 2, CAP))
         assert h32.last_activity() == tuple(int(a[1]) for a in d32.activity()), p
     assert sb.lib().solo_b200_encoder_last_activity(h16.h, lv.ctypes.data, lv.ctypes.data) == -1     # foreign handle
     for o in (he, h16, h32, eb, d16, d32):
@@ -234,17 +204,14 @@ def test_drop_in_handles_report_what_the_batch_row_reports(sb):
 def test_malformed_rows_report_127_and_no_flags(sb):
     """A 32 kHz batch whose odd rows get garbage, 16 kHz streams' packets, lying lengths or bad lostflags: the even rows
     report what a clean batch's do, and every rejected row reports level 127 and flags 0."""
-    f, g = np.load(os.path.join(GOLDEN, "golden_32k.npz")), load_golden()
+    f, g = mk.load(), load_golden()
     pk = mk.packets(f, "hb40")
     N = 200
     rng = np.random.Generator(np.random.PCG64(12))
     clean, mixed = sb.DecoderBatch(N, samplerate=32000), sb.DecoderBatch(N, samplerate=32000)
     rejected = 0
     for p in range(30):
-        b, nb, fl = receive(pk[p][0], pk[p][1], 4)
-        tb = np.zeros((N, CAP), np.uint8)
-        tb[:, :len(b)] = np.frombuffer(b, np.uint8)
-        tnb, tf = np.tile(np.array(nb, np.int16), (N, 1)), np.full(N, fl, np.int32)
+        tb, tnb, tf = received([pk[p]] * N, [4] * N, CAP)
         pc, rc = clean.decode(tb, tnb, tf)
         lc, fc = clean.activity()
         mb, mnb, mf = tb.copy(), tnb.copy(), tf.copy()

@@ -2,8 +2,6 @@
 batched host and device entry points, the drop-in handles and the state hand-over, in both decoder arithmetics.  Every PCM
 comparison is exact (0 LSB): against golden_32k.npz's per-packet md5, or against the reference's decoders in oracle/_ref."""
 import ctypes as C
-import hashlib
-import os
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -11,30 +9,11 @@ import pytest
 
 from solo_b200 import api
 from tests.golden import make_golden_32k as mk
-from tests.parity import received, ref, sb  # noqa: F401  (fixtures)
-from tests.util import GOLDEN, load_golden, loss_flags, receive
+from tests.parity import DeviceDecoder, batch_rows, received, ref, sb  # noqa: F401  (fixtures)
+from tests.util import load_golden, loss_flags, receive
 
 pytestmark = pytest.mark.gpu
 CAP = 256
-
-
-def load32():
-    return np.load(os.path.join(GOLDEN, "golden_32k.npz"))
-
-
-def md5_rows(pcm):
-    """uint8 [rows, 16]: md5 of every row's int16 PCM."""
-    return np.array([np.frombuffer(hashlib.md5(np.ascontiguousarray(r).tobytes()).digest(), np.uint8) for r in pcm])
-
-
-def rx_packet(pk, flag):
-    """(payload row, nbytes, lostflag) the receiver hands the decoder for one fixture packet (DTX: concealed as lost)."""
-    b, nb = pk
-    pb, pnb, f = receive(b, nb, flag)
-    row = np.zeros(CAP, np.uint8)
-    row[:len(pb)] = np.frombuffer(pb, np.uint8)
-    return row, pnb, f
-
 
 CASES = mk.decode_cases()
 
@@ -43,8 +22,7 @@ CASES = mk.decode_cases()
 def test_fixture_on_batched_host_and_device_calls(sb, key, stream, kind, rule):
     """N = 257 streams that all decode one fixture stream, through decode_host and decode_device: every row of every
     packet has the reference's PCM (per-packet md5, 0 LSB)."""
-    import torch
-    f = load32()
+    f = mk.load()
     cfg = mk.STREAMS[stream][1]
     pk, flags = mk.packets(f, stream), mk.flags_of(f, stream, rule)
     want = f[key + "_packet_md5"]
@@ -52,21 +30,13 @@ def test_fixture_on_batched_host_and_device_calls(sb, key, stream, kind, rule):
     dh = sb.DecoderBatch(N, arith=kind, samplerate=32000, **cfg)
     dd = sb.DecoderBatch(N, arith=kind, samplerate=32000, **cfg)
     assert dh.samples == 32 * cfg["framesize_ms"]
-    dev = torch.device("cuda", 0)
-    d_pcm = torch.zeros((N, dh.samples), dtype=torch.int16, device=dev)
-    d_ret = torch.full((N,), -99, dtype=torch.int32, device=dev)
+    dev = DeviceDecoder(dd, CAP)
     for p in range(len(pk)):
-        row, pnb, fl = rx_packet(pk[p], flags[p])
-        tb, tnb, tf = np.tile(row, (N, 1)), np.tile(np.array(pnb, np.int16), (N, 1)), np.full(N, fl, np.int32)
+        tb, tnb, tf = received([pk[p]] * N, [flags[p]] * N, CAP)
         pcm, ret = dh.decode(tb, tnb, tf)
         assert (ret == 0).all(), p
-        assert (md5_rows(pcm) == want[p]).all(), ("host entry point: PCM differs from the reference's (0 LSB bar)", key, p)
-        t_b, t_nb, t_f = (torch.from_numpy(a).to(dev) for a in (tb, tnb, tf))
-        dd.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), d_ret.data_ptr(),
-                         torch.cuda.current_stream().cuda_stream)
-        torch.cuda.synchronize()
-        assert int((d_ret != 0).sum().item()) == 0, p
-        assert np.array_equal(d_pcm.cpu().numpy(), pcm), ("device entry point differs from host entry point", key, p)
+        assert (mk.packet_md5(pcm) == want[p]).all(), ("host entry point: PCM differs from the reference's (0 LSB bar)", key, p)
+        assert np.array_equal(dev.decode(tb, tnb, tf)[0], pcm), ("device entry point differs from host entry point", key, p)
     dh.close(), dd.close()
 
 
@@ -75,30 +45,20 @@ def test_fixture_on_a_65536_stream_batch(sb, arith, stream, rule):
     """One wave of 65 536 32 kHz streams through decode_device; a fixed sample of 1 024 rows (first, last and spread) is
     checked against the fixture's per-packet md5 (0 LSB) for the first 30 packets."""
     import torch
-    f = load32()
+    f = mk.load()
     cfg = mk.STREAMS[stream][1]
     key = "%s_%s_%s" % (arith, stream, rule)
     pk, flags, want = mk.packets(f, stream), mk.flags_of(f, stream, rule), f[key + "_packet_md5"]
     N = 65536
     rows = np.unique(np.concatenate([[0, N - 1], np.random.Generator(np.random.PCG64(65)).choice(N, 1022, replace=False)]))
     db = sb.DecoderBatch(N, arith=arith, samplerate=32000, **cfg)
-    dev = torch.device("cuda", 0)
-    d_pcm = torch.zeros((N, db.samples), dtype=torch.int16, device=dev)
-    d_ret = torch.full((N,), -99, dtype=torch.int32, device=dev)
-    idx = torch.from_numpy(rows).to(dev)
+    dev = DeviceDecoder(db, CAP)
     for p in range(30):
-        row, pnb, fl = rx_packet(pk[p], flags[p])
-        t_b = torch.from_numpy(row).to(dev).expand(N, CAP).contiguous()
-        t_nb = torch.tensor(pnb, dtype=torch.int16, device=dev).expand(N, 2).contiguous()
-        t_f = torch.full((N,), fl, dtype=torch.int32, device=dev)
-        db.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), d_ret.data_ptr(),
-                         torch.cuda.current_stream().cuda_stream)
-        torch.cuda.synchronize()
-        assert int((d_ret != 0).sum().item()) == 0, p
-        got = md5_rows(d_pcm[idx].cpu().numpy())
+        pcm, _ = dev.decode(*received([pk[p]], [flags[p]], CAP), rows=rows)      # one row, broadcast on the device
+        got = mk.packet_md5(pcm)
         assert (got == want[p]).all(), ("PCM differs from the reference's (0 LSB bar)", key, p, int(rows[np.argmax((got != want[p]).any(1))]))
     db.close()
-    del d_pcm
+    del dev
     torch.cuda.empty_cache()
 
 
@@ -108,12 +68,11 @@ def test_per_stream_loss_against_reference(sb, ref, cfg):
     """N = 97 streams, each its own signal (the fixture's input at its own offset, FIX-encoded at 32 kHz by the reference)
     and its own 50 % loss process; every row of every packet equal to the reference's float decoder and, where that mode
     exists, to its fixed-point decoder (0 LSB)."""
-    from tests.ref32 import Ref32Decoder, Ref32Encoder
     x = mk.inputs()["hb"]
     N, T = 97, 16
     kinds = ["flp"] + (["fix"] if cfg["framesize_ms"] == 40 else [])
     pool = ThreadPoolExecutor(32)
-    enc = [Ref32Encoder("fix", rate=16000 + 1000 * (s % 9), **cfg) for s in range(N)]
+    enc = [ref.RefEncoder("fix", rate=16000 + 1000 * (s % 9), samplerate=32000, **cfg) for s in range(N)]
     k = enc[0].samples
     off = [(s * 7919) % (len(x) - k * T) for s in range(N)]
     pk = []
@@ -122,7 +81,7 @@ def test_per_stream_loss_against_reference(sb, ref, cfg):
     flags = np.array([loss_flags(T, 50, seed=31 + s) for s in range(N)], np.int32)
     for kind in kinds:
         db = sb.DecoderBatch(N, arith=kind, samplerate=32000, **cfg)
-        rd = [Ref32Decoder(kind, **cfg) for _ in range(N)]
+        rd = [ref.RefDecoder(kind, samplerate=32000, **cfg) for _ in range(N)]
         for p in range(T):
             tb, tnb, tf = received(pk[p], flags[:, p], CAP)
             pcm, ret = db.decode(tb, tnb, tf)
@@ -140,7 +99,7 @@ def test_per_stream_loss_against_reference(sb, ref, cfg):
 
 def test_chunking_does_not_change_pcm(sb):
     """The host entry point's pipelining (1, 3 and 7 chunks) gives the same PCM on a 32 kHz batch."""
-    f = load32()
+    f = mk.load()
     pk, flags = mk.packets(f, "hb40"), mk.flags_of(f, "hb40", "loss")
     N = 6000
     out = {}
@@ -149,11 +108,9 @@ def test_chunking_does_not_change_pcm(sb):
         db = sb.DecoderBatch(N, samplerate=32000)
         res = []
         for p in range(12):
-            row, pnb, fl = rx_packet(pk[p], flags[p])
+            tb, tnb, tf = received([pk[p]] * N, [flags[p]] * N, CAP)
             # rows differ: stream s starts s % 5 packets later into the lossy sequence (lost packets in its place before)
-            tb = np.tile(row, (N, 1))
-            tnb = np.tile(np.array(pnb, np.int16), (N, 1))
-            tf = np.where(np.arange(N) % 5 > p, 1, fl).astype(np.int32)
+            tf = np.where(np.arange(N) % 5 > p, 1, tf).astype(np.int32)
             pcm, ret = db.decode(tb, tnb, tf)
             assert (ret == 0).all()
             res.append(pcm.copy())
@@ -166,7 +123,7 @@ def test_chunking_does_not_change_pcm(sb):
 def test_state_export_import_and_refused_cross_rate(sb):
     """A 32 kHz stream's state moved mid-stream into another batch continues bit for bit; a 16 kHz blob is refused by a 32
     kHz batch and a 32 kHz blob by a 16 kHz batch, with nothing copied."""
-    f = load32()
+    f = mk.load()
     pk, flags, want = mk.packets(f, "hb40"), mk.flags_of(f, "hb40", "loss"), f["flp_hb40_loss_packet_md5"]
     assert sb.dec_state_bytes(32000) > sb.dec_state_bytes(16000) == sb.state_bytes()[1]
     a = sb.DecoderBatch(4, samplerate=32000)
@@ -174,9 +131,7 @@ def test_state_export_import_and_refused_cross_rate(sb):
     d16 = sb.DecoderBatch(2)
 
     def step(batch, p):
-        row, pnb, fl = rx_packet(pk[p], flags[p])
-        n = batch.n
-        pcm, ret = batch.decode(np.tile(row, (n, 1)), np.tile(np.array(pnb, np.int16), (n, 1)), np.full(n, fl, np.int32))
+        pcm, ret = batch.decode(*received([pk[p]] * batch.n, [flags[p]] * batch.n, CAP))
         assert (ret == 0).all()
         return pcm
     for p in range(20):
@@ -192,7 +147,7 @@ def test_state_export_import_and_refused_cross_rate(sb):
         b.import_state(0, before16)
     for p in range(20, 40):
         pa, pb = step(a, p), step(b, p)
-        assert (md5_rows(pa) == want[p]).all() and (md5_rows(pb[1:2]) == want[p]).all(), p
+        assert (mk.packet_md5(pa) == want[p]).all() and (mk.packet_md5(pb[1:2]) == want[p]).all(), p
     a.close(), b.close(), d16.close()
 
 
@@ -200,7 +155,7 @@ def test_drop_in_handles_of_both_rates_at_once(sb):
     """AGR_Sate_Decoder_Init handles of 16 and 32 kHz streams alive together (their arena segments never shared), each
     decoding its fixture: 32 kHz ones give nSamplesOut = 1280 and the reference float build's PCM (0 LSB), 16 kHz ones
     golden.npz's.  The encoder refuses 32 kHz with the reason in solo_b200_last_error()."""
-    f, g = load32(), load_golden()
+    f, g = mk.load(), load_golden()
     pk32, fl32, want32 = mk.packets(f, "hb40"), mk.flags_of(f, "hb40", "mode4"), f["flp_hb40_mode4_packet_md5"]
     h32 = [sb.SoloDecoder(samplerate=32000) for _ in range(3)]
     h16 = [sb.SoloDecoder() for _ in range(2)]
@@ -209,7 +164,7 @@ def test_drop_in_handles_of_both_rates_at_once(sb):
             b, nb = pk32[p]
             y, r = h.decode(b, nb, fl32[p])
             assert r == 0 and h.last_nsamples == 1280 and y.shape == (1280,)
-            assert (md5_rows(y[None]) == want32[p]).all(), p
+            assert (mk.packet_md5(y[None]) == want32[p]).all(), p
         n0 = int(g["fix_nbytes"][p, 0])
         for h in h16:
             y, r = h.decode(bytes(g["fix_bits"][p, :n0]), tuple(int(v) for v in g["fix_nbytes"][p]), 4)
@@ -230,7 +185,7 @@ def test_drop_in_handles_of_both_rates_at_once(sb):
 def test_drop_in_fixed_point_arithmetic_from_environment(sb, monkeypatch):
     """SOLO_B200_DEC_ARITH=fix makes 32 kHz handles decode to the reference fixed-point build's PCM (0 LSB); 20 ms packets
     are refused in that mode, as at 16 kHz."""
-    f = load32()
+    f = mk.load()
     monkeypatch.setenv("SOLO_B200_DEC_ARITH", "fix")
     for stream in ("hb40", "joint"):
         cfg = mk.STREAMS[stream][1]
@@ -241,7 +196,7 @@ def test_drop_in_fixed_point_arithmetic_from_environment(sb, monkeypatch):
             b, nb = pk[p]
             pb, pnb, fl_p = receive(b, nb, fl[p])
             y, r = h.decode(pb, pnb, fl_p)
-            assert r == 0 and (md5_rows(y[None]) == want[p]).all(), (stream, p)
+            assert r == 0 and (mk.packet_md5(y[None]) == want[p]).all(), (stream, p)
         h.close()
     with pytest.raises(sb.SoloError):
         sb.SoloDecoder(samplerate=32000, framesize_ms=20)
@@ -250,38 +205,28 @@ def test_drop_in_fixed_point_arithmetic_from_environment(sb, monkeypatch):
 def test_apply_loss_device_feeds_a_32k_batch(sb):
     """Untrimmed fixture rows and per-row lostflags -> apply_loss_device -> decode_device: the fixture's lossy PCM (0 LSB)."""
     import torch
-    f = load32()
+    f = mk.load()
     pk, flags, want = mk.packets(f, "hb40"), mk.flags_of(f, "hb40", "loss"), f["flp_hb40_loss_packet_md5"]
     N = 129
     db = sb.DecoderBatch(N, samplerate=32000)
-    dev = torch.device("cuda", 0)
+    dev = DeviceDecoder(db, CAP)
     st = torch.cuda.current_stream().cuda_stream
-    d_pcm = torch.zeros((N, 1280), dtype=torch.int16, device=dev)
-    d_ret = torch.full((N,), -99, dtype=torch.int32, device=dev)
-    tb_out = torch.zeros((N, CAP), dtype=torch.uint8, device=dev)
-    tnb_out = torch.zeros((N, 2), dtype=torch.int16, device=dev)
     for p in range(40):
         b, nb = pk[p]
         fl = flags[p]
         if nb[0] <= 0:
             b, nb, fl = bytes(16), (16, 8), 1
-        row = np.zeros(CAP, np.uint8)
-        row[:len(b)] = np.frombuffer(b, np.uint8)
-        t_b = torch.from_numpy(np.tile(row, (N, 1))).to(dev)
-        t_nb = torch.from_numpy(np.tile(np.array(nb, np.int16), (N, 1))).to(dev)
-        t_f = torch.full((N,), fl, dtype=torch.int32, device=dev)
-        sb.apply_loss_device(t_b.data_ptr(), t_nb.data_ptr(), t_f.data_ptr(), tb_out.data_ptr(), tnb_out.data_ptr(), CAP, N, st)
-        db.decode_device(d_pcm.data_ptr(), tb_out.data_ptr(), CAP, tnb_out.data_ptr(), t_f.data_ptr(), d_ret.data_ptr(), st)
-        torch.cuda.synchronize()
-        assert int((d_ret != 0).sum().item()) == 0, p
-        assert (md5_rows(d_pcm.cpu().numpy()) == want[p]).all(), ("PCM differs (0 LSB bar)", p)
+        t_b, t_nb, t_f = (torch.from_numpy(a).cuda() for a in batch_rows([(b, nb, fl)] * N, CAP))
+        sb.apply_loss_device(t_b.data_ptr(), t_nb.data_ptr(), t_f.data_ptr(), dev.tb.data_ptr(), dev.tnb.data_ptr(), CAP, N, st)
+        pcm, _ = dev.decode(tf=t_f)
+        assert (mk.packet_md5(pcm) == want[p]).all(), ("PCM differs (0 LSB bar)", p)
     db.close()
 
 
 def test_malformed_rows_do_not_touch_their_neighbours(sb):
     """A 32 kHz batch whose odd rows get garbage, 16 kHz streams' packets (8 kHz core), lying lengths or short rows: the
     even rows decode exactly as a clean batch does (0 LSB), the bad rows report errors, and nothing faults."""
-    f, g = load32(), load_golden()
+    f, g = mk.load(), load_golden()
     pk = mk.packets(f, "hb40")
     N = 200
     rng = np.random.Generator(np.random.PCG64(12))
@@ -290,10 +235,7 @@ def test_malformed_rows_do_not_touch_their_neighbours(sb):
     bad_rows = np.arange(1, N, 2)
     errors = 0
     for p in range(30):
-        row, pnb, fl = rx_packet(pk[p], 4)
-        tb = np.tile(row, (N, 1))
-        tnb = np.tile(np.array(pnb, np.int16), (N, 1))
-        tf = np.full(N, fl, np.int32)
+        tb, tnb, tf = received([pk[p]] * N, [4] * N, CAP)
         pc, rc = clean.decode(tb, tnb, tf)
         assert (rc == 0).all()
         mb, mnb, mf = tb.copy(), tnb.copy(), tf.copy()

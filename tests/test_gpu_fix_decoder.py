@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
-from tests.parity import DevicePath, batch_packets, received, ref, sb  # noqa: F401  (fixtures)
+from tests.parity import DeviceDecoder, DevicePath, batch_packets, received, ref, sb  # noqa: F401  (fixtures)
 from tests.util import load_clip, load_golden, loss_flags, signal_classes, speech_replay, trim_payload
 
 pytestmark = pytest.mark.gpu
@@ -51,7 +51,6 @@ class RefFixRows:
 def test_odd_batch_with_per_stream_loss_matches_fixed_point_reference(sb, ref, joint, signal):
     """N = 257 streams (speech replay, or the eight signal classes in neighbouring streams), each with its own 50 % loss
     process; every row of decode_host and of decode_device against the fixed-point reference."""
-    import torch
     N, cap = 257, 320            # the 200 Hz sine class reaches 205 bytes per packet
     T = 40 if signal == "speech" else 25
     x = speech_replay(load_clip(), N, T) if signal == "speech" else signal_classes(load_clip(), N, T)
@@ -60,21 +59,14 @@ def test_odd_batch_with_per_stream_loss_matches_fixed_point_reference(sb, ref, j
     dh = sb.DecoderBatch(N, joint_hb=joint, arith="fix")
     dd = sb.DecoderBatch(N, joint_hb=joint, arith="fix")
     rr = RefFixRows(ref, range(N), joint_hb=joint)
-    dev = torch.device("cuda", 0)
-    d_pcm = torch.zeros((N, 640), dtype=torch.int16, device=dev)
-    d_ret = torch.full((N,), -99, dtype=torch.int32, device=dev)
+    dev = DeviceDecoder(dd, cap)
     for p in range(T):
         bits, nb = eb.encode(x[p], cap=cap)
         tb, tnb, tf = received(batch_packets(bits, nb), flags[:, p], cap)
         pcm, ret = dh.decode(tb, tnb, tf)
         assert (ret == 0).all(), p
         rr.check(tb, tnb, tf, pcm)
-        t_b, t_nb, t_f = (torch.from_numpy(a).to(dev) for a in (tb, tnb, tf))
-        dd.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), cap, t_nb.data_ptr(), t_f.data_ptr(), d_ret.data_ptr(),
-                         torch.cuda.current_stream().cuda_stream)
-        torch.cuda.synchronize()
-        assert int((d_ret != 0).sum().item()) == 0, p
-        assert np.array_equal(d_pcm.cpu().numpy(), pcm), p
+        assert np.array_equal(dev.decode(tb, tnb, tf)[0], pcm), p
     rr.close()
     eb.close(); dh.close(); dd.close()
 

@@ -2,15 +2,13 @@
 tolerance against the numpy restatement of tests/server_ref.py: random layouts at every row length, a 65 536-stream layout,
 argument checking, out-of-range members on the device path, 32 kHz rows, and a whole MCU tick (decode, activity, mix,
 downlink encode) on the device against the same tick through host calls and numpy mixing."""
-import os
-
 import numpy as np
 import pytest
 
 from tests.golden import make_golden_32k as mk
-from tests.parity import sb  # noqa: F401  (fixture)
+from tests.parity import DeviceDecoder, batch_packets, received, sb  # noqa: F401  (fixture)
 from tests.server_ref import POISON, csr, mixed_layout, numpy_mix, to_dev
-from tests.util import GOLDEN, load_clip, loss_flags, receive, signal_classes
+from tests.util import load_clip, loss_flags, signal_classes
 
 pytestmark = pytest.mark.gpu
 CAP = 256
@@ -168,37 +166,28 @@ def test_32khz_decoder_rows(sb):
     """A 32 kHz decoder batch (1 280-sample rows) decodes golden_32k.npz's hb40 packets under per-stream loss; its device
     rows, levels and flags go through mix_device and the result equals numpy on the same rows."""
     import torch
-    f = np.load(os.path.join(GOLDEN, "golden_32k.npz"))
-    pk = mk.packets(f, "hb40")
+    pk = mk.packets(mk.load(), "hb40")
     N, T, k = 64, 12, 3
     lost = np.array([loss_flags(T, 30, seed=80 + s) for s in range(N)], np.int32)
-    d = sb.DecoderBatch(N, samplerate=32000)
+    d = DeviceDecoder(sb.DecoderBatch(N, samplerate=32000), CAP)
     rooms = [np.arange(0, 40, 2), np.arange(1, 40, 2)[::-1], np.arange(40, 52), np.array([60])]
     rs, mb = csr(rooms)
     st = torch.cuda.current_stream().cuda_stream
-    d_pcm = torch.zeros((N, 1280), dtype=torch.int16, device=dev())
     d_out = torch.full((N, 1280), POISON, dtype=torch.int16, device=dev())
-    d_lv, d_fl = (torch.zeros(N, dtype=torch.uint8, device=dev()) for _ in range(2))
     d_rs, d_mb = to_dev(rs), to_dev(mb)
     d_tk = torch.zeros((len(rooms), k), dtype=torch.int32, device=dev())
     seen = 0
     for p in range(T):
-        rx = [receive(pk[p + 5][0], pk[p + 5][1], int(lost[s, p])) for s in range(N)]
-        tb = np.zeros((N, CAP), np.uint8)
-        for s, (b, nb, fl) in enumerate(rx):
-            tb[s, :len(b)] = np.frombuffer(b, np.uint8)
-        t_b, t_nb, t_f = to_dev(tb), to_dev(np.array([r[1] for r in rx], np.int16)), to_dev(np.array([r[2] for r in rx], np.int32))
-        d.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), 0, st)
-        d.activity_device(d_pcm.data_ptr(), d_lv.data_ptr(), d_fl.data_ptr(), st)
-        sb.mix_device(d_pcm.data_ptr(), d_out.data_ptr(), 1280, N, d_lv.data_ptr(), d_fl.data_ptr(), d_rs.data_ptr(),
+        pcm, _ = d.decode(*received([pk[p + 5]] * N, lost[:, p], CAP))
+        lv, fl = d.activity()
+        sb.mix_device(d.pcm.data_ptr(), d_out.data_ptr(), 1280, N, d.level.data_ptr(), d.vad.data_ptr(), d_rs.data_ptr(),
                       d_mb.data_ptr(), len(rooms), k, d_tk.data_ptr(), st)
         torch.cuda.synchronize()
-        pcm, lv, fl = d_pcm.cpu().numpy(), d_lv.cpu().numpy(), d_fl.cpu().numpy()
         want, wt = numpy_mix(pcm, lv, fl, rooms, k, np.full((N, 1280), POISON, np.int16))
         assert np.array_equal(d_tk.cpu().numpy(), wt) and np.array_equal(d_out.cpu().numpy(), want), p
         seen += int((wt >= 0).sum())
     assert seen > 0
-    d.close()
+    d.db.close()
 
 
 def test_mcu_tick_device_equals_host(sb):
@@ -229,11 +218,7 @@ def test_mcu_tick_device_equals_host(sb):
     talked = 0
     for p in range(T):
         bits, nb = up.encode(x[p], cap=CAP)
-        rx = [receive(bytes(bits[s, :max(int(nb[s, 0]), 0)]), tuple(int(v) for v in nb[s]), int(lost[s, p])) for s in range(N)]
-        tb = np.zeros((N, CAP), np.uint8)
-        for s, (b, _, _) in enumerate(rx):
-            tb[s, :len(b)] = np.frombuffer(b, np.uint8)
-        tnb, tf = np.array([r[1] for r in rx], np.int16), np.array([r[2] for r in rx], np.int32)
+        tb, tnb, tf = received(batch_packets(bits, nb), lost[:, p], CAP)
         # path 1
         t_b, t_nb, t_f = to_dev(tb), to_dev(tnb), to_dev(tf)
         d1.decode_device(d_pcm.data_ptr(), t_b.data_ptr(), CAP, t_nb.data_ptr(), t_f.data_ptr(), 0, st)

@@ -1,4 +1,5 @@
-"""Shared helpers of the test-suite (input synthesis, the reference driver's loss process, what the receiver decodes)."""
+"""Shared helpers of the test-suite (input synthesis at 16 and 32 kHz, the reference driver's loss process, what the receiver
+decodes)."""
 import os
 import re
 import struct
@@ -174,6 +175,33 @@ def near_silent_classes(clip, n_rows, n_packets, samples=640, seed=9):
             v = sp * env
         out[s] = np.clip(np.round(v), -32768, 32767).astype(np.int16)
     return np.ascontiguousarray(out.reshape(n_rows, n_packets, samples).transpose(1, 0, 2))
+
+
+def upsample2(clip):
+    """The clip at 32 kHz by an integer-exact rule: every 16 kHz sample x[n] is followed by the rounded-down mean of x[n]
+    and x[n + 1] (the last one by itself).  No content above 8 kHz beyond the rule's images."""
+    x = clip.astype(np.int32)
+    nxt = np.concatenate([x[1:], x[-1:]])
+    y = np.empty(2 * len(x), np.int32)
+    y[0::2] = x
+    y[1::2] = (x + nxt) >> 1
+    return y.astype(np.int16)
+
+
+def with_high_band(clip, seed=32):
+    """upsample2(clip) plus seeded white noise of standard deviation 400 (content across 0-16 kHz, so that the 8-16 kHz
+    band carries a signal), clipped to int16."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    y = upsample2(clip).astype(np.float64) + rng.normal(0.0, 400.0, 2 * len(clip))
+    return np.clip(np.round(y), -32768, 32767).astype(np.int16)
+
+
+def chirp(n_samples, amp=8000):
+    """A linear chirp from 100 Hz to 15 kHz over n_samples at 32 kHz."""
+    t = np.arange(n_samples) / 32000.0
+    T = n_samples / 32000.0
+    ph = 2 * np.pi * (100.0 * t + (15000.0 - 100.0) * t * t / (2 * T))
+    return np.round(amp * np.sin(ph)).astype(np.int16)
 
 
 def loss_with_bursts(T, n_rows, seed=3):
