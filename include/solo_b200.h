@@ -114,6 +114,10 @@ solo_b200_dec_batch *solo_b200_dec_batch_create_out(int n_streams, const USER_Ct
                                                     int out_samplerate);
 int solo_b200_dec_batch_decode_host(solo_b200_dec_batch *b, int16_t *pcm, const uint8_t *bits, int cap,
                                     const int16_t *nbytes, const int32_t *lostflag, int32_t *ret);
+/* d_pcm's alignment: a full-band batch (16 kHz, or 32 kHz at its own rate) writes its rows with 8-byte stores, so d_pcm
+   must be 8-byte aligned; a core-output batch accepts any 2-byte alignment (16-byte aligned rows are stored 16 bytes at a
+   time, others sample by sample).  Otherwise -1 with solo_b200_last_error() naming the alignment, before anything is
+   enqueued. */
 int solo_b200_dec_batch_decode_device(solo_b200_dec_batch *b, int16_t *d_pcm, const uint8_t *d_bits, int cap,
                                       const int16_t *d_nbytes, const int32_t *d_lostflag, int32_t *d_ret, void *cuda_stream);
 void solo_b200_dec_batch_destroy(solo_b200_dec_batch *b);

@@ -1486,6 +1486,12 @@ static int dec_launch(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u
 int solo_b200_dec_batch_decode_device(solo_b200_dec_batch* b, int16_t* d_pcm, const uint8_t* d_bits, int cap, const int16_t* d_nbytes,
                                       const int32_t* d_lostflag, int32_t* d_ret, void* cuda_stream) {
     if (!b || !d_pcm || !d_bits || !d_nbytes || !d_lostflag || cap < 16) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    // full-band rows are written by the synthesis kernel's 8-byte stores; core-output rows take any 2-byte alignment
+    const uintptr_t align = b->core_only ? 2 : 8;
+    if ((uintptr_t)d_pcm % align) {
+        snprintf(g_err, sizeof g_err, "decode_device: d_pcm must be %d-byte aligned (%s rows)", (int)align, b->core_only ? "core-output" : "full-band");
+        return -1;
+    }
     CK(cudaSetDevice(b->device));
     b->wave = WAVE_DEVICE;
     return dec_launch(b, 0, b->n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, (cudaStream_t)cuda_stream);

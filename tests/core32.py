@@ -1,11 +1,11 @@
-"""What the core-output tests of 32 kHz streams share (tests/test_dec32_core.py on the CPU, tests/test_gpu_dec32_core.py on
-the GPU): the decoder configurations, the skip check for the reference with its low band tapped, and the loss and damage
-processes."""
+"""What the 32 kHz decoder tests share (tests/test_dec32*.py on the CPU, tests/test_gpu_dec32*.py on the GPU): the decoder
+configurations, the skip check for the reference with its low band tapped, the signal classes and lockstep matrix beyond
+the fixture, and the loss and damage processes."""
 import numpy as np
 import pytest
 
 from tests.golden import make_golden_32k as mk
-from tests.util import load_clip, receive, with_high_band
+from tests.util import chirp, load_clip, loss_flags, loss_with_bursts, receive, upsample2, with_high_band
 
 # (configuration, arithmetics): every configuration of the 32 kHz decoder in each arithmetic that has it
 CONFIGS = [("40ms", dict(framesize_ms=40), ("flp", "fix")), ("20ms", dict(framesize_ms=20), ("flp",)),
@@ -69,3 +69,49 @@ def malformed_sequence(f, g, stream, n, seed):
             fl = int(rng.integers(-3, 9))
         out.append((b, nb, fl))
     return out
+
+
+def signals32(n_packets, seed=11):
+    """(name, int16 32 kHz signal) classes beyond the fixture: speech with noise, zeros, DC, full-scale square, a chirp over
+    the whole band, loud noise, 2 kHz sine, speech fading to silence (for DTX)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    clip = load_clip()
+    L = 1280 * n_packets
+    t = np.arange(L)
+    sp = with_high_band(clip)[:L]
+    fade = (upsample2(clip)[:L] * np.clip(1.0 - t / (0.6 * L), 0, 1)).astype(np.int16)
+    return [
+        ("speech_hb", sp),
+        ("zeros", np.zeros(L, np.int16)),
+        ("dc", np.full(L, 1000, np.int16)),
+        ("square", np.where((t // 40) % 2 == 0, 32767, -32767).astype(np.int16)),
+        ("chirp", chirp(L)),
+        ("noise20000", np.clip(rng.normal(0, 20000, L), -32768, 32767).astype(np.int16)),
+        ("sine2k", (8000 * np.sin(2 * np.pi * 2000 * t / 32000)).astype(np.int16)),
+        ("fade", fade),
+    ]
+
+
+LOCKSTEP = [
+    # (configuration, rate, use_md_index, dtx, loss process)
+    (dict(framesize_ms=40), 15600, 0, 0, "none"),
+    (dict(framesize_ms=40), 32000, 1, 1, "bursts"),
+    (dict(framesize_ms=40), 64000, 0, 0, "first"),
+    (dict(framesize_ms=20), 24000, 1, 0, "bursts"),
+    (dict(framesize_ms=20), 15600, 0, 1, "first"),
+    (dict(framesize_ms=40, joint_hb=1), 14800, 0, 0, "bursts"),
+    (dict(framesize_ms=40, joint_hb=1), 40000, 1, 1, "first"),
+]
+LOCKSTEP_IDS = ["%s-%d-mdi%d-dtx%d-%s" % ("joint" if c.get("joint_hb") else "%dms" % c["framesize_ms"], r, m, d, l)
+                for c, r, m, d, l in LOCKSTEP]
+
+
+def flags_for(kind, n, s):
+    """The lostflags of n packets under loss process `kind` ("none", "first" or "bursts"), seeded by s."""
+    if kind == "none":
+        return [4] * n
+    if kind == "first":        # loss from the very first packet (a lost burst before anything was decoded), then 30 %
+        fl = loss_flags(n, 30, seed=7 + s)
+        return [1] * 4 + fl[4:]
+    # row 1: loss_with_bursts leaves every fifth row loss-free, row 0 among them
+    return [int(v) for v in loss_with_bursts(n, 2, seed=20 + s)[1]]

@@ -161,16 +161,18 @@ class RefRows:
 
 class DeviceDecoder:
     """A decoder batch through decode_device and activity_device on torch buffers of its own (cuda:0), in order on `stream`
-    (default: the current stream).  Same call shapes as the batch's host calls, decode and activity."""
+    (default: the current stream).  Same call shapes as the batch's host calls, decode and activity.  pcm: a cuda:0 int16
+    tensor [N, samples] to decode into instead of its own (a view at any offset, to place the rows)."""
 
-    def __init__(self, db, cap=256, stream=None):
+    def __init__(self, db, cap=256, stream=None, pcm=None):
         import torch
         self.torch, self.db, self.cap = torch, db, cap
         self.stream = torch.cuda.current_stream() if stream is None else stream
         N, dev = db.n, torch.device("cuda", 0)
         self.tb, self.tnb = torch.zeros((N, cap), dtype=torch.uint8, device=dev), torch.zeros((N, 2), dtype=torch.int16, device=dev)
         self.flags, self.ret = torch.zeros(N, dtype=torch.int32, device=dev), torch.full((N,), -99, dtype=torch.int32, device=dev)
-        self.pcm = torch.zeros((N, db.samples), dtype=torch.int16, device=dev)
+        self.pcm = torch.zeros((N, db.samples), dtype=torch.int16, device=dev) if pcm is None else pcm
+        assert self.pcm.shape == (N, db.samples) and self.pcm.is_contiguous()
         self.level, self.vad = torch.zeros(N, dtype=torch.uint8, device=dev), torch.zeros(N, dtype=torch.uint8, device=dev)
 
     def decode(self, tb=None, tnb=None, tf=None, rows=None, check=True):

@@ -10,10 +10,10 @@ import hashlib
 import numpy as np
 import pytest
 
+from tests.core32 import LOCKSTEP, LOCKSTEP_IDS, flags_for, signals32
 from tests.golden import make_golden_32k as mk
 from tests.parity import ref, sim  # noqa: F401  (fixtures)
-from tests.util import (chirp, fuzz_decoder, load_clip, load_golden, loss_flags, loss_with_bursts, receive, upsample2,
-                        with_high_band)
+from tests.util import fuzz_decoder, load_clip, load_golden, receive, with_high_band
 
 CASES = mk.decode_cases()
 
@@ -74,50 +74,7 @@ def test_low_rate_handset_stream_is_rejected_not_misdecoded(ref, sim):
     e.close(), d.close()
 
 
-def signals32(n_packets, seed=11):
-    """(name, int16 32 kHz signal) classes beyond the fixture: speech with noise, zeros, DC, full-scale square, a chirp over
-    the whole band, loud noise, 2 kHz sine, speech fading to silence (for DTX)."""
-    rng = np.random.Generator(np.random.PCG64(seed))
-    clip = load_clip()
-    L = 1280 * n_packets
-    t = np.arange(L)
-    sp = with_high_band(clip)[:L]
-    fade = (upsample2(clip)[:L] * np.clip(1.0 - t / (0.6 * L), 0, 1)).astype(np.int16)
-    return [
-        ("speech_hb", sp),
-        ("zeros", np.zeros(L, np.int16)),
-        ("dc", np.full(L, 1000, np.int16)),
-        ("square", np.where((t // 40) % 2 == 0, 32767, -32767).astype(np.int16)),
-        ("chirp", chirp(L)),
-        ("noise20000", np.clip(rng.normal(0, 20000, L), -32768, 32767).astype(np.int16)),
-        ("sine2k", (8000 * np.sin(2 * np.pi * 2000 * t / 32000)).astype(np.int16)),
-        ("fade", fade),
-    ]
-
-
-LOCKSTEP = [
-    # (configuration, rate, use_md_index, dtx, loss process)
-    (dict(framesize_ms=40), 15600, 0, 0, "none"),
-    (dict(framesize_ms=40), 32000, 1, 1, "bursts"),
-    (dict(framesize_ms=40), 64000, 0, 0, "first"),
-    (dict(framesize_ms=20), 24000, 1, 0, "bursts"),
-    (dict(framesize_ms=20), 15600, 0, 1, "first"),
-    (dict(framesize_ms=40, joint_hb=1), 14800, 0, 0, "bursts"),
-    (dict(framesize_ms=40, joint_hb=1), 40000, 1, 1, "first"),
-]
-
-
-def flags_for(kind, n, s):
-    if kind == "none":
-        return [4] * n
-    if kind == "first":        # loss from the very first packet (a lost burst before anything was decoded), then 30 %
-        fl = loss_flags(n, 30, seed=7 + s)
-        return [1] * 4 + fl[4:]
-    return [int(v) for v in loss_with_bursts(n, 1, seed=20 + s)[0]]
-
-
-@pytest.mark.parametrize("cfg,rate,mdi,dtx,loss", LOCKSTEP, ids=["%s-%d-mdi%d-dtx%d-%s" % ("joint" if c.get("joint_hb") else "%dms" % c["framesize_ms"], r, m, d, l)
-                                                             for c, r, m, d, l in LOCKSTEP])
+@pytest.mark.parametrize("cfg,rate,mdi,dtx,loss", LOCKSTEP, ids=LOCKSTEP_IDS)
 def test_lockstep_with_reference_decoders(ref, sim, cfg, rate, mdi, dtx, loss):
     """Reference FIX encoder at 32 kHz -> (receiver under the loss process) -> host model and the reference decoders, float
     and (40 ms packets, joint mode 1) fixed point, over eight signal classes: every packet's PCM identical (0 LSB)."""

@@ -7,7 +7,8 @@ oracle.ref.RefDecoder(..., samplerate=32000, out_samplerate=16000) returns what 
 import numpy as np
 import pytest
 
-from tests.core32 import CORE, MODE_IDS, MODES, malformed_sequence, mixed_loss, stream_of, tap  # noqa: F401  (tap: fixture)
+from tests.core32 import (CORE, LOCKSTEP, LOCKSTEP_IDS, MODE_IDS, MODES, flags_for, malformed_sequence, mixed_loss,  # noqa: F401
+                          signals32, stream_of, tap)  # (tap: fixture)
 from tests.golden import make_golden_32k as mk
 from tests.parity import ref, sim  # noqa: F401  (fixtures)
 from tests.util import load_clip, load_golden, receive, upsample2
@@ -90,6 +91,22 @@ def test_core_rows_with_dtx(ref, sim, tap, name, cfg, kind):
     assert sum(nb[0] <= 0 for _, nb in pk) >= 3, "the signal must produce DTX packets"
     core_lockstep(ref, sim, kind, cfg, pk, [4] * n, ("dtx",))
     core_lockstep(ref, sim, kind, cfg, pk, mixed_loss(n, seed=77), ("dtx", "loss"))
+
+
+@pytest.mark.parametrize("cfg,rate,mdi,dtx,loss", LOCKSTEP, ids=LOCKSTEP_IDS)
+def test_core_rows_over_signal_classes(ref, sim, tap, cfg, rate, mdi, dtx, loss):
+    """The full-band lockstep's matrix (tests/test_dec32.py) at core output: the reference FIX encoder at 32 kHz over the
+    eight signal classes at the row's rate, use_md_index and DTX, under its loss process; float rows for every
+    configuration, fixed-point rows for 40 ms packets and joint mode 1."""
+    n = 24 if cfg["framesize_ms"] == 40 else 40
+    kinds = ["flp"] + (["fix"] if cfg["framesize_ms"] == 40 else [])
+    for s, (name, x) in enumerate(signals32(n)):
+        e = ref.RefEncoder("fix", rate=rate, dtx=dtx, use_md_index=mdi, samplerate=32000, **cfg)
+        k = e.samples
+        pk = [e.encode(x[p * k:(p + 1) * k])[:2] for p in range(n)]
+        e.close()
+        for kind in kinds:
+            core_lockstep(ref, sim, kind, dict(cfg, use_md_index=mdi), pk, flags_for(loss, n, s), (name,))
 
 
 @pytest.mark.parametrize("name,cfg,kind", MODES, ids=MODE_IDS)
