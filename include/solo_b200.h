@@ -136,6 +136,44 @@ int solo_b200_dec_batch_import_state(solo_b200_dec_batch *b, int idx, const void
 int solo_b200_dec_batch_export_state_sized(solo_b200_dec_batch *b, int idx, void *blob, int blob_bytes);
 int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch *b, int idx, const void *blob, int blob_bytes);
 
+/* Stream membership on the device, for participants joining, leaving and moving between batches or GPUs without stopping
+   the GPU.  The calls follow the queues' reset (solo_b200_rx_reset / solo_b200_tx_reset):
+     - `streams` is a host array of n stream indices; n = 0 does nothing;
+     - the list is checked first: -1 with nothing done (solo_b200_last_error() set) for a stream outside [0, N), a stream
+       listed twice, and for the bad settings and d_blobs described below;
+     - the work is one kernel (two for a 32 kHz decoder import) ordered on `cuda_stream`, after the packet waves already
+       enqueued there; the call then synchronises that CUDA stream only, never the device, so other tenants' work and the
+       batch's other streams keep running.
+   reset: re-initialises the listed streams exactly as create would.  From the next wave a reset stream produces exactly
+     what a stream of a newly created batch with the same ctrl and settings produces on the same input: encoder payload
+     bytes and nbytes, decoder PCM, return codes and activity flags.  Settings are host arrays of n entries, one per listed
+     stream; an entry of -1, or a NULL array, takes the batch's create value.
+       encoder: rate_bps, dtx, loss_perc with the ranges and checks of set_control_host (-1 and nothing done for an entry
+                out of range).  A reset stream is create followed by set_control with those settings.
+       decoder: arith SOLO_B200_DEC_FLP or SOLO_B200_DEC_FIX (FIX refused with 20 ms packets, as create refuses it).  A
+                core-output batch resets its streams into core output.  Packet size, joint mode and useMDIndex are the
+                batch's.
+   export_states / import_states: copy the listed streams' states to / from d_blobs [n][state_bytes] in device memory --
+     this GPU's HBM, a peer GPU's HBM after solo_b200_enable_peer_access, or mapped pinned host memory.  d_blobs must be
+     8-byte aligned (-1 before anything is enqueued otherwise).  state_bytes is solo_b200_enc_state_bytes() or
+     solo_b200_dec_state_bytes_rate(samplerate).  Bytes [i * state_bytes, (i + 1) * state_bytes) are exactly the blob of
+     export_state(streams[i]), and import_state accepts them; import_states accepts export_state's blobs likewise.
+     A 32 kHz decoder import refuses blobs of the other output mode, as import_state_sized does, all or nothing: a check
+     kernel runs first, and if any blob is of the other mode nothing is imported and the call returns -1 after its
+     synchronise.
+   Like the per-stream hand-over, blobs leave out the payload copies a decoder stream reads only while it continues a
+   corrupted packet (see DecStale in solo_b200/csrc/sb_dec.cuh): a reset stream never reads them; an imported stream reads
+   the destination slot's copy, as after import_state.
+   Streams that left are still coded by every wave; reset them when the slot is reused.
+   Launches: a reset or an export is one kernel; an import two for a 32 kHz decoder batch, one otherwise. */
+int solo_b200_enc_batch_reset(solo_b200_enc_batch *b, const int32_t *streams, int n, const int32_t *rate_bps, const int32_t *dtx,
+                              const int32_t *loss_perc, void *cuda_stream);
+int solo_b200_dec_batch_reset(solo_b200_dec_batch *b, const int32_t *streams, int n, const int32_t *arith, void *cuda_stream);
+int solo_b200_enc_batch_export_states(solo_b200_enc_batch *b, const int32_t *streams, int n, void *d_blobs, void *cuda_stream);
+int solo_b200_enc_batch_import_states(solo_b200_enc_batch *b, const int32_t *streams, int n, const void *d_blobs, void *cuda_stream);
+int solo_b200_dec_batch_export_states(solo_b200_dec_batch *b, const int32_t *streams, int n, void *d_blobs, void *cuda_stream);
+int solo_b200_dec_batch_import_states(solo_b200_dec_batch *b, const int32_t *streams, int n, const void *d_blobs, void *cuda_stream);
+
 /* Packet framing around one payload row [MD1 | MD2 | HB] (reference drivers enc_main.c:212-234, dec_main.c:196-307, README
    "Bitstream sending" / "Bitstream screening and synthesis at receiver").  Host functions, no GPU involved.
      split : the two network packets of a row -- description 1 = MD1, description 2 = MD2 + 8 high-band bytes (pointers into

@@ -67,6 +67,11 @@ def lib():
             getattr(L, f).argtypes = [vp, C.c_int, vp]
         for f in ("solo_b200_dec_batch_export_state_sized", "solo_b200_dec_batch_import_state_sized"):
             getattr(L, f).argtypes = [vp, C.c_int, vp, C.c_int]
+        L.solo_b200_enc_batch_reset.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp]
+        L.solo_b200_dec_batch_reset.argtypes = [vp, vp, C.c_int, vp, vp]
+        for f in ("solo_b200_enc_batch_export_states", "solo_b200_enc_batch_import_states", "solo_b200_dec_batch_export_states",
+                  "solo_b200_dec_batch_import_states"):
+            getattr(L, f).argtypes = [vp, vp, C.c_int, vp, vp]
         pp, ip = C.POINTER(vp), C.POINTER(C.c_int)
         L.solo_b200_split_packet.argtypes = [vp, vp, pp, ip, pp, ip]
         L.solo_b200_merge_packets.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp]
@@ -162,6 +167,31 @@ def _queue_reset(fn, name, h, streams, start, stream):
     streams = np.ascontiguousarray(streams, np.int32).ravel()
     start = np.ascontiguousarray(np.broadcast_to(np.asarray(start, np.int64) & 0xFFFFFFFF, streams.shape), np.uint32)
     r = fn(h, streams.ctypes.data, start.ctypes.data, len(streams), stream)
+    if r:
+        raise SoloError("%s failed (%d): %s" % (name, r, _err()))
+
+
+def _stream_list(streams):
+    s = np.asarray(streams, np.int64).ravel()
+    if (s < 0).any() or (s > np.iinfo(np.int32).max).any():
+        raise SoloError("a stream index is outside the batch")
+    return np.ascontiguousarray(s.astype(np.int32))
+
+
+def _settings(name, v, n, keep):
+    """A reset setting as an int32 [n] host array (None: NULL, a scalar: the same for every listed stream)."""
+    if v is None:
+        return None
+    a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, np.int64), (n,)))
+    if (a < np.iinfo(np.int32).min).any() or (a > np.iinfo(np.int32).max).any():
+        raise SoloError("%s: a setting is out of range" % name)
+    keep.append(a.astype(np.int32))
+    return keep[-1].ctypes.data
+
+
+def _move_states(fn, name, h, streams, d_blobs, stream):
+    s = _stream_list(streams)
+    r = fn(h, s.ctypes.data, len(s), d_blobs, stream)
     if r:
         raise SoloError("%s failed (%d): %s" % (name, r, _err()))
 
@@ -339,6 +369,26 @@ class EncoderBatch:
         if r:
             raise SoloError("set_control_device failed (%d): %s" % (r, _err()))
 
+    def reset(self, streams, rate=None, dtx=None, loss=None, stream=0):
+        """Re-initialise the listed streams as a new batch's, then give them rate / dtx / loss: None or -1 keeps the create
+        value, a scalar applies to every listed stream, an array has one entry per listed stream.  Ordered on `stream`;
+        returns once that stream is done.  Raises SoloError, with nothing done, for a stream outside [0, N), one listed
+        twice or a setting out of range (see solo_b200_enc_batch_reset)."""
+        s, keep = _stream_list(streams), []
+        args = [_settings("enc_reset", v, len(s), keep) for v in (rate, dtx, loss)]
+        r = lib().solo_b200_enc_batch_reset(self.h, s.ctypes.data, len(s), *args, stream)
+        if r:
+            raise SoloError("enc_reset failed (%d): %s" % (r, _err()))
+
+    def export_states(self, streams, d_blobs, stream=0):
+        """The listed streams' states into d_blobs (a device address: uint8 [len(streams), enc_state_bytes], 8-byte
+        aligned; this GPU's, a peer GPU's or mapped host memory), ordered on `stream`."""
+        _move_states(lib().solo_b200_enc_batch_export_states, "enc_export_states", self.h, streams, d_blobs, stream)
+
+    def import_states(self, streams, d_blobs, stream=0):
+        """The listed streams' states from d_blobs (laid out as export_states writes them), ordered on `stream`."""
+        _move_states(lib().solo_b200_enc_batch_import_states, "enc_import_states", self.h, streams, d_blobs, stream)
+
     def close(self):
         if getattr(self, "h", None):
             lib().solo_b200_enc_batch_destroy(self.h)
@@ -410,6 +460,30 @@ class DecoderBatch:
         r = lib().solo_b200_dec_batch_decode_device(self.h, d_pcm, d_bits, cap, d_nbytes, d_flags, d_ret, stream)
         if r:
             raise SoloError("decode_device failed (%d): %s" % (r, _err()))
+
+    def reset(self, streams, arith=None, stream=0):
+        """Re-initialise the listed streams as a new batch's.  arith: None or -1 keeps the create arithmetic, "flp" / "fix"
+        (or 0 / 1) for every listed stream, or an array with one entry per listed stream.  Ordered on `stream`; returns
+        once that stream is done.  Raises SoloError, with nothing done, for a stream outside [0, N), one listed twice or
+        a bad arithmetic (see solo_b200_dec_batch_reset)."""
+        s, keep = _stream_list(streams), []
+        if isinstance(arith, str):
+            if arith not in DEC_ARITH:
+                raise SoloError("arith must be one of %s, not %r" % (sorted(DEC_ARITH), arith))
+            arith = DEC_ARITH[arith]
+        r = lib().solo_b200_dec_batch_reset(self.h, s.ctypes.data, len(s), _settings("dec_reset", arith, len(s), keep), stream)
+        if r:
+            raise SoloError("dec_reset failed (%d): %s" % (r, _err()))
+
+    def export_states(self, streams, d_blobs, stream=0):
+        """The listed streams' states into d_blobs (a device address: uint8 [len(streams), dec_state_bytes(samplerate)],
+        8-byte aligned; this GPU's, a peer GPU's or mapped host memory), ordered on `stream`."""
+        _move_states(lib().solo_b200_dec_batch_export_states, "dec_export_states", self.h, streams, d_blobs, stream)
+
+    def import_states(self, streams, d_blobs, stream=0):
+        """The listed streams' states from d_blobs (laid out as export_states writes them), ordered on `stream`; a 32 kHz
+        batch refuses the whole list if any blob is of the other output mode."""
+        _move_states(lib().solo_b200_dec_batch_import_states, "dec_import_states", self.h, streams, d_blobs, stream)
 
     def activity(self):
         """(level uint8 [N], flags uint8 [N]) of the last decode() wave: the RFC 6464 level of every output row, the VAD

@@ -102,10 +102,10 @@ template <int KHZ> struct DecCtrlT {
 
 // SKP_Silk_init_decoder + AGR_Sate_Decoder_Init, expressed for the core the first good frame selects (the PLC and CNG
 // reset themselves to it on their first call, PLC.c:52-55, CNG.c:89-94).
-template <int KHZ> SB_FN void dec_state_init(DecStateT<KHZ>* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0, i32 arith = DEC_FLP,
-                                              i32 core_only = 0) {
+// dec_state_fields sets what Init sets on a zeroed state; dec_state_init zeroes the state first (the device's reset kernel
+// zeroes it with word stores instead of this byte-wise memset, then calls dec_state_fields).
+template <int KHZ> SB_FN void dec_state_fields(DecStateT<KHZ>* st, i32 useMDIndex, i32 framesize_ms, i32 joint_hb, i32 arith, i32 core_only) {
     SB_DEC_DIMS(KHZ);
-    memset(st, 0, sizeof(DecStateT<KHZ>));
     st->useMDIndex = useMDIndex;
     st->core_only = core_only ? 1 : 0;
     st->arith = arith == DEC_FIX ? DEC_FIX : DEC_FLP;
@@ -122,6 +122,11 @@ template <int KHZ> SB_FN void dec_state_init(DecStateT<KHZ>* st, i32 useMDIndex,
     for (int i = 0; i < LPC_ORDER; i++) { acc += step; st->cng_smth_NLSF_Q15[i] = acc; }
     st->cng_rand_seed = 3176576;
     st->hb_first = 1;
+}
+template <int KHZ> SB_FN void dec_state_init(DecStateT<KHZ>* st, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0, i32 arith = DEC_FLP,
+                                              i32 core_only = 0) {
+    memset(st, 0, sizeof(DecStateT<KHZ>));
+    dec_state_fields(st, useMDIndex, framesize_ms, joint_hb, arith, core_only);
 }
 
 // Length split of AGR_Sate_decode_process (AGR_BWE_decode_frame_FLP.c:171-190): {n0, n1} as passed by the

@@ -51,9 +51,9 @@ SB_FN void enc_set_control(EncSilk* st, i32 rate_bps, i32 dtx, i32 loss_perc) {
 }
 
 // ---- Init: AGR_Sate_Encoder_Init + SKP_Silk_init_encoder_FIX + first SKP_Silk_control_encoder_FIX --------------
-// Returns 0, or -1 for a configuration the reference rejects / this build does not cover.
-SB_FN int enc_state_init(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0) {
-    memset(st, 0, sizeof(EncState));
+// enc_state_fields sets what Init sets on a zeroed state; enc_state_init zeroes the state first (the device's reset kernel
+// zeroes it with word stores instead of this byte-wise memset, then calls enc_state_fields).
+SB_FN void enc_state_fields(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 useMDIndex, i32 framesize_ms, i32 joint_hb) {
     st->frames_per_packet = framesize_ms == 20 ? 1 : 2;
     st->hb_frame = joint_hb ? 320 : HB_FRAME;
     // the Init settings go through the per-packet control; the reference starts with no expected loss (AGR_BWE_SDK_API.c:38)
@@ -71,6 +71,11 @@ SB_FN int enc_state_init(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 u
     st->LastGainIndex = 1;
     st->nsq[0].lagPrev = 100;
     st->hb_first = 1;
+}
+// Returns 0, or -1 for a configuration the reference rejects / this build does not cover.
+SB_FN int enc_state_init(EncState* st, i32 targetRate_bps, i32 dtx_enable, i32 useMDIndex, i32 framesize_ms = 40, i32 joint_hb = 0) {
+    memset(st, 0, sizeof(EncState));
+    enc_state_fields(st, targetRate_bps, dtx_enable, useMDIndex, framesize_ms, joint_hb);
     return 0;
 }
 

@@ -13,7 +13,10 @@
 //   sb_dec_synth_kernel          warp per stream       QMF synthesis filter bank + float -> int16
 // The two decoder kernels exist once per SILK core rate (template argument KHZ): 8 for 16 kHz streams, 16 for 32 kHz
 // streams.  A batch holds one configuration, so it picks its instantiation when it is created.
-// Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams.
+// Between packets, sb_enc_control_kernel (thread per stream) changes the rate / DTX / expected-loss settings of streams;
+// sb_enc_reset_kernel / sb_dec_reset_kernel (thread per listed stream) give listed streams a fresh state, and
+// sb_state_copy_kernel (warp per listed stream, after sb_dec_blob_check_kernel for a 32 kHz decoder import) moves listed
+// streams' states to or from device blobs.
 // After a wave, and only when the caller asks for it, sb_activity_kernel (warp per stream) reports every stream's audio level
 // and voice-activity / concealment flags of that wave (sb_activity.cuh).
 // The conference mixer (solo_b200_mix_*, sb_mix.cuh) is two launches of its own: sb_mix_select_kernel (warp per room) picks
@@ -211,6 +214,64 @@ __global__ void __launch_bounds__(SB_TPB) sb_dec_init_kernel(DecStateT<KHZ>* sta
                                                              int core_only) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) dec_state_init(&states[s], mdi, framesize_ms, joint_hb, arith, core_only);
+}
+
+// ---- stream membership: reset, export and import of a list of streams (solo_b200_{enc,dec}_batch_reset / *_states) -----
+// Reset, one thread per listed stream: the stream as create made it (the batch's create settings), then its own settings
+// through the per-packet control -- create followed by set_control is create with those settings.  An entry of -1, or a
+// NULL array, keeps the create value.  The state is zeroed with word stores (16 bytes for EncState, 4 for the decoder's
+// 4-byte aligned states) where the init bodies' memset stores byte by byte, then the init bodies set their fields.
+template <class W, class S> __device__ __forceinline__ void zero_state(S* st) {
+    static_assert(sizeof(S) % sizeof(W) == 0 && alignof(S) >= alignof(W), "zero_state word");
+    W* w = reinterpret_cast<W*>(st);
+#pragma unroll 8
+    for (int k = 0; k < (int)(sizeof(S) / sizeof(W)); k++) w[k] = W{};
+}
+__global__ void __launch_bounds__(SB_TPB) sb_enc_reset_kernel(EncState* states, const i32* __restrict__ streams, int n, const i32* __restrict__ rate,
+                                                              const i32* __restrict__ dtx, const i32* __restrict__ loss, int rate0, int dtx0,
+                                                              int mdi, int framesize_ms, int joint_hb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    EncState* st = &states[streams[i]];
+    zero_state<uint4>(st);
+    enc_state_fields(st, rate0, dtx0, mdi, framesize_ms, joint_hb);
+    enc_set_control(st, rate ? rate[i] : -1, dtx ? dtx[i] : -1, loss ? loss[i] : -1);
+}
+template <int KHZ>
+__global__ void __launch_bounds__(SB_TPB) sb_dec_reset_kernel(DecStateT<KHZ>* states, const i32* __restrict__ streams, int n, const i32* __restrict__ arith,
+                                                              int arith0, int mdi, int framesize_ms, int joint_hb, int core_only) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    DecStateT<KHZ>* st = &states[streams[i]];
+    zero_state<u32>(st);
+    dec_state_fields(st, mdi, framesize_ms, joint_hb, arith && arith[i] != -1 ? arith[i] : arith0, core_only);
+}
+// 32 kHz import: a blob of the other output mode than the batch's sets *bad, and then the copy kernel copies nothing
+__global__ void __launch_bounds__(SB_TPB) sb_dec_blob_check_kernel(const DecState32* blobs, int n, int core_only, int* bad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && blobs[i].core_only != core_only) *bad = 1;
+}
+// One warp per listed stream moves its state between the batch's array and row i of `blobs` (to_blobs: export) in words of
+// W: 8 bytes (256 contiguous bytes per warp instruction) for the encoder's and the 32 kHz decoder's states, 4 bytes for the
+// 16 kHz decoder's, whose 4 252-byte stride keeps only 4-byte alignment; four loads in flight per lane.  Blobs in another
+// GPU's memory are read and written with ordinary loads and stores over NVLink, as the ingest path's kernels do with peer
+// rows.  skip != NULL and *skip != 0: the import check found a blob of the other mode, nothing is copied.
+#define SB_COPY_WARPS 8
+template <class W>
+__global__ void __launch_bounds__(SB_COPY_WARPS * 32) sb_state_copy_kernel(W* states, int words, const i32* __restrict__ streams, int n,
+                                                                           W* blobs, int to_blobs, const int* __restrict__ skip) {
+    const int i = blockIdx.x * SB_COPY_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= n || (skip && *skip)) return;
+    W* s = states + (size_t)streams[i] * words;
+    W* b = blobs + (size_t)i * words;
+    W* dst = to_blobs ? b : s;
+    const W* src = to_blobs ? s : b;
+    int k = lane;
+    for (; k + 96 < words; k += 128) {
+        const W w0 = src[k], w1 = src[k + 32], w2 = src[k + 64], w3 = src[k + 96];
+        dst[k] = w0; dst[k + 32] = w1; dst[k + 64] = w2; dst[k + 96] = w3;
+    }
+    for (; k < words; k += 32) dst[k] = src[k];
 }
 
 // CORE = false: band signals of `spp`-sample packets into band_low / band_high, rows of spp / 2 samples, for the synthesis
@@ -985,20 +1046,47 @@ static int launched(const char* kernel) {
     return e == cudaSuccess ? 0 : fail(kernel, e);
 }
 
-// The device staging of one call of the mixer and queue *_host entry points, on the call's stream.  span() lays out the
+// The stream list of a reset, export or import (the queues' and the codec batches'): true when its n entries are distinct
+// streams of [0, N); otherwise false with g_err naming the first bad entry.
+static bool streams_ok(const i32* streams, int n, int N, const char* who) {
+    std::vector<u8> seen((size_t)N, 0);
+    for (int i = 0; i < n; i++) {
+        if (streams[i] < 0 || streams[i] >= N) { snprintf(g_err, sizeof g_err, "%s: stream %d outside [0, %d)", who, streams[i], N); return false; }
+        if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "%s: stream %d is listed twice", who, streams[i]); return false; }
+    }
+    return true;
+}
+
+// The device staging of one call of the mixer, queue and stream-membership entry points, on the call's stream.  span() lays out the
 // call's arrays: each gets a 16-byte-aligned place in one allocation, is copied in from `in` and back to `out` where those
 // are not NULL, and its device address is written to `dev` when run() has allocated.  Copies back happen only when every
 // earlier step succeeded, the launch's execution included.  finish() always frees, synchronises and returns the first error.
+// With `kept`, the allocation is that buffer instead, grown when too small and never freed here: an object whose calls
+// each end with a synchronise of their stream keeps one, so that its calls do not pay for an allocation from a memory
+// pool that returns its memory at every synchronise.
+struct DevBuf { u8* d = nullptr; size_t bytes = 0; };
 struct Staging {
     struct Span { void** dev; const void* in; void* out; size_t bytes, off; };
     cudaStream_t st;
     const char* who;            // names the entry point in errors
+    DevBuf* keep;
     std::vector<Span> spans;
     size_t size = 0;
     u8* d = nullptr;
     int r = 0;
 
-    Staging(cudaStream_t stream, const char* name) : st(stream), who(name) {}
+    Staging(cudaStream_t stream, const char* name, DevBuf* kept = nullptr) : st(stream), who(name), keep(kept) {}
+    bool alloc() {
+        if (!keep) return ok(cudaMallocAsync(&d, size, st), who);
+        if (keep->bytes < size) {
+            if (keep->d) cudaFreeAsync(keep->d, st);
+            *keep = DevBuf();
+            if (!ok(cudaMallocAsync(&keep->d, size, st), who)) return false;
+            keep->bytes = size;
+        }
+        d = keep->d;
+        return true;
+    }
     bool ok(cudaError_t e, const char* what) { if (!r && e != cudaSuccess) r = fail(what, e); return !r; }
     template <class T> void span(T*& dev, const void* in, void* out, size_t bytes) {
         spans.push_back({(void**)&dev, in, out, bytes, size});
@@ -1008,7 +1096,7 @@ struct Staging {
     bool back(void* host, const void* dev, size_t bytes) { return !bytes || ok(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st), who); }
     // allocate, copy in, launch() (0 or the error it reported), then wait and copy back; false after any failure
     template <class F> bool run(F launch) {
-        if (!ok(cudaMallocAsync(&d, size, st), who)) return false;
+        if (!alloc()) return false;
         for (Span& p : spans) *p.dev = d + p.off;
         for (Span& p : spans)
             if (p.in && p.bytes && !ok(cudaMemcpyAsync(d + p.off, p.in, p.bytes, cudaMemcpyHostToDevice, st), who)) return false;
@@ -1020,7 +1108,7 @@ struct Staging {
         return true;
     }
     int finish() {
-        if (d) cudaFreeAsync(d, st);
+        if (d && !keep) cudaFreeAsync(d, st);
         sync();
         return r;
     }
@@ -1068,9 +1156,10 @@ struct Batch {
     // staging for the *_host entry points and the arena
     i16* d_pcm; u8* d_bits; i16* d_nbytes; int bits_cap;
     u8* d_act;                  // [2][n]: level | flags of the activity entry points (allocated on first use)
+    DevBuf d_list;              // the stream lists and settings of reset / export_states / import_states (grown on use)
     ~Batch() {
         for (int i = 0; i < nst; i++) cudaStreamDestroy(st[i]);
-        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes); cudaFree(d_act);
+        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes); cudaFree(d_act); cudaFree(d_list.d);
     }
 };
 struct solo_b200_enc_batch : Batch {
@@ -1078,11 +1167,14 @@ struct solo_b200_enc_batch : Batch {
     EncScratch* d_scratch;
     i16* d_bands;               // [n][spp]: low band | high band of the packet, written by the QMF kernel
     i32* d_ctrl;                // [3][n]: rate | DTX | loss staging of the set_control host entry points (allocated on first use)
+    USER_Ctrl_enc ctrl;         // the create settings (targetRate_bps after the <= 0 -> 15600 rule), what a reset restores
     ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); cudaFree(d_ctrl); }
 };
 struct solo_b200_dec_batch : Batch {
     int khz;                    // SILK core rate: 8 (16 kHz streams, DecState) or 16 (32 kHz streams, DecState32)
     int core_only;              // 1: 32 kHz streams decoded to their 16 kHz core (spp = the core's rows, no band buffers)
+    USER_Ctrl_dec ctrl;         // the create settings and arithmetic, what a reset restores
+    int arith;
     void* d_states;             // DecStateT<khz>[n]
     DecStale* d_stale;          // payload copies that outlive a packet call (only touched after a corrupted packet, see sb_dec.cuh)
     i32* d_flags; i32* d_ret;   // staging for the *_host entry points and the arena
@@ -1276,6 +1368,8 @@ static solo_b200_enc_batch* enc_batch_create_impl(int n_streams, const USER_Ctrl
         return batch_destroy(b);
     }
     int rate = ctrl->targetRate_bps <= 0 ? 15600 : ctrl->targetRate_bps;
+    b->ctrl = *ctrl;
+    b->ctrl.targetRate_bps = rate;
     sb_enc_init_kernel<<<(n_streams + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states, n_streams, rate, ctrl->dtx_enable, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0);
     count_launch();
     cudaError_t e = cudaStreamSynchronize(b->st[0]);
@@ -1422,6 +1516,8 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
     solo_b200_dec_batch* b = new solo_b200_dec_batch();
     b->khz = ctrl->samplerate == 32000 ? 16 : 8;
     b->core_only = core_only;
+    b->ctrl = *ctrl;
+    b->arith = arith;
     const size_t band = core_only ? 0 : (size_t)ctrl->samplerate / 2000 * ctrl->framesize_ms;   // samples per band and packet
     if (!batch_setup(b, n_streams, device, out_samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
         cudaMalloc(&b->d_states, state_stride(b) * (size_t)n_streams) != cudaSuccess ||
@@ -1534,6 +1630,109 @@ int solo_b200_dec_batch_import_state_sized(solo_b200_dec_batch* b, int idx, cons
         return -1;
     }
     return state_copy(b, idx, (void*)blob, 0, blob_bytes < 0 ? 0 : blob_bytes);
+}
+
+// ---- stream membership on the device: reset, export and import of a list of streams -----------------------------------
+// The list and the settings are checked on the host first; then one or two kernels on the caller's stream, which the call
+// synchronises (the Staging of the host arrays ends with it).  The device is never synchronised: other tenants' work and
+// the waves on other CUDA streams keep running.
+static int list_args_ok(const void* b, const i32* streams, int n, const char* who) {
+    if (b && n >= 0 && (n == 0 || streams)) return 1;
+    snprintf(g_err, sizeof g_err, "%s: bad argument", who);
+    return 0;
+}
+
+int solo_b200_enc_batch_reset(solo_b200_enc_batch* b, const int32_t* streams, int n, const int32_t* rate_bps, const int32_t* dtx,
+                              const int32_t* loss_perc, void* cuda_stream) {
+    if (!list_args_ok(b, streams, n, "enc_reset") || !streams_ok(streams, n, b->n, "enc_reset")) return -1;
+    if (!control_in_range(rate_bps, dtx, loss_perc, n)) { snprintf(g_err, sizeof g_err, "enc_reset: a setting is out of range"); return -1; }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(b->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const i32 *d_streams, *d_rate = nullptr, *d_dtx = nullptr, *d_loss = nullptr;
+    Staging s(st, "enc_reset", &b->d_list);
+    s.span(d_streams, streams, nullptr, 4 * (size_t)n);
+    if (rate_bps) s.span(d_rate, rate_bps, nullptr, 4 * (size_t)n);
+    if (dtx) s.span(d_dtx, dtx, nullptr, 4 * (size_t)n);
+    if (loss_perc) s.span(d_loss, loss_perc, nullptr, 4 * (size_t)n);
+    const USER_Ctrl_enc& c = b->ctrl;
+    s.run([&] {
+        sb_enc_reset_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(b->d_states, d_streams, n, d_rate, d_dtx, d_loss, c.targetRate_bps,
+                                                                        c.dtx_enable ? 1 : 0, c.useMDIndex, c.framesize_ms, c.joint_enable ? 1 : 0);
+        return launched("sb_enc_reset_kernel");
+    });
+    return s.finish();
+}
+
+int solo_b200_dec_batch_reset(solo_b200_dec_batch* b, const int32_t* streams, int n, const int32_t* arith, void* cuda_stream) {
+    if (!list_args_ok(b, streams, n, "dec_reset") || !streams_ok(streams, n, b->n, "dec_reset")) return -1;
+    for (int i = 0; arith && i < n; i++)
+        if (arith[i] != -1 && check_dec_arith(&b->ctrl, arith[i])) return -1;     // g_err names the arithmetic
+    if (n == 0) return 0;
+    CK(cudaSetDevice(b->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const i32 *d_streams, *d_arith = nullptr;
+    Staging s(st, "dec_reset", &b->d_list);
+    s.span(d_streams, streams, nullptr, 4 * (size_t)n);
+    if (arith) s.span(d_arith, arith, nullptr, 4 * (size_t)n);
+    const USER_Ctrl_dec& c = b->ctrl;
+    const int g = (n + SB_TPB - 1) / SB_TPB, joint = c.joint_enable ? 1 : 0;
+    s.run([&] {
+        if (b->khz == 16)
+            sb_dec_reset_kernel<16><<<g, SB_TPB, 0, st>>>((DecState32*)b->d_states, d_streams, n, d_arith, b->arith, c.useMDIndex, c.framesize_ms, joint, b->core_only);
+        else sb_dec_reset_kernel<8><<<g, SB_TPB, 0, st>>>((DecState*)b->d_states, d_streams, n, d_arith, b->arith, c.useMDIndex, c.framesize_ms, joint, 0);
+        return launched("sb_dec_reset_kernel");
+    });
+    return s.finish();
+}
+
+static_assert(sizeof(EncState) % 8 == 0 && sizeof(DecState) % 4 == 0 && sizeof(DecState32) % 8 == 0, "the copy kernel's words");
+// export (to_blobs = 1) or import of the listed streams' states through d_blobs [n][stride]; check_mode >= 0 (a 32 kHz decoder
+// import): blobs whose core_only differs from check_mode refuse the whole import
+static int states_move(Batch* b, void* d_states, size_t stride, const i32* streams, int n, void* d_blobs, int to_blobs, int check_mode,
+                       void* cuda_stream, const char* who) {
+    if (!list_args_ok(b, streams, n, who) || !streams_ok(streams, n, b->n, who)) return -1;
+    if (n == 0) return 0;
+    if (!d_blobs || (uintptr_t)d_blobs % 8) { snprintf(g_err, sizeof g_err, "%s: d_blobs must be a non-NULL, 8-byte aligned device address", who); return -1; }
+    CK(cudaSetDevice(b->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const i32* d_streams;
+    int* d_bad = nullptr;
+    int bad = 0;
+    Staging s(st, who, &b->d_list);
+    s.span(d_streams, streams, nullptr, 4 * (size_t)n);
+    if (check_mode >= 0) s.span(d_bad, &bad, &bad, sizeof bad);
+    s.run([&] {
+        if (d_bad) {
+            sb_dec_blob_check_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>((const DecState32*)d_blobs, n, check_mode, d_bad);
+            if (int e = launched("sb_dec_blob_check_kernel")) return e;
+        }
+        const int g = (n + SB_COPY_WARPS - 1) / SB_COPY_WARPS;
+        if (stride % 8 == 0)
+            sb_state_copy_kernel<u64><<<g, SB_COPY_WARPS * 32, 0, st>>>((u64*)d_states, (int)(stride / 8), d_streams, n, (u64*)d_blobs, to_blobs, d_bad);
+        else sb_state_copy_kernel<u32><<<g, SB_COPY_WARPS * 32, 0, st>>>((u32*)d_states, (int)(stride / 4), d_streams, n, (u32*)d_blobs, to_blobs, d_bad);
+        return launched("sb_state_copy_kernel");
+    });
+    if (int r = s.finish()) return r;
+    if (bad) {
+        snprintf(g_err, sizeof g_err, "%s: a state blob of a %s stream, this batch decodes %s: nothing imported", who,
+                 check_mode ? "full-band 32 kHz" : "core-output (16 kHz)", check_mode ? "to the 16 kHz core" : "the full 32 kHz band");
+        return -1;
+    }
+    return 0;
+}
+int solo_b200_enc_batch_export_states(solo_b200_enc_batch* b, const int32_t* streams, int n, void* d_blobs, void* cuda_stream) {
+    return states_move(b, b ? b->d_states : nullptr, sizeof(EncState), streams, n, d_blobs, 1, -1, cuda_stream, "enc_export_states");
+}
+int solo_b200_enc_batch_import_states(solo_b200_enc_batch* b, const int32_t* streams, int n, const void* d_blobs, void* cuda_stream) {
+    return states_move(b, b ? b->d_states : nullptr, sizeof(EncState), streams, n, (void*)d_blobs, 0, -1, cuda_stream, "enc_import_states");
+}
+int solo_b200_dec_batch_export_states(solo_b200_dec_batch* b, const int32_t* streams, int n, void* d_blobs, void* cuda_stream) {
+    return states_move(b, b ? b->d_states : nullptr, b ? state_stride(b) : 0, streams, n, d_blobs, 1, -1, cuda_stream, "dec_export_states");
+}
+int solo_b200_dec_batch_import_states(solo_b200_dec_batch* b, const int32_t* streams, int n, const void* d_blobs, void* cuda_stream) {
+    const int check = b && b->khz == 16 ? b->core_only : -1;
+    return states_move(b, b ? b->d_states : nullptr, b ? state_stride(b) : 0, streams, n, (void*)d_blobs, 0, check, cuda_stream, "dec_import_states");
 }
 
 int solo_b200_enc_batch_activity_host(solo_b200_enc_batch* b, uint8_t* level, uint8_t* flags) {
@@ -1933,11 +2132,7 @@ static int queue_reset(Q* q, const i32* streams, const u32* start, int n, cudaSt
                        void (*kernel)(D, const i32*, const u32*, int), int block, const char* who,
                        int (*also)(Q*, const i32*, int, cudaStream_t) = nullptr) {
     if (!q || n < 0 || (n > 0 && (!streams || !start))) { snprintf(g_err, sizeof g_err, "%s: bad argument", who); return -1; }
-    std::vector<u8> seen((size_t)q->q.n, 0);
-    for (int i = 0; i < n; i++) {
-        if (streams[i] < 0 || streams[i] >= q->q.n) { snprintf(g_err, sizeof g_err, "%s: stream %d outside [0, %d)", who, streams[i], q->q.n); return -1; }
-        if (seen[streams[i]]++) { snprintf(g_err, sizeof g_err, "%s: stream %d is listed twice", who, streams[i]); return -1; }
-    }
+    if (!streams_ok(streams, n, q->q.n, who)) return -1;
     if (n == 0) return 0;
     CK(cudaSetDevice(q->device));
     const i32* d_streams; const u32* d_start;
