@@ -81,30 +81,24 @@ __global__ void __launch_bounds__(SB_HB_WARPS * 32) sb_enc_hb_warp_kernel(EncSta
 
 }  // namespace
 
-// called from the host code in solo_b200.cu; return a CUDA error code
-extern "C" int sb_launch_enc_analysis_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream) {
-    static bool configured = false;
-    const int smem = (int)SB_ANA_TABS_BYTES + SB_ANA_WARPS * (int)sizeof(AnaSmem);
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(sb_enc_analysis_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        configured = true;
-    }
-    sb_enc_analysis_warp_kernel<<<(n + SB_ANA_WARPS - 1) / SB_ANA_WARPS, SB_ANA_WARPS * 32, smem, (cudaStream_t)stream>>>(
-        (EncState*)states, (EncScratch*)scratch, (const i16*)bands, spp, n);
-    return (int)cudaGetLastError();
+static const int ANA_SMEM = (int)SB_ANA_TABS_BYTES + SB_ANA_WARPS * (int)sizeof(AnaSmem);
+static const int HB_SMEM = SB_HB_WARPS * (int)sizeof(HbSmem);
+
+// Called from the host code in solo_b200.cu.  The shared-memory limit is an attribute of the current device, so every
+// encoder batch sets it on its own device when it is created; returns a CUDA error code.  Not part of the library's ABI.
+extern "C" __attribute__((visibility("hidden"))) int sb_enc_analysis_setup(void) {
+    cudaError_t e = cudaFuncSetAttribute(sb_enc_analysis_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ANA_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sb_enc_hb_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HB_SMEM);
+    return (int)e;
 }
-extern "C" int sb_launch_enc_hb_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream) {
-    static bool configured = false;
-    const int smem = SB_HB_WARPS * (int)sizeof(HbSmem);
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(sb_enc_hb_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        configured = true;
-    }
-    sb_enc_hb_warp_kernel<<<(n + SB_HB_WARPS - 1) / SB_HB_WARPS, SB_HB_WARPS * 32, smem, (cudaStream_t)stream>>>(
+// the launches alone: the caller checks them
+extern "C" void sb_launch_enc_analysis_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream) {
+    sb_enc_analysis_warp_kernel<<<(n + SB_ANA_WARPS - 1) / SB_ANA_WARPS, SB_ANA_WARPS * 32, ANA_SMEM, (cudaStream_t)stream>>>(
         (EncState*)states, (EncScratch*)scratch, (const i16*)bands, spp, n);
-    return (int)cudaGetLastError();
+}
+extern "C" void sb_launch_enc_hb_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream) {
+    sb_enc_hb_warp_kernel<<<(n + SB_HB_WARPS - 1) / SB_HB_WARPS, SB_HB_WARPS * 32, HB_SMEM, (cudaStream_t)stream>>>(
+        (EncState*)states, (EncScratch*)scratch, (const i16*)bands, spp, n);
 }
 #ifdef SB_PHASE_TIMING
 extern "C" int sb_phase_times_read(long long* stamps, int* lines, int cap) {

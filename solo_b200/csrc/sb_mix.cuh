@@ -1,5 +1,5 @@
 // solo_b200 -- per-room mix-minus of the loudest talkers (include/solo_b200.h, solo_b200_mix_*).  Written once for the mix
-// kernels (solo_b200.cu) and the host model (tests/hostsim/mix.cpp).
+// kernels (solo_b200.cu) and the host model (tests/hostsim/server.cpp).
 //   selection : a room's talkers are its up-to-k eligible members ((flags & 3) != 0, RFC 6464's V bit) with the smallest
 //               (level, stream index) -- lower level is louder, ties go to the lower index
 //   mixing    : out[i][t] = clamp(sum over talkers j != i of in[j][t], -32768, 32767), summed in int32 (k <= 8 rows of

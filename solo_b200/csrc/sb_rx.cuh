@@ -1,5 +1,5 @@
 // solo_b200 -- receive queue of descriptions (include/solo_b200.h, solo_b200_rx_*).  The per-arrival and per-slot rules,
-// written once for the queue's kernels (solo_b200.cu) and the host models (tests/hostsim/rx.cpp and rx_timing.cpp), and
+// written once for the queue's kernels (solo_b200.cu) and the host model (tests/hostsim/server.cpp), and
 // the per-row merge rule that solo_b200_merge_packets and the pull kernel share.
 //   current : packet index p is current for a stream whose last played index is `last` when (p - last) mod 2^32 lies in
 //             [1, 2^31); "newer" is a larger distance p - last.  A slot keeps the newest current index among its held one

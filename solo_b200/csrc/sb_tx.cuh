@@ -1,6 +1,6 @@
 // solo_b200 -- send queue of descriptions (include/solo_b200.h, solo_b200_tx_*) and the downlink contributor lists
 // (solo_b200_mix_contributors_*).  The per-row and per-member rules, written once for the kernels (solo_b200.cu) and the
-// host model (tests/hostsim/tx.cpp).
+// host model (tests/hostsim/server.cpp).
 //   row     : an encoded row {bits, nbytes[2]} is DTX (nbytes[0] <= 0), bad (what solo_b200_split_packet refuses, or
 //             nbytes[0] > cap) or sent: description 1 = bits[0, n0 - n1), description 2 = bits[n0 - n1, n0); a description
 //             of 0 bytes is not emitted.  The two descriptions are the row's first n0 bytes in order, so a sent row's

@@ -57,8 +57,9 @@ using namespace sb;
 #define SB_TPB 64
 #define SB_DEC_TPB 64
 // the warp-per-stream analysis kernels live in sb_analysis.cu
-extern "C" int sb_launch_enc_analysis_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
-extern "C" int sb_launch_enc_hb_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
+extern "C" int sb_enc_analysis_setup(void);
+extern "C" void sb_launch_enc_analysis_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
+extern "C" void sb_launch_enc_hb_warp(void* states, void* scratch, const void* bands, int spp, int n, void* stream);
 #define SB_FINISH_MINB 8     // 128 registers: every stream of a chunk resident
 #define SB_DECODE_MINB 8
 
@@ -1035,13 +1036,12 @@ static void prof_end(cudaStream_t st, EvPair* p) {
     std::lock_guard<std::mutex> lk(g_mu);
     g_events.push_back(*p);
 }
-static void count_launch() {
-    std::lock_guard<std::mutex> lk(g_mu);
-    g_launches++;
-}
 // right after one kernel launch: count it and report a launch error under the kernel's name
 static int launched(const char* kernel) {
-    count_launch();
+    {
+        std::lock_guard<std::mutex> lk(g_mu);
+        g_launches++;
+    }
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail(kernel, e);
 }
@@ -1057,9 +1057,9 @@ static bool streams_ok(const i32* streams, int n, int N, const char* who) {
     return true;
 }
 
-// The device staging of one call of the mixer, queue and stream-membership entry points, on the call's stream.  span() lays out the
-// call's arrays: each gets a 16-byte-aligned place in one allocation, is copied in from `in` and back to `out` where those
-// are not NULL, and its device address is written to `dev` when run() has allocated.  Copies back happen only when every
+// The device staging of one call of the mixer, queue, stream-membership, activity and set_control entry points, on the call's
+// stream.  span() lays out the call's arrays: each gets a 16-byte-aligned place in one allocation, is copied in from `in`
+// and back to `out` where those are not NULL, and its device address is written to `dev` when run() has allocated.  Copies back happen only when every
 // earlier step succeeded, the launch's execution included.  finish() always frees, synchronises and returns the first error.
 // With `kept`, the allocation is that buffer instead, grown when too small and never freed here: an object whose calls
 // each end with a synchronise of their stream keeps one, so that its calls do not pay for an allocation from a memory
@@ -1155,20 +1155,18 @@ struct Batch {
     cudaStream_t st[SB_PIPE_STREAMS];
     // staging for the *_host entry points and the arena
     i16* d_pcm; u8* d_bits; i16* d_nbytes; int bits_cap;
-    u8* d_act;                  // [2][n]: level | flags of the activity entry points (allocated on first use)
-    DevBuf d_list;              // the stream lists and settings of reset / export_states / import_states (grown on use)
+    DevBuf d_list;              // the Staging of reset / export / import, activity and set_control host calls (grown on use)
     ~Batch() {
         for (int i = 0; i < nst; i++) cudaStreamDestroy(st[i]);
-        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes); cudaFree(d_act); cudaFree(d_list.d);
+        cudaFree(d_pcm); cudaFree(d_bits); cudaFree(d_nbytes); cudaFree(d_list.d);
     }
 };
 struct solo_b200_enc_batch : Batch {
     EncState* d_states;
     EncScratch* d_scratch;
     i16* d_bands;               // [n][spp]: low band | high band of the packet, written by the QMF kernel
-    i32* d_ctrl;                // [3][n]: rate | DTX | loss staging of the set_control host entry points (allocated on first use)
     USER_Ctrl_enc ctrl;         // the create settings (targetRate_bps after the <= 0 -> 15600 rule), what a reset restores
-    ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); cudaFree(d_ctrl); }
+    ~solo_b200_enc_batch() { cudaFree(d_states); cudaFree(d_scratch); cudaFree(d_bands); }
 };
 struct solo_b200_dec_batch : Batch {
     int khz;                    // SILK core rate: 8 (16 kHz streams, DecState) or 16 (32 kHz streams, DecState32)
@@ -1303,14 +1301,12 @@ static int activity_launch(const solo_b200_dec_batch* b, int lo, int n, const i1
 // stream; returns when the arrays are filled
 template <class B> static int activity_host(B* b, int lo, int n, u8* level, u8* flags) {
     cudaStream_t st = b->st[0];
-    if (!b->d_act) CK(cudaMalloc(&b->d_act, 2 * (size_t)b->n));
-    u8* dl = b->d_act + lo;
-    u8* df = b->d_act + b->n + lo;
-    if (int e = activity_launch(b, lo, n, b->d_pcm, dl, df, st)) return e;
-    CK(cudaMemcpyAsync(level, dl, (size_t)n, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(flags, df, (size_t)n, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
+    u8 *d_level, *d_flags;
+    Staging s(st, "activity_host", &b->d_list);
+    s.span(d_level, nullptr, level, (size_t)n);
+    s.span(d_flags, nullptr, flags, (size_t)n);
+    s.run([&] { return activity_launch(b, lo, n, b->d_pcm, d_level, d_flags, st); });
+    return s.finish();
 }
 // the activity entry point of kind `want` (WAVE_HOST / WAVE_DEVICE) reports on a last wave of the same kind only: the
 // other kind's PCM rows are not where it looks
@@ -1320,6 +1316,19 @@ static int activity_wave_check(const Batch* b, int want) {
                                         : want == WAVE_HOST ? "activity_host: the last packet wave was a *_device call"
                                                             : "activity_device: the last packet wave was a *_host call");
     return -1;
+}
+// solo_b200_{enc,dec}_batch_activity_host / _device
+template <class B> static int batch_activity_host(B* b, u8* level, u8* flags) {
+    if (!b || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_HOST)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_host(b, 0, b->n, level, flags);
+}
+template <class B> static int batch_activity_device(B* b, const i16* d_pcm, u8* d_level, u8* d_flags, void* cuda_stream) {
+    if (!b || !d_pcm || !d_level || !d_flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
+    if (activity_wave_check(b, WAVE_DEVICE)) return -1;
+    CK(cudaSetDevice(b->device));
+    return activity_launch(b, 0, b->n, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
 }
 
 extern "C" {
@@ -1354,24 +1363,30 @@ int solo_b200_profile_read(double* ms_total, long long* launches) {
 }
 
 // ---- encoder batch --------------------------------------------------------------------------------
+// (re)initialise streams [lo, lo + n) of an encoder batch on its first CUDA stream, with ctrl's rate (> 0), DTX and MD index
+static int enc_init_launch(solo_b200_enc_batch* b, int lo, int n, const USER_Ctrl_enc* ctrl) {
+    sb_enc_init_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states + lo, n, ctrl->targetRate_bps, ctrl->dtx_enable, ctrl->useMDIndex,
+                                                                          ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0);
+    return launched("sb_enc_init_kernel");
+}
 static solo_b200_enc_batch* enc_batch_create_impl(int n_streams, const USER_Ctrl_enc* ctrl, int device, int nst) {
     if (n_streams <= 0) { snprintf(g_err, sizeof g_err, "bad encoder configuration"); return nullptr; }
     if (check_enc_ctrl(ctrl)) return nullptr;
     if (require_gpu(device)) return nullptr;
     solo_b200_enc_batch* b = new solo_b200_enc_batch();
+    // the kernels' shared-memory limits are attributes of the device that require_gpu selected
     if (!batch_setup(b, n_streams, device, ctrl->samplerate, ctrl->framesize_ms, ctrl->joint_enable, nst) ||
         cudaMalloc(&b->d_states, sizeof(EncState) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_scratch, sizeof(EncScratch) * (size_t)n_streams) != cudaSuccess ||
         cudaMalloc(&b->d_bands, sizeof(i16) * (size_t)b->spp * (size_t)n_streams) != cudaSuccess ||
-        cudaFuncSetAttribute(sb_enc_nsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SB_NSQ_SPB * sizeof(NsqSmem))) != cudaSuccess) {
+        cudaFuncSetAttribute(sb_enc_nsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SB_NSQ_SPB * sizeof(NsqSmem))) != cudaSuccess ||
+        sb_enc_analysis_setup() != cudaSuccess) {
         fail("enc_batch_create", cudaGetLastError());
         return batch_destroy(b);
     }
-    int rate = ctrl->targetRate_bps <= 0 ? 15600 : ctrl->targetRate_bps;
     b->ctrl = *ctrl;
-    b->ctrl.targetRate_bps = rate;
-    sb_enc_init_kernel<<<(n_streams + SB_TPB - 1) / SB_TPB, SB_TPB, 0, b->st[0]>>>(b->d_states, n_streams, rate, ctrl->dtx_enable, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable ? 1 : 0);
-    count_launch();
+    if (b->ctrl.targetRate_bps <= 0) b->ctrl.targetRate_bps = 15600;
+    if (enc_init_launch(b, 0, n_streams, &b->ctrl)) return batch_destroy(b);
     cudaError_t e = cudaStreamSynchronize(b->st[0]);
     if (e != cudaSuccess) { fail("enc init kernel", e); return batch_destroy(b); }
     return b;
@@ -1396,21 +1411,26 @@ static int enc_launch(solo_b200_enc_batch* b, int lo, int n, const i16* d_pcm, u
     prof_begin(st, 0, &ev);
     i16* bands = b->d_bands + (size_t)lo * b->spp;
     sb_enc_qmf_kernel<<<(n + SB_QMF_SPB - 1) / SB_QMF_SPB, SB_QMF_SPB * 32, 0, st>>>(states, pcm, bands, b->spp, n, pcm_is_local(b->device, pcm));
+    if (int e = launched("sb_enc_qmf_kernel")) return e;
     sb_enc_vad_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(states, scratch, bands, b->spp, n);
-    { int e = sb_launch_enc_hb_warp(states, scratch, bands, b->spp, n, st); if (e) return fail("high-band analysis launch", (cudaError_t)e); }
-    { int e = sb_launch_enc_analysis_warp(states, scratch, bands, b->spp, n, st); if (e) return fail("analysis launch", (cudaError_t)e); }
+    if (int e = launched("sb_enc_vad_kernel")) return e;
+    sb_launch_enc_hb_warp(states, scratch, bands, b->spp, n, st);
+    if (int e = launched("sb_enc_hb_warp_kernel")) return e;
+    sb_launch_enc_analysis_warp(states, scratch, bands, b->spp, n, st);
+    if (int e = launched("sb_enc_analysis_warp_kernel")) return e;
     sb_enc_shape_post_kernel<<<(8 * n + 127) / 128, 128, 0, st>>>(states, scratch, n);
+    if (int e = launched("sb_enc_shape_post_kernel")) return e;
     sb_enc_prefilter_kernel<<<dim3((n + SB_TPB - 1) / SB_TPB, 2), SB_TPB, 0, st>>>(states, scratch, n);
-    for (int i = 0; i < 6; i++) count_launch();
+    if (int e = launched("sb_enc_prefilter_kernel")) return e;
     prof_end(st, &ev);
     prof_begin(st, 1, &ev);
     sb_enc_nsq_kernel<<<(n + SB_NSQ_SPB - 1) / SB_NSQ_SPB, SB_NSQ_WARPS * 32, SB_NSQ_SPB * sizeof(NsqSmem), st>>>(states, scratch, n);
+    if (int e = launched("sb_enc_nsq_kernel")) return e;
     prof_end(st, &ev);
     prof_begin(st, 2, &ev);
     sb_enc_finish_kernel<<<(2 * n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(states, scratch, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, n);
+    if (int e = launched("sb_enc_finish_kernel")) return e;
     prof_end(st, &ev);
-    count_launch(); count_launch();
-    CK(cudaGetLastError());
     return 0;
 }
 
@@ -1421,19 +1441,24 @@ int solo_b200_enc_batch_encode_device(solo_b200_enc_batch* b, const int16_t* d_p
     return enc_launch(b, 0, b->n, d_pcm, d_bits, cap, d_nbytes, (cudaStream_t)cuda_stream);
 }
 
+// streams [lo, lo + m) through the batch's staging on st: PCM rows in, the encoder kernels, payload rows and lengths out.
+// The host arrays start at row lo; the caller waits for st.
+static int enc_host_range(solo_b200_enc_batch* b, int lo, int m, const i16* pcm, u8* bits, int cap, i16* nbytes, cudaStream_t st) {
+    CK(cudaMemcpyAsync(b->d_pcm + (size_t)lo * b->spp, pcm, sizeof(i16) * b->spp * (size_t)m, cudaMemcpyHostToDevice, st));
+    if (int e = enc_launch(b, lo, m, b->d_pcm, b->d_bits, cap, b->d_nbytes, st)) return e;
+    CK(cudaMemcpyAsync(bits, b->d_bits + (size_t)lo * cap, (size_t)cap * m, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(nbytes, b->d_nbytes + 2 * (size_t)lo, sizeof(i16) * 2 * (size_t)m, cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
 int solo_b200_enc_batch_encode_host(solo_b200_enc_batch* b, const int16_t* pcm, uint8_t* bits, int cap, int16_t* nbytes) {
     if (!b || !pcm || !bits || !nbytes || cap < 16) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
     CK(cudaSetDevice(b->device));
     int r = staging(b, cap);
     if (r) return r;
     b->wave = WAVE_HOST;
-    return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {   // per chunk: H2D, encoder kernels, D2H
-        const size_t m = (size_t)(hi - lo);
-        CK(cudaMemcpyAsync(b->d_pcm + (size_t)lo * b->spp, pcm + (size_t)lo * b->spp, sizeof(i16) * b->spp * m, cudaMemcpyHostToDevice, st));
-        if (int e = enc_launch(b, lo, hi - lo, b->d_pcm, b->d_bits, cap, b->d_nbytes, st)) return e;
-        CK(cudaMemcpyAsync(bits + (size_t)lo * cap, b->d_bits + (size_t)lo * cap, (size_t)cap * m, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(nbytes + 2 * (size_t)lo, b->d_nbytes + 2 * (size_t)lo, sizeof(i16) * 2 * m, cudaMemcpyDeviceToHost, st));
-        return 0;
+    return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {
+        return enc_host_range(b, lo, hi - lo, pcm + (size_t)lo * b->spp, bits + (size_t)lo * cap, cap, nbytes + 2 * (size_t)lo, st);
     });
 }
 
@@ -1454,18 +1479,13 @@ static int enc_control_launch(solo_b200_enc_batch* b, int lo, int n, const i32* 
 }
 // host arrays of streams [lo, lo + n) through the batch's staging into the control kernel on st; returns when it is done
 static int enc_control_host(solo_b200_enc_batch* b, int lo, int n, const i32* rate, const i32* dtx, const i32* loss, cudaStream_t st) {
-    if (!b->d_ctrl) CK(cudaMalloc(&b->d_ctrl, sizeof(i32) * 3 * (size_t)b->n));
-    const i32* src[3] = {rate, dtx, loss};
-    const i32* dev[3] = {nullptr, nullptr, nullptr};
-    for (int k = 0; k < 3; k++) {
-        if (!src[k]) continue;
-        i32* d = b->d_ctrl + (size_t)k * b->n + lo;
-        CK(cudaMemcpyAsync(d, src[k], sizeof(i32) * (size_t)n, cudaMemcpyHostToDevice, st));
-        dev[k] = d;
-    }
-    if (int e = enc_control_launch(b, lo, n, dev[0], dev[1], dev[2], st)) return e;
-    CK(cudaStreamSynchronize(st));
-    return 0;
+    const i32 *d_rate = nullptr, *d_dtx = nullptr, *d_loss = nullptr;
+    Staging s(st, "set_control", &b->d_list);
+    if (rate) s.span(d_rate, rate, nullptr, 4 * (size_t)n);
+    if (dtx) s.span(d_dtx, dtx, nullptr, 4 * (size_t)n);
+    if (loss) s.span(d_loss, loss, nullptr, 4 * (size_t)n);
+    s.run([&] { return enc_control_launch(b, lo, n, d_rate, d_dtx, d_loss, st); });
+    return s.finish();
 }
 
 int solo_b200_enc_batch_set_control_device(solo_b200_enc_batch* b, const int32_t* d_rate_bps, const int32_t* d_dtx, const int32_t* d_loss_perc, void* cuda_stream) {
@@ -1497,11 +1517,11 @@ static int check_dec_arith(const USER_Ctrl_dec* c, int arith) {
     return 0;
 }
 // (re)initialise streams [lo, lo + n) of a decoder batch on its first CUDA stream
-static void dec_init_launch(solo_b200_dec_batch* b, int lo, int n, int mdi, int framesize_ms, int joint_enable, int arith) {
+static int dec_init_launch(solo_b200_dec_batch* b, int lo, int n, int mdi, int framesize_ms, int joint_enable, int arith) {
     const int g = (n + SB_TPB - 1) / SB_TPB, joint = joint_enable ? 1 : 0;
     if (b->khz == 16) sb_dec_init_kernel<16><<<g, SB_TPB, 0, b->st[0]>>>((DecState32*)b->d_states + lo, n, mdi, framesize_ms, joint, arith, b->core_only);
     else sb_dec_init_kernel<8><<<g, SB_TPB, 0, b->st[0]>>>((DecState*)b->d_states + lo, n, mdi, framesize_ms, joint, arith, 0);
-    count_launch();
+    return launched("sb_dec_init_kernel");
 }
 // out_samplerate: ctrl->samplerate, or 16000 for 32 kHz streams decoded to their 16 kHz core
 static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl_dec* ctrl, int device, int nst, int arith, int out_samplerate) {
@@ -1529,7 +1549,7 @@ static solo_b200_dec_batch* dec_batch_create_impl(int n_streams, const USER_Ctrl
         fail("dec_batch_create", cudaGetLastError());
         return batch_destroy(b);
     }
-    dec_init_launch(b, 0, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable, arith);
+    if (dec_init_launch(b, 0, n_streams, ctrl->useMDIndex, ctrl->framesize_ms, ctrl->joint_enable, arith)) return batch_destroy(b);
     cudaError_t e = cudaStreamSynchronize(b->st[0]);
     if (e != cudaSuccess) { fail("dec init kernel", e); return batch_destroy(b); }
     return b;
@@ -1544,11 +1564,12 @@ solo_b200_dec_batch* solo_b200_dec_batch_create_out(int n_streams, const USER_Ct
     return dec_batch_create_impl(n_streams, ctrl, device, SB_PIPE_STREAMS, arith, out_samplerate);
 }
 
-// the decoder kernels of core rate KHZ for streams [lo, lo + n) of b: decode and synthesis, or the core-output decode alone
+// the decoder kernels of core rate KHZ for streams [lo, lo + n) of b: decode and synthesis, or the core-output decode alone;
+// the first launch error
 extern "C++" {
 template <int KHZ>
-static void dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
-                        i32* d_ret, cudaStream_t st) {
+static int dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
+                       i32* d_ret, cudaStream_t st) {
     DecStateT<KHZ>* states = (DecStateT<KHZ>*)b->d_states + lo;
     // core output: the PCM rows (b->spp samples) are the low band of 2 * b->spp-sample packets
     if constexpr (KHZ == 16) if (b->core_only) {
@@ -1556,27 +1577,26 @@ static void dec_kernels(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const
                                                                                     d_lostflag + lo, d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo,
                                                                                     b->d_act_flags + lo, b->d_stale + lo, d_pcm + (size_t)lo * b->spp,
                                                                                     nullptr, 2 * b->spp, n);
-        return;
+        return launched("sb_decode_kernel");
     }
     const size_t half = (size_t)(b->spp / 2);
     sb_decode_kernel<KHZ><<<(n + SB_DEC_TPB - 1) / SB_DEC_TPB, SB_DEC_TPB, 0, st>>>(states, d_bits + (size_t)lo * cap, cap, d_nbytes + 2 * (size_t)lo, d_lostflag + lo,
                                                                        d_ret ? d_ret + lo : nullptr, b->d_ret_int + lo, b->d_act_flags + lo, b->d_stale + lo,
                                                                        b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half, b->spp, n);
+    if (int e = launched("sb_decode_kernel")) return e;
     sb_dec_synth_kernel<KHZ><<<(n + SB_SYN_WARPS - 1) / SB_SYN_WARPS, SB_SYN_WARPS * 32, 0, st>>>(states, b->d_band_low + (size_t)lo * half, b->d_band_high + (size_t)lo * half,
                                                                                                b->d_ret_int + lo, d_pcm + (size_t)lo * b->spp, b->spp, n);
+    return launched("sb_dec_synth_kernel");
 }
 }  // extern "C++"
 static int dec_launch(solo_b200_dec_batch* b, int lo, int n, i16* d_pcm, const u8* d_bits, int cap, const i16* d_nbytes, const i32* d_lostflag,
                       i32* d_ret, cudaStream_t st) {
     if (n <= 0) return 0;
     EvPair ev; prof_begin(st, 3, &ev);
-    if (b->khz == 16) dec_kernels<16>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
-    else dec_kernels<8>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
+    const int r = b->khz == 16 ? dec_kernels<16>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st)
+                               : dec_kernels<8>(b, lo, n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, st);
     prof_end(st, &ev);
-    count_launch();
-    if (!b->core_only) count_launch();      // the synthesis kernel
-    CK(cudaGetLastError());
-    return 0;
+    return r;
 }
 
 int solo_b200_dec_batch_decode_device(solo_b200_dec_batch* b, int16_t* d_pcm, const uint8_t* d_bits, int cap, const int16_t* d_nbytes,
@@ -1593,6 +1613,20 @@ int solo_b200_dec_batch_decode_device(solo_b200_dec_batch* b, int16_t* d_pcm, co
     return dec_launch(b, 0, b->n, d_pcm, d_bits, cap, d_nbytes, d_lostflag, d_ret, (cudaStream_t)cuda_stream);
 }
 
+// streams [lo, lo + m) through the batch's staging on st: payload rows, lengths and loss flags in, the decoder kernels, PCM
+// rows and (ret != NULL) return codes out.  The host arrays start at row lo; the caller waits for st.
+static int dec_host_range(solo_b200_dec_batch* b, int lo, int m, i16* pcm, const u8* bits, int cap, const i16* nbytes, const i32* lostflag,
+                          i32* ret, cudaStream_t st) {
+    const size_t r = (size_t)m;
+    CK(cudaMemcpyAsync(b->d_bits + (size_t)lo * cap, bits, (size_t)cap * r, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b->d_nbytes + 2 * (size_t)lo, nbytes, sizeof(i16) * 2 * r, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b->d_flags + lo, lostflag, sizeof(i32) * r, cudaMemcpyHostToDevice, st));
+    if (int e = dec_launch(b, lo, m, b->d_pcm, b->d_bits, cap, b->d_nbytes, b->d_flags, b->d_ret, st)) return e;
+    CK(cudaMemcpyAsync(pcm, b->d_pcm + (size_t)lo * b->spp, sizeof(i16) * b->spp * r, cudaMemcpyDeviceToHost, st));
+    if (ret) CK(cudaMemcpyAsync(ret, b->d_ret + lo, sizeof(i32) * r, cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
 int solo_b200_dec_batch_decode_host(solo_b200_dec_batch* b, int16_t* pcm, const uint8_t* bits, int cap, const int16_t* nbytes,
                                     const int32_t* lostflag, int32_t* ret) {
     if (!b || !pcm || !bits || !nbytes || !lostflag || cap < 16) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
@@ -1600,15 +1634,9 @@ int solo_b200_dec_batch_decode_host(solo_b200_dec_batch* b, int16_t* pcm, const 
     int r = dec_staging(b, cap);
     if (r) return r;
     b->wave = WAVE_HOST;
-    return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {   // per chunk: H2D, decoder kernels, D2H
-        const size_t m = (size_t)(hi - lo);
-        CK(cudaMemcpyAsync(b->d_bits + (size_t)lo * cap, bits + (size_t)lo * cap, (size_t)cap * m, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(b->d_nbytes + 2 * (size_t)lo, nbytes + 2 * (size_t)lo, sizeof(i16) * 2 * m, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(b->d_flags + lo, lostflag + lo, sizeof(i32) * m, cudaMemcpyHostToDevice, st));
-        if (int e = dec_launch(b, lo, hi - lo, b->d_pcm, b->d_bits, cap, b->d_nbytes, b->d_flags, b->d_ret, st)) return e;
-        CK(cudaMemcpyAsync(pcm + (size_t)lo * b->spp, b->d_pcm + (size_t)lo * b->spp, sizeof(i16) * b->spp * m, cudaMemcpyDeviceToHost, st));
-        if (ret) CK(cudaMemcpyAsync(ret + lo, b->d_ret + lo, sizeof(i32) * m, cudaMemcpyDeviceToHost, st));
-        return 0;
+    return host_chunks(b, [&](int lo, int hi, cudaStream_t st) {
+        return dec_host_range(b, lo, hi - lo, pcm + (size_t)lo * b->spp, bits + (size_t)lo * cap, cap, nbytes + 2 * (size_t)lo, lostflag + lo,
+                              ret ? ret + lo : nullptr, st);
     });
 }
 
@@ -1735,29 +1763,13 @@ int solo_b200_dec_batch_import_states(solo_b200_dec_batch* b, const int32_t* str
     return states_move(b, b ? b->d_states : nullptr, b ? state_stride(b) : 0, streams, n, (void*)d_blobs, 0, check, cuda_stream, "dec_import_states");
 }
 
-int solo_b200_enc_batch_activity_host(solo_b200_enc_batch* b, uint8_t* level, uint8_t* flags) {
-    if (!b || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
-    if (activity_wave_check(b, WAVE_HOST)) return -1;
-    CK(cudaSetDevice(b->device));
-    return activity_host(b, 0, b->n, level, flags);
-}
+int solo_b200_enc_batch_activity_host(solo_b200_enc_batch* b, uint8_t* level, uint8_t* flags) { return batch_activity_host(b, level, flags); }
 int solo_b200_enc_batch_activity_device(solo_b200_enc_batch* b, const int16_t* d_pcm, uint8_t* d_level, uint8_t* d_flags, void* cuda_stream) {
-    if (!b || !d_pcm || !d_level || !d_flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
-    if (activity_wave_check(b, WAVE_DEVICE)) return -1;
-    CK(cudaSetDevice(b->device));
-    return activity_launch(b, 0, b->n, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
+    return batch_activity_device(b, d_pcm, d_level, d_flags, cuda_stream);
 }
-int solo_b200_dec_batch_activity_host(solo_b200_dec_batch* b, uint8_t* level, uint8_t* flags) {
-    if (!b || !level || !flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
-    if (activity_wave_check(b, WAVE_HOST)) return -1;
-    CK(cudaSetDevice(b->device));
-    return activity_host(b, 0, b->n, level, flags);
-}
+int solo_b200_dec_batch_activity_host(solo_b200_dec_batch* b, uint8_t* level, uint8_t* flags) { return batch_activity_host(b, level, flags); }
 int solo_b200_dec_batch_activity_device(solo_b200_dec_batch* b, const int16_t* d_pcm, uint8_t* d_level, uint8_t* d_flags, void* cuda_stream) {
-    if (!b || !d_pcm || !d_level || !d_flags) { snprintf(g_err, sizeof g_err, "bad argument"); return -1; }
-    if (activity_wave_check(b, WAVE_DEVICE)) return -1;
-    CK(cudaSetDevice(b->device));
-    return activity_launch(b, 0, b->n, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
+    return batch_activity_device(b, d_pcm, d_level, d_flags, cuda_stream);
 }
 
 // ---- packet framing (host, no GPU involved): enc_main.c:212-234 / dec_main.c:196-307 / README "Bitstream sending" --------
@@ -2400,7 +2412,8 @@ template <class B> static void arena_release(ArenaSeg<B>* sg, int slot) {   // u
     sg->n_used--;
 }
 // A slot on the current device: a free one of a segment with this packet layout, or the first one of a new segment made by
-// create(device).  init(batch, slot) enqueues the (re)initialisation of that one stream with the caller's settings.
+// create(device).  init(batch, slot) enqueues the (re)initialisation of that one stream with the caller's settings and
+// returns its launch error.
 template <class B, class Create, class Init>
 static Handle<B>* arena_open(std::vector<ArenaSeg<B>*>& segs, unsigned magic, int samplerate, int framesize_ms, int joint_enable, const char* who,
                              const char* what, Create create, Init init) {
@@ -2421,8 +2434,7 @@ static Handle<B>* arena_open(std::vector<ArenaSeg<B>*>& segs, unsigned magic, in
     {
         std::lock_guard<std::mutex> lk2(sg->mu);
         cudaSetDevice(dev);
-        init(sg->b, slot);
-        if (cudaStreamSynchronize(sg->b->st[0]) != cudaSuccess) { arena_release(sg, slot); fprintf(stderr, "solo_b200: %s slot init failed\n", what); return nullptr; }
+        if (init(sg->b, slot) || cudaStreamSynchronize(sg->b->st[0]) != cudaSuccess) { arena_release(sg, slot); fprintf(stderr, "solo_b200: %s slot init failed\n", what); return nullptr; }
     }
     return new Handle<B>{magic, sg, slot};
 }
@@ -2459,11 +2471,7 @@ void* AGR_Sate_Encoder_Init(USER_Ctrl_enc* enc_Ctrl) {
     if (check_enc_ctrl(enc_Ctrl)) { fprintf(stderr, "solo_b200: AGR_Sate_Encoder_Init: unsupported configuration: %s\n", g_err); return nullptr; }
     return arena_open(g_enc_segs, ENC_MAGIC, enc_Ctrl->samplerate, enc_Ctrl->framesize_ms, enc_Ctrl->joint_enable, "AGR_Sate_Encoder_Init", "encoder",
                       [&](int dev) { return enc_batch_create_impl(SB_ARENA_SEG, enc_Ctrl, dev, 1); },
-                      [&](solo_b200_enc_batch* b, int slot) {   // the caller's rate / DTX / MD-index settings
-                          sb_enc_init_kernel<<<1, SB_TPB, 0, b->st[0]>>>(b->d_states + slot, 1, enc_Ctrl->targetRate_bps, enc_Ctrl->dtx_enable, enc_Ctrl->useMDIndex,
-                                                                        enc_Ctrl->framesize_ms, enc_Ctrl->joint_enable ? 1 : 0);
-                          count_launch();
-                      });
+                      [&](solo_b200_enc_batch* b, int slot) { return enc_init_launch(b, slot, 1, enc_Ctrl); });   // the caller's settings
 }
 SKP_int32 AGR_Sate_Encoder_Encode(void* SATEEnc_State, const SKP_int16* AGR_Sate_PCM, SKP_uint8* AGR_Sate_Bit, SKP_int32 AGR_Sate_Buf_Size,
                                   SKP_int16* nBytesOut) {
@@ -2475,15 +2483,11 @@ SKP_int32 AGR_Sate_Encoder_Encode(void* SATEEnc_State, const SKP_int16* AGR_Sate
     int16_t nb[2] = {0, 0};
     {
         std::lock_guard<std::mutex> lk(h->seg->mu);
-        if (cudaSetDevice(b->device) != cudaSuccess || staging(b, cap)) { fprintf(stderr, "solo_b200: encode failed: %s\n", g_err); return -1; }
-        const size_t s = (size_t)h->slot;
-        cudaStream_t st = b->st[0];
-        bool ok = cudaMemcpyAsync(b->d_pcm + s * b->spp, AGR_Sate_PCM, sizeof(i16) * b->spp, cudaMemcpyHostToDevice, st) == cudaSuccess;
-        ok = ok && enc_launch(b, h->slot, 1, b->d_pcm, b->d_bits, cap, b->d_nbytes, st) == 0;
-        ok = ok && cudaMemcpyAsync(tmp, b->d_bits + s * cap, cap, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-        ok = ok && cudaMemcpyAsync(nb, b->d_nbytes + 2 * s, sizeof nb, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-        if (!ok) { fprintf(stderr, "solo_b200: encode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError())); return -1; }
+        if (cudaSetDevice(b->device) != cudaSuccess || staging(b, cap) || enc_host_range(b, h->slot, 1, AGR_Sate_PCM, tmp, cap, nb, b->st[0]) ||
+            cudaStreamSynchronize(b->st[0]) != cudaSuccess) {
+            fprintf(stderr, "solo_b200: encode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError()));
+            return -1;
+        }
         h->coded = 1;
     }
     // DTX packets return the high-band bytes (4 per 20 ms frame) with nBytesOut[0] == 0 (App. A Q16)
@@ -2531,7 +2535,7 @@ void* AGR_Sate_Decoder_Init(USER_Ctrl_dec* dec_Ctrl) {
     return arena_open(g_dec_segs, DEC_MAGIC, dec_Ctrl->samplerate, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, "AGR_Sate_Decoder_Init", "decoder",
                       [&](int dev) { return dec_batch_create_impl(SB_ARENA_SEG, dec_Ctrl, dev, 1, SOLO_B200_DEC_FLP, dec_Ctrl->samplerate); },
                       [&](solo_b200_dec_batch* b, int slot) {
-                          dec_init_launch(b, slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, arith);
+                          return dec_init_launch(b, slot, 1, dec_Ctrl->useMDIndex, dec_Ctrl->framesize_ms, dec_Ctrl->joint_enable, arith);
                       });
 }
 SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, SKP_int16* nSamplesOut, const SKP_uint8* AGR_Sate_Bit,
@@ -2549,17 +2553,11 @@ SKP_int32 AGR_Sate_Decoder_Decode(void* SATEDec_State, SKP_int16* AGR_Sate_PCM, 
     int32_t flag = lostflag, ret = 0;
     {
         std::lock_guard<std::mutex> lk(h->seg->mu);
-        if (cudaSetDevice(b->device) != cudaSuccess || dec_staging(b, cap)) { fprintf(stderr, "solo_b200: decode failed: %s\n", g_err); return -1; }
-        const size_t s = (size_t)h->slot;
-        cudaStream_t st = b->st[0];
-        bool ok = cudaMemcpyAsync(b->d_bits + s * cap, tmp, cap, cudaMemcpyHostToDevice, st) == cudaSuccess;
-        ok = ok && cudaMemcpyAsync(b->d_nbytes + 2 * s, nb, sizeof nb, cudaMemcpyHostToDevice, st) == cudaSuccess;
-        ok = ok && cudaMemcpyAsync(b->d_flags + s, &flag, sizeof flag, cudaMemcpyHostToDevice, st) == cudaSuccess;
-        ok = ok && dec_launch(b, h->slot, 1, b->d_pcm, b->d_bits, cap, b->d_nbytes, b->d_flags, b->d_ret, st) == 0;
-        ok = ok && cudaMemcpyAsync(AGR_Sate_PCM, b->d_pcm + s * b->spp, sizeof(i16) * b->spp, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-        ok = ok && cudaMemcpyAsync(&ret, b->d_ret + s, sizeof ret, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-        if (!ok) { fprintf(stderr, "solo_b200: decode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError())); return -1; }
+        if (cudaSetDevice(b->device) != cudaSuccess || dec_staging(b, cap) ||
+            dec_host_range(b, h->slot, 1, AGR_Sate_PCM, tmp, cap, nb, &flag, &ret, b->st[0]) || cudaStreamSynchronize(b->st[0]) != cudaSuccess) {
+            fprintf(stderr, "solo_b200: decode failed: %s\n", g_err[0] ? g_err : cudaGetErrorString(cudaGetLastError()));
+            return -1;
+        }
         h->coded = 1;
     }
     // the reference rewrites the caller's nBytes[] while splitting the payload (AGR_BWE_decode_frame_FLP.c:171-190)
