@@ -1228,25 +1228,11 @@ struct HbScr {
     i16 coef[HB_ORDER];
     union { BurgScr burg; A2nlsfScr a2n; } u;
 };
-// One high-band frame of F samples: buffer update, order-8 LPC (Burg over four 88-sample blocks), two-stage LSP VQ,
-// residual energy per sub-frame.  hb, H: shared memory; high: the new samples; outputs: global memory.
-template <int F> SB_CFN void c_hb_analyse_frame(EncBands* hb, HbScr* H, const i16* high, i32* lsp_idx_out, i32* nrg0_out) {
-    enum { LPCF = 80, BL = LPCF + HB_ORDER, SF = F >> 2 };
+// AGR_Sate_lsp_quant_highband (AGR_BWE_quant_highband.c:23-104) on H->NLSF_Q15: Laroia weights into H->weight, 256-entry
+// first stage over the lanes, 16-entry weighted second stage; the quantised vector replaces H->NLSF_Q15, lane 0 stores the
+// index.  The caller synchronises the warp before it reads the results.
+SB_CFN void c_hb_lsp_quant(HbScr* H, i32* lsp_idx_out) {
     const int lane = SB_LANE;
-    SB_PARFOR(i, 0, F) hb->x_hb_buf[F + 40 + i] = high[i];
-    SB_SYNC();
-    SB_PARFOR(t, 0, 4 * BL) { const int k = t / BL, i = t - k * BL; H->LPC_in_pre[t] = hb->x_hb_buf[F - HB_ORDER + k * LPCF + i]; }
-    SB_SYNC();
-    i32 rn, rq;
-    c_burg2<HB_ORDER>(&rn, &rq, H->A_Q16, &H->u.burg, H->LPC_in_pre, 4, H->LPC_in_pre, 4, BL, SB_FIXC(2.5e-5f, 32));
-    SB_SYNC();
-    {
-        const i32 f = c_bwexpander32_factor(HB_ORDER, SB_FIXC(0.99995f, 16));
-        if (lane < HB_ORDER) H->A_Q16[0][lane] = smulww(H->A_Q16[0][lane], f);
-    }
-    SB_SYNC();
-    c_a2nlsf<HB_ORDER>(H->NLSF_Q15, H->A_Q16[0], &H->u.a2n);
-    // ---- AGR_Sate_lsp_quant_highband: 256-entry first stage over the lanes, 16-entry weighted second stage ----
     if (lane == 0) { i32 w[HB_ORDER], nl[HB_ORDER]; for (int i = 0; i < HB_ORDER; i++) nl[i] = H->NLSF_Q15[i]; nlsf_vq_weights_laroia(w, nl, HB_ORDER); for (int i = 0; i < HB_ORDER; i++) H->weight[i] = w[i]; }
     SB_SYNC();
     i32 lsp[HB_ORDER];
@@ -1269,6 +1255,26 @@ template <int F> SB_CFN void c_hb_analyse_frame(EncBands* hb, HbScr* H, const i1
     SB_SYNC();
     if (lane < HB_ORDER) H->NLSF_Q15[lane] = (i32)cb1[idx1 * HB_ORDER + lane] + (i32)cb2[idx2 * HB_ORDER + lane];
     if (lane == 0) *lsp_idx_out = shl(idx2, 8) + idx1;
+}
+// One high-band frame of F samples: buffer update, order-8 LPC (Burg over four 88-sample blocks), two-stage LSP VQ,
+// residual energy per sub-frame.  hb, H: shared memory; high: the new samples; outputs: global memory.
+template <int F> SB_CFN void c_hb_analyse_frame(EncBands* hb, HbScr* H, const i16* high, i32* lsp_idx_out, i32* nrg0_out) {
+    enum { LPCF = 80, BL = LPCF + HB_ORDER, SF = F >> 2 };
+    const int lane = SB_LANE;
+    SB_PARFOR(i, 0, F) hb->x_hb_buf[F + 40 + i] = high[i];
+    SB_SYNC();
+    SB_PARFOR(t, 0, 4 * BL) { const int k = t / BL, i = t - k * BL; H->LPC_in_pre[t] = hb->x_hb_buf[F - HB_ORDER + k * LPCF + i]; }
+    SB_SYNC();
+    i32 rn, rq;
+    c_burg2<HB_ORDER>(&rn, &rq, H->A_Q16, &H->u.burg, H->LPC_in_pre, 4, H->LPC_in_pre, 4, BL, SB_FIXC(2.5e-5f, 32));
+    SB_SYNC();
+    {
+        const i32 f = c_bwexpander32_factor(HB_ORDER, SB_FIXC(0.99995f, 16));
+        if (lane < HB_ORDER) H->A_Q16[0][lane] = smulww(H->A_Q16[0][lane], f);
+    }
+    SB_SYNC();
+    c_a2nlsf<HB_ORDER>(H->NLSF_Q15, H->A_Q16[0], &H->u.a2n);
+    c_hb_lsp_quant(H, lsp_idx_out);
     SB_SYNC();
     if (lane == 0) { i32 nl[HB_ORDER]; i16 a12[HB_ORDER]; for (int i = 0; i < HB_ORDER; i++) nl[i] = H->NLSF_Q15[i]; nlsf2a_stable(a12, nl, HB_ORDER); for (int i = 0; i < HB_ORDER; i++) H->coef[i] = a12[i]; }
     SB_SYNC();

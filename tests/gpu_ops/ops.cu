@@ -3,7 +3,8 @@
 // case from global memory, stages the routine's scratch struct and arrays in shared memory as the analysis kernel does,
 // calls the routine and writes every output back.  tests/test_gpu_ops.py compares the results with the reference.
 // The quantiser kernel's device code runs here too, whole packets in the production kernel's layout (sb_ops_nsq,
-// tests/test_gpu_nsq.py).
+// tests/test_gpu_nsq.py), and so does the device code of the band-split, high-band analysis and synthesis filter-bank
+// kernels (sb_ops_qmf_split, sb_ops_hb, sb_ops_hb_vq, sb_ops_synth; tests/test_gpu_bands.py).
 // Every launcher takes host arrays, copies them to the device and back, and returns a CUDA error code (0 = success).
 #define SB_COOP 1
 #define SB_DIV_OUTLINE 1
@@ -12,6 +13,7 @@
 #include <string.h>
 #include <vector>
 #include "sb_coop.cuh"
+#include "sb_dec.cuh"
 #include "sb_nsq_warp.cuh"
 #include "../../oracle/nsq_io.h"
 
@@ -235,6 +237,175 @@ __global__ void __launch_bounds__(32, 12) nsq_kernel(NsqState* ns, EncScratch* s
     nsq_packet_warp(*S, &ns[3 * s], &scratch[s], nf);
 }
 
+// ---- the band-split kernel's device code (qmf_output_pair) in sb_enc_qmf_kernel's staging: one-warp blocks, history
+//      reversed from the filter memory, the packet's samples >> 1, the memory written back from the staged row -------------
+__global__ void __launch_bounds__(32) qmf_split_kernel(const i32* spp_of, i16* mems, const i16* pcm, i16* bands) {
+    __shared__ __align__(16) i16 xs[PACKET + 64];
+    __shared__ i16 coef[64];
+    const int lane = threadIdx.x, s = blockIdx.x;
+    const int spp = spp_of[s];
+    for (int i = lane; i < 64; i += 32) coef[i] = SB_T(qmf_fix)[i];
+    i16* mem = mems + (size_t)s * 64;
+    for (int i = lane; i < 63; i += 32) xs[i] = mem[62 - i];                     // x[i] = mem[M - i - 2]
+    for (int i = lane; i < spp; i += 32) xs[63 + i] = (i16)(pcm[(size_t)s * PACKET + i] >> 1);
+    __syncwarp();
+    i16* out = bands + (size_t)s * PACKET;
+    const int half = spp >> 1;
+    for (int k = lane; k < half; k += 32) {
+        i16 lo, hi;
+        qmf_output_pair(xs, coef, k, &lo, &hi);
+        out[k] = lo; out[half + k] = hi;
+    }
+    for (int i = lane; i < 63; i += 32) mem[i] = xs[spp + 62 - i];               // mem[i] = x[N + M - 2 - i]
+}
+
+// ---- the high-band analysis kernel's device code (c_hb_analyse_packet, c_hb_lsp_quant) in sb_enc_hb_warp_kernel's layout:
+//      kHbWarps warps per block (SB_HB_WARPS of sb_analysis.cu), one HbSmem slot each, a warp beyond the last case returns ----
+constexpr int kHbWarps = 4;
+struct HbSmem {
+    EncBands hb;
+    HbScr H;
+    alignas(16) i16 high[PACKET / 2];
+};
+constexpr int kHbSmem = kHbWarps * (int)sizeof(HbSmem);
+struct HbCase { i32 F, n; };      // frame length (160 or 320), high-band samples per packet (160 or 320)
+struct HbFrameOut {
+    i32 lsp_idx, nrg0[4];
+    i32 nlsf_pre[HB_ORDER], nlsf_q[HB_ORDER], weight[HB_ORDER];
+    i16 coef[HB_ORDER];
+    i16 x_hb_buf[2 * 320 + 40];
+    i32 hb_first;
+};
+__device__ __forceinline__ void ops_copy16(void* dst, const void* src, int bytes, int lane) {
+    const int4* s = reinterpret_cast<const int4*>(src);
+    int4* d = reinterpret_cast<int4*>(dst);
+    for (int i = lane; i < bytes / 16; i += 32) d[i] = s[i];
+}
+// One packet of every case: high [n][PACKET / 2] (the case's first k.n samples); the state moves between global and shared
+// memory as in the product kernel.
+// per_frame = 0: one c_hb_analyse_packet call over the whole packet, as the product kernel makes it (its loop over the
+//   packet's frames, scr->hb_lsp_idx[f] / hb_nrg0[f]); out[f] gets those and the state after the packet.
+// per_frame = 1: one c_hb_analyse_packet call per frame, so that each frame's working set is read before the next frame
+//   overwrites it; the packet loop itself is not run in this mode.  The NLSF vector the LSP search started from is
+//   recovered by running c_a2nlsf once more on the polynomial the frame's c_a2nlsf left behind (widened in place): its root
+//   search succeeds on that polynomial at the first attempt.  (A frame that ended in A2NLSF's white-spectrum fallback would
+//   not be recovered this way; Burg's filters do not reach that fallback, see tests/test_gpu_bands.py.)
+__global__ void __launch_bounds__(kHbWarps * 32) hb_kernel(const HbCase* cases, EncBands* states, EncScratch* scratch, const i16* high, int n,
+                                                           int per_frame, HbFrameOut* out) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int s = blockIdx.x * kHbWarps + w;
+    if (s >= n) return;
+    HbSmem* S = reinterpret_cast<HbSmem*>(smem_raw) + w;
+    const HbCase k = cases[s];
+    const int nf = k.n / k.F;
+    EncScratch* scr = &scratch[s];
+    ops_copy16(&S->hb, &states[s], (int)sizeof(EncBands), lane);
+    ops_copy16(S->high, high + (size_t)s * (PACKET / 2), k.n * 2, lane);
+    if (lane < 2) scr->hb_lsp_idx[lane] = 0x5a5a5a5a;
+    if (lane < 8) scr->hb_nrg0[lane >> 2][lane & 3] = 0x5a5a5a5a;
+    __syncwarp();
+    if (!per_frame) {
+        c_hb_analyse_packet(&S->hb, &S->H, S->high, k.n, k.F, scr);
+        __syncwarp();
+        for (int f = 0; f < nf; f++) {
+            HbFrameOut* o = &out[(size_t)s * 2 + f];
+            if (lane == 0) { o->lsp_idx = scr->hb_lsp_idx[f]; o->hb_first = S->hb.hb_first; }
+            if (lane < 4) o->nrg0[lane] = scr->hb_nrg0[f][lane];
+            for (int i = lane; i < 2 * 320 + 40; i += 32) o->x_hb_buf[i] = S->hb.x_hb_buf[i];
+        }
+    }
+    for (int f = 0; per_frame && f < nf; f++) {
+        c_hb_analyse_packet(&S->hb, &S->H, S->high + f * k.F, k.F, k.F, scr);
+        __syncwarp();
+        HbFrameOut* o = &out[(size_t)s * 2 + f];
+        if (lane == 0) { o->lsp_idx = scr->hb_lsp_idx[0]; o->hb_first = S->hb.hb_first; }
+        if (lane < 4) o->nrg0[lane] = scr->hb_nrg0[0][lane];
+        if (lane < HB_ORDER) {
+            o->nlsf_q[lane] = S->H.NLSF_Q15[lane];
+            o->weight[lane] = S->H.weight[lane];
+            o->coef[lane] = S->H.coef[lane];
+            S->H.A_Q16[1][lane] = S->H.A_Q16[0][lane];
+        }
+        for (int i = lane; i < 2 * 320 + 40; i += 32) o->x_hb_buf[i] = S->hb.x_hb_buf[i];
+        if (lane == 0) scr->hb_lsp_idx[0] = 0x5a5a5a5a;
+        if (lane < 4) scr->hb_nrg0[0][lane] = 0x5a5a5a5a;
+        __syncwarp();
+        c_a2nlsf<HB_ORDER>(S->H.NLSF_Q15, S->H.A_Q16[1], &S->H.u.a2n);
+        __syncwarp();
+        if (lane < HB_ORDER) o->nlsf_pre[lane] = S->H.NLSF_Q15[lane];
+        __syncwarp();
+    }
+    ops_copy16(&states[s], &S->hb, (int)sizeof(EncBands), lane);
+}
+// c_hb_lsp_quant alone: nlsf [n][8] -> index, quantised vector, Laroia weights
+__global__ void __launch_bounds__(kHbWarps * 32) hb_vq_kernel(const i32* nlsf, int n, i32* idx, i32* nlsf_q, i32* weight) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int s = blockIdx.x * kHbWarps + w;
+    if (s >= n) return;
+    HbScr* H = &(reinterpret_cast<HbSmem*>(smem_raw) + w)->H;
+    if (lane < HB_ORDER) { H->NLSF_Q15[lane] = nlsf[s * HB_ORDER + lane]; H->weight[lane] = -1; }
+    __syncwarp();
+    c_hb_lsp_quant(H, &idx[s]);
+    __syncwarp();
+    if (lane < HB_ORDER) { nlsf_q[s * HB_ORDER + lane] = H->NLSF_Q15[lane]; weight[s * HB_ORDER + lane] = H->weight[lane]; }
+}
+
+// ---- the synthesis kernel's device code (qmf_synth_group, qmf_synth_group_fix) in sb_dec_synth_kernel's layout: kSynWarps
+//      warps per block (SB_SYN_WARPS of solo_b200.cu), band signals and memories staged in shared memory, a fixed-point stream
+//      staged as int16 in the first half of its rows, PCM written with 8-byte stores ---------------------------------------------
+constexpr int kSynWarps = 4;
+enum { SYN_N2MAX = 640 };         // 40 ms of a 32 kHz stream's bands
+struct SynMem { float g0[64], g1[64]; };
+__global__ void __launch_bounds__(kSynWarps * 32) synth_kernel(const i32* fix_of, const i32* n2_of, SynMem* mem, const i16* band_low,
+                                                               const float* band_high, i16* pcm, int n) {
+    __shared__ float xx[kSynWarps][2][32 + SYN_N2MAX];
+    __shared__ float coef[64];
+    __shared__ i16 coef_fix[64];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < 64; i += blockDim.x) { coef[i] = SB_T(qmf_flt)[i]; coef_fix[i] = SB_T(qmf_fix)[i]; }
+    __syncthreads();
+    const int s = blockIdx.x * kSynWarps + w;
+    if (s >= n) return;
+    const int N2 = n2_of[s];
+    float* xx1 = xx[w][0];
+    float* xx2 = xx[w][1];
+    SynMem* st = &mem[s];
+    const i16* lo = band_low + (size_t)s * SYN_N2MAX;
+    const float* hi = band_high + (size_t)s * SYN_N2MAX;
+    int2* out = reinterpret_cast<int2*>(pcm + (size_t)s * 2 * SYN_N2MAX);
+    if (fix_of[s]) {
+        i16* yy1 = reinterpret_cast<i16*>(xx1);
+        i16* yy2 = reinterpret_cast<i16*>(xx2);
+        for (int i = lane; i < N2; i += 32) { yy1[i] = lo[N2 - 1 - i]; yy2[i] = (i16)__float2int_rz(hi[N2 - 1 - i]); }
+        yy1[N2 + lane] = (i16)__float2int_rz(st->g0[2 * lane + 1]);
+        yy2[N2 + lane] = (i16)__float2int_rz(st->g1[2 * lane + 1]);
+        __syncwarp();
+        for (int g = lane; g < N2 / 2; g += 32) {
+            i16 y[4];
+            qmf_synth_group_fix(yy1, yy2, coef_fix, N2, 2 * g, y);
+            out[g] = make_int2((int)((u16)y[0] | ((u32)(u16)y[1] << 16)), (int)((u16)y[2] | ((u32)(u16)y[3] << 16)));
+        }
+        __syncwarp();
+        st->g0[2 * lane + 1] = (float)yy1[lane];
+        st->g1[2 * lane + 1] = (float)yy2[lane];
+        return;
+    }
+    for (int i = lane; i < N2; i += 32) { xx1[i] = (float)lo[N2 - 1 - i]; xx2[i] = hi[N2 - 1 - i]; }
+    xx1[N2 + lane] = st->g0[2 * lane + 1];
+    xx2[N2 + lane] = st->g1[2 * lane + 1];
+    __syncwarp();
+    for (int g = lane; g < N2 / 2; g += 32) {
+        i16 y[4];
+        qmf_synth_group(xx1, xx2, coef, N2, 2 * g, y);
+        out[g] = make_int2((int)((u16)y[0] | ((u32)(u16)y[1] << 16)), (int)((u16)y[2] | ((u32)(u16)y[3] << 16)));
+    }
+    __syncwarp();
+    st->g0[2 * lane + 1] = xx1[lane];
+    st->g1[2 * lane + 1] = xx2[lane];
+}
+
 template <class T> struct Dev {
     T* p = nullptr;
     size_t n = 0;
@@ -408,6 +579,115 @@ extern "C" int sb_ops_nsq(int n, int npk, int nf, const NsqStateIO* st0, const N
                 o->Seed = scr[s].c[f].Seed;
             }
             for (int qz = 0; qz < 3; qz++) nsqio_state_from(&st_after[((size_t)s * npk + p) * 3 + qz], &ns[s * 3 + qz]);
+        }
+    }
+    return 0;
+}
+
+// n cases of npk packets: spp [n] (640 or 320 samples per packet), mem0 [n][64], pcm [n][npk][PACKET] -> bands [n][npk][PACKET]
+// ([low | high], spp samples), mem_after [n][npk][64].  One launch per packet; the memories stay on the device between them.
+extern "C" int sb_ops_qmf_split(int n, int npk, const int32_t* spp, const int16_t* mem0, const int16_t* pcm, int16_t* bands, int16_t* mem_after) {
+    if (n <= 0 || npk <= 0) return -1;
+    for (int i = 0; i < n; i++) if (spp[i] != PACKET && spp[i] != PACKET / 2) return -1;
+    Dev<i32> dspp(spp, n);
+    Dev<i16> dmem(mem0, (size_t)n * 64), dpcm(nullptr, (size_t)n * PACKET), dout(nullptr, (size_t)n * PACKET);
+    SB_CHECK(dspp.err); SB_CHECK(dmem.err); SB_CHECK(dpcm.err); SB_CHECK(dout.err);
+    std::vector<i16> h((size_t)n * PACKET);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) memcpy(&h[(size_t)s * PACKET], pcm + ((size_t)s * npk + p) * PACKET, sizeof(i16) * PACKET);
+        SB_CHECK(cudaMemcpy(dpcm.p, h.data(), sizeof(i16) * h.size(), cudaMemcpyHostToDevice));
+        SB_CHECK(cudaMemset(dout.p, 0xA5, sizeof(i16) * h.size()));
+        qmf_split_kernel<<<n, 32>>>(dspp.p, dmem.p, dpcm.p, dout.p);
+        SB_CHECK(finish());
+        SB_CHECK(dout.back(h.data()));
+        for (int s = 0; s < n; s++) memcpy(bands + ((size_t)s * npk + p) * PACKET, &h[(size_t)s * PACKET], sizeof(i16) * PACKET);
+        std::vector<i16> m((size_t)n * 64);
+        SB_CHECK(dmem.back(m.data()));
+        for (int s = 0; s < n; s++) memcpy(mem_after + ((size_t)s * npk + p) * 64, &m[(size_t)s * 64], sizeof(i16) * 64);
+    }
+    return 0;
+}
+
+extern "C" int sb_ops_hb_out_bytes() { return (int)sizeof(HbFrameOut); }
+
+// n cases of npk packets from the reset state (zero buffer, hb_first = 1 as enc_state_fields sets it): cases [n] (F, samples
+// per packet), high [n][npk][PACKET / 2] -> out [n][npk][2] (HbFrameOut; a packet of one frame leaves its second record
+// zero).  per_frame: see hb_kernel.  One launch per packet.
+// (out is untyped here: a parameter of the harness's internal record type would give the entry point internal linkage)
+extern "C" int sb_ops_hb(int n, int npk, int per_frame, const int32_t* cases, const int16_t* high, void* out_) {
+    HbFrameOut* out = static_cast<HbFrameOut*>(out_);
+    if (n <= 0 || npk <= 0) return -1;
+    for (int i = 0; i < n; i++) {
+        const int F = cases[2 * i], m = cases[2 * i + 1];
+        if ((F != HB_FRAME && F != 2 * HB_FRAME) || (m != HB_FRAME && m != 2 * HB_FRAME) || m % F) return -1;
+    }
+    SB_CHECK(cudaFuncSetAttribute(hb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHbSmem));
+    Dev<HbCase> dk(reinterpret_cast<const HbCase*>(cases), n);
+    std::vector<EncBands> reset(n);
+    memset(reset.data(), 0, sizeof(EncBands) * n);
+    for (int i = 0; i < n; i++) reset[i].hb_first = 1;
+    Dev<EncBands> dst(reset.data(), n);
+    Dev<EncScratch> dscr(nullptr, n);
+    Dev<i16> dhigh(nullptr, (size_t)n * (PACKET / 2));
+    Dev<HbFrameOut> dout(nullptr, (size_t)n * 2);
+    SB_CHECK(dk.err); SB_CHECK(dst.err); SB_CHECK(dscr.err); SB_CHECK(dhigh.err); SB_CHECK(dout.err);
+    std::vector<i16> h((size_t)n * (PACKET / 2));
+    std::vector<HbFrameOut> o((size_t)n * 2);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) memcpy(&h[(size_t)s * (PACKET / 2)], high + ((size_t)s * npk + p) * (PACKET / 2), sizeof(i16) * (PACKET / 2));
+        SB_CHECK(cudaMemcpy(dhigh.p, h.data(), sizeof(i16) * h.size(), cudaMemcpyHostToDevice));
+        SB_CHECK(cudaMemset(dout.p, 0, sizeof(HbFrameOut) * o.size()));
+        hb_kernel<<<(n + kHbWarps - 1) / kHbWarps, kHbWarps * 32, kHbSmem>>>(dk.p, dst.p, dscr.p, dhigh.p, n, per_frame, dout.p);
+        SB_CHECK(finish());
+        SB_CHECK(dout.back(o.data()));
+        for (int s = 0; s < n; s++) memcpy(out + ((size_t)s * npk + p) * 2, &o[(size_t)s * 2], sizeof(HbFrameOut) * 2);
+    }
+    return 0;
+}
+
+// nlsf [n][8] -> idx [n], nlsf_q [n][8], weight [n][8]
+extern "C" int sb_ops_hb_vq(int n, const int32_t* nlsf, int32_t* idx, int32_t* nlsf_q, int32_t* weight) {
+    if (n <= 0) return -1;
+    SB_CHECK(cudaFuncSetAttribute(hb_vq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHbSmem));
+    Dev<i32> dn(nlsf, (size_t)n * HB_ORDER), di(nullptr, n), dq(nullptr, (size_t)n * HB_ORDER), dw(nullptr, (size_t)n * HB_ORDER);
+    SB_CHECK(dn.err); SB_CHECK(di.err); SB_CHECK(dq.err); SB_CHECK(dw.err);
+    hb_vq_kernel<<<(n + kHbWarps - 1) / kHbWarps, kHbWarps * 32, kHbSmem>>>(dn.p, n, di.p, dq.p, dw.p);
+    SB_CHECK(finish());
+    SB_CHECK(di.back(idx)); SB_CHECK(dq.back(nlsf_q));
+    return (int)dw.back(weight);
+}
+
+// n streams of npk packets: fix [n] (0 = float, 1 = fixed point), n2 [n] (160, 320 or 640 band samples per packet), mem0 [n]
+// (g0_mem, g1_mem), low [n][npk][640] int16, high [n][npk][640] float -> pcm [n][npk][1280], mem_after [n][npk].  One launch
+// per packet; the memories stay on the device between them.
+extern "C" int sb_ops_synth(int n, int npk, const int32_t* fix, const int32_t* n2, const float* mem0, const int16_t* low, const float* high,
+                            int16_t* pcm, float* mem_after) {
+    if (n <= 0 || npk <= 0) return -1;
+    for (int i = 0; i < n; i++) if (n2[i] != 160 && n2[i] != 320 && n2[i] != 640) return -1;
+    const size_t B = SYN_N2MAX;
+    Dev<i32> dfix(fix, n), dn2(n2, n);
+    Dev<SynMem> dmem(reinterpret_cast<const SynMem*>(mem0), n);
+    Dev<i16> dlow(nullptr, n * B), dpcm(nullptr, n * 2 * B);
+    Dev<float> dhigh(nullptr, n * B);
+    SB_CHECK(dfix.err); SB_CHECK(dn2.err); SB_CHECK(dmem.err); SB_CHECK(dlow.err); SB_CHECK(dpcm.err); SB_CHECK(dhigh.err);
+    std::vector<i16> hl(n * B), hp(n * 2 * B);
+    std::vector<float> hh(n * B);
+    std::vector<SynMem> m(n);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) {
+            memcpy(&hl[s * B], low + ((size_t)s * npk + p) * B, sizeof(i16) * B);
+            memcpy(&hh[s * B], high + ((size_t)s * npk + p) * B, sizeof(float) * B);
+        }
+        SB_CHECK(cudaMemcpy(dlow.p, hl.data(), sizeof(i16) * hl.size(), cudaMemcpyHostToDevice));
+        SB_CHECK(cudaMemcpy(dhigh.p, hh.data(), sizeof(float) * hh.size(), cudaMemcpyHostToDevice));
+        SB_CHECK(cudaMemset(dpcm.p, 0xA5, sizeof(i16) * hp.size()));
+        synth_kernel<<<(n + kSynWarps - 1) / kSynWarps, kSynWarps * 32>>>(dfix.p, dn2.p, dmem.p, dlow.p, dhigh.p, dpcm.p, n);
+        SB_CHECK(finish());
+        SB_CHECK(dpcm.back(hp.data()));
+        SB_CHECK(dmem.back(m.data()));
+        for (int s = 0; s < n; s++) {
+            memcpy(pcm + ((size_t)s * npk + p) * 2 * B, &hp[s * 2 * B], sizeof(i16) * 2 * B);
+            memcpy(mem_after + ((size_t)s * npk + p) * 128, &m[s], sizeof(SynMem));
         }
     }
     return 0;
