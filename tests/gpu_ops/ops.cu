@@ -4,7 +4,8 @@
 // calls the routine and writes every output back.  tests/test_gpu_ops.py compares the results with the reference.
 // The quantiser kernel's device code runs here too, whole packets in the production kernel's layout (sb_ops_nsq,
 // tests/test_gpu_nsq.py), and so does the device code of the band-split, high-band analysis and synthesis filter-bank
-// kernels (sb_ops_qmf_split, sb_ops_hb, sb_ops_hb_vq, sb_ops_synth; tests/test_gpu_bands.py).
+// kernels (sb_ops_qmf_split, sb_ops_hb, sb_ops_hb_vq, sb_ops_synth; tests/test_gpu_bands.py), and that of the voice-activity
+// kernel and the high-band store of the entropy-coding kernel (sb_ops_vad, sb_ops_hb_store; tests/test_gpu_enc_stages.py).
 // Every launcher takes host arrays, copies them to the device and back, and returns a CUDA error code (0 = success).
 #define SB_COOP 1
 #define SB_DIV_OUTLINE 1
@@ -16,6 +17,7 @@
 #include "sb_dec.cuh"
 #include "sb_nsq_warp.cuh"
 #include "../../oracle/nsq_io.h"
+#include "../../oracle/vad_io.h"
 
 using namespace sb;
 
@@ -406,6 +408,43 @@ __global__ void __launch_bounds__(kSynWarps * 32) synth_kernel(const i32* fix_of
     st->g1[2 * lane + 1] = xx2[lane];
 }
 
+// ---- the voice-activity kernel's body (vad_packet) in sb_enc_vad_kernel's layout: one thread per stream, kTpb threads per
+//      block (SB_TPB of solo_b200.cu), the state copied to registers / local memory and back, the low band through 16-byte
+//      loads.  out [n][2][6]: speech activity, four band qualities, tilt of each frame ---------------------------------------
+constexpr int kTpb = 64;
+__global__ void __launch_bounds__(kTpb) vad_kernel(VadState* states, const i32* nf_of, const i16* __restrict__ bands, int n, i32* out) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    VadState v = states[s];
+    __align__(16) i16 low[2 * FRAME];
+    const int nf = nf_of[s];
+    const int4* src = reinterpret_cast<const int4*>(bands + (size_t)s * 2 * FRAME);
+    int4* dst = reinterpret_cast<int4*>(low);
+    for (int i = 0; i < nf * FRAME / 8; i++) dst[i] = src[i];
+    i32 sa[2], q[2][4], tilt[2];
+    vad_packet(&v, low, nf, sa, q, tilt);
+    for (int f = 0; f < nf; f++) {
+        i32* o = out + ((size_t)s * 2 + f) * 6;
+        o[0] = sa[f];
+        for (int b = 0; b < 4; b++) o[1 + b] = q[f][b];
+        o[5] = tilt[f];
+    }
+    states[s] = v;
+}
+
+// ---- the last step of the entropy-coding kernel (enc_store_high_band: gains, their 32-level VQ, bit packing, length
+//      fields) in sb_enc_finish_kernel's thread mapping: two threads per stream, thread k packing high-band frame k, kTpb
+//      threads per block with SB_FINISH_MINB's register budget.  The kernel's earlier steps (description coding, the
+//      partners' shuffles and the barrier before this store) do not run here.  lb_nb1 [n][2]: the low-band bytes and description 1's length; total [n][2]:
+//      what each thread returned -----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kTpb, 8) hb_store_kernel(const EncCore* states, const EncScratch* scratch, const i32* lb_nb1, u8* bits, int cap,
+                                                         i16* nbytes, i32* total, int n) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    const int s = t >> 1, k = t & 1;
+    if (s >= n) return;
+    total[t] = enc_store_high_band(&states[s], &scratch[s], k, lb_nb1[2 * s], lb_nb1[2 * s + 1], bits + (size_t)s * cap, cap, &nbytes[2 * s]);
+}
+
 template <class T> struct Dev {
     T* p = nullptr;
     size_t n = 0;
@@ -691,4 +730,69 @@ extern "C" int sb_ops_synth(int n, int npk, const int32_t* fix, const int32_t* n
         }
     }
     return 0;
+}
+
+// n streams of npk packets of nf [n] frames: st0 [n][28], low [n][npk][2][FRAME] -> out [n][npk][2][6] (see vad_kernel; a
+// 20 ms stream's second row stays zero), st_after [n][npk][28].  One launch per packet; the states stay on the device.
+extern "C" int sb_ops_vad(int n, int npk, const int32_t* nf, const int32_t* st0, const int16_t* low, int32_t* out, int32_t* st_after) {
+    if (n <= 0 || npk <= 0) return -1;
+    for (int i = 0; i < n; i++) if (nf[i] != 1 && nf[i] != 2) return -1;
+    std::vector<VadState> v(n);
+    for (int s = 0; s < n; s++) vadio_to(&v[s], st0 + (size_t)s * VADIO_WORDS);
+    Dev<VadState> dv(v.data(), n);
+    Dev<i32> dnf(nf, n), dout(nullptr, (size_t)n * 12);
+    Dev<i16> dlow(nullptr, (size_t)n * 2 * FRAME);
+    SB_CHECK(dv.err); SB_CHECK(dnf.err); SB_CHECK(dout.err); SB_CHECK(dlow.err);
+    std::vector<i16> h((size_t)n * 2 * FRAME);
+    std::vector<i32> o((size_t)n * 12);
+    for (int p = 0; p < npk; p++) {
+        for (int s = 0; s < n; s++) memcpy(&h[(size_t)s * 2 * FRAME], low + ((size_t)s * npk + p) * 2 * FRAME, sizeof(i16) * 2 * FRAME);
+        SB_CHECK(cudaMemcpy(dlow.p, h.data(), sizeof(i16) * h.size(), cudaMemcpyHostToDevice));
+        SB_CHECK(cudaMemset(dout.p, 0, sizeof(i32) * o.size()));
+        vad_kernel<<<(n + kTpb - 1) / kTpb, kTpb>>>(dv.p, dnf.p, dlow.p, n, dout.p);
+        SB_CHECK(finish());
+        SB_CHECK(dout.back(o.data()));
+        SB_CHECK(dv.back(v.data()));
+        for (int s = 0; s < n; s++) {
+            memcpy(out + ((size_t)s * npk + p) * 12, &o[(size_t)s * 12], sizeof(i32) * 12);
+            vadio_from(st_after + ((size_t)s * npk + p) * VADIO_WORDS, &v[s]);
+        }
+    }
+    return 0;
+}
+
+// n packets, one per stream: cfg [n][4] = frames per packet, high-band frame length, low-band bytes lb, description 1's
+// length nb1; lsp_idx [n][2], nrg0 [n][2][4], r16 [n][2][FRAME] (the high-band frames' inputs) -> bits [n][cap] (poisoned
+// with 0xA5 first), nbytes [n][2], total [n][2] (each thread's return value).  One launch.
+extern "C" int sb_ops_hb_store(int n, int cap, const int32_t* cfg, const int32_t* lsp_idx, const int32_t* nrg0, const int16_t* r16,
+                               uint8_t* bits, int16_t* nbytes, int32_t* total) {
+    if (n <= 0 || cap <= 0) return -1;
+    std::vector<EncCore> st(n);
+    std::vector<EncScratch> scr(n);
+    std::vector<i32> lb(2 * (size_t)n);
+    for (int s = 0; s < n; s++) {
+        const int32_t* c = cfg + 4 * (size_t)s;
+        if ((c[0] != 1 && c[0] != 2) || (c[1] != HB_FRAME && c[1] != 2 * HB_FRAME) || c[0] * FRAME < c[1]) return -1;
+        memset(&st[s], 0, sizeof(EncCore));
+        memset(&scr[s], 0, sizeof(EncScratch));
+        st[s].frames_per_packet = c[0];
+        st[s].hb_frame = c[1];
+        lb[2 * s] = c[2];
+        lb[2 * s + 1] = c[3];
+        memcpy(scr[s].hb_lsp_idx, lsp_idx + 2 * (size_t)s, sizeof(scr[s].hb_lsp_idx));
+        memcpy(scr[s].hb_nrg0, nrg0 + 8 * (size_t)s, sizeof(scr[s].hb_nrg0));
+        memcpy(scr[s].r16, r16 + 2 * FRAME * (size_t)s, sizeof(scr[s].r16));
+    }
+    Dev<EncCore> dst(st.data(), n);
+    Dev<EncScratch> dscr(scr.data(), n);
+    Dev<i32> dlb(lb.data(), lb.size()), dtot(nullptr, 2 * (size_t)n);
+    Dev<u8> dbits(nullptr, (size_t)n * cap);
+    Dev<i16> dnb(nullptr, 2 * (size_t)n);
+    SB_CHECK(dst.err); SB_CHECK(dscr.err); SB_CHECK(dlb.err); SB_CHECK(dtot.err); SB_CHECK(dbits.err); SB_CHECK(dnb.err);
+    SB_CHECK(cudaMemset(dbits.p, 0xA5, (size_t)n * cap));
+    SB_CHECK(cudaMemset(dnb.p, 0xA5, sizeof(i16) * 2 * (size_t)n));
+    hb_store_kernel<<<(2 * n + kTpb - 1) / kTpb, kTpb>>>(dst.p, dscr.p, dlb.p, dbits.p, cap, dnb.p, dtot.p, n);
+    SB_CHECK(finish());
+    SB_CHECK(dbits.back(bits)); SB_CHECK(dnb.back(nbytes));
+    return (int)dtot.back(total);
 }

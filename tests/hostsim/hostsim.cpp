@@ -108,6 +108,7 @@ static void run32m(const std::function<void()>& f) {
 #include "../../solo_b200/csrc/sb_dec.cuh"
 #include "../../solo_b200/csrc/sb_activity.cuh"
 #include "../../oracle/nsq_io.h"
+#include "../../oracle/vad_io.h"
 #ifdef SB_EMU
 #include "../../solo_b200/csrc/sb_coop.cuh"
 // ---- the quantiser kernel's device code (sb_nsq_warp.cuh) under the same 32-fibre emulation: one stream per "warp"
@@ -301,6 +302,37 @@ int hs_nsq_run(int kernel_code, int n, int npk, int nf, const NsqStateIO* st0, c
 #else
     return -1;
 #endif
+}
+// the voice-activity stage of one packet (vad_packet) from a state given as oracle/vad_io.h's words: low [nf][FRAME] ->
+// out [nf][6] (speech activity, four band qualities, tilt), st [VADIO_WORDS] in / out
+void hs_vad_packet(int* st, int nf, const short* low, int* out) {
+    sb::VadState v;
+    vadio_to(&v, st);
+    int sa[2], q[2][4], tilt[2];
+    sb::vad_packet(&v, low, nf, sa, q, tilt);
+    for (int f = 0; f < nf; f++) {
+        out[6 * f] = sa[f];
+        for (int b = 0; b < 4; b++) out[6 * f + 1 + b] = q[f][b];
+        out[6 * f + 5] = tilt[f];
+    }
+    vadio_from(st, &v);
+}
+// the high-band half of the entropy coding (enc_store_high_band) on one packet: cfg = frames per packet, high-band frame
+// length, low-band bytes, description 1's length; lsp_idx [2], nrg0 [2][4], r16 [2][FRAME] -> out [cap], nb [2]; returns
+// the packet's total size
+int hs_hb_store(const int* cfg, const int* lsp_idx, const int* nrg0, const short* r16, unsigned char* out, int cap, short* nb) {
+    static sb::EncCore st;
+    static sb::EncScratch scr;
+    memset(&st, 0, sizeof(st));
+    memset(&scr, 0, sizeof(scr));
+    st.frames_per_packet = cfg[0];
+    st.hb_frame = cfg[1];
+    memcpy(scr.hb_lsp_idx, lsp_idx, sizeof(scr.hb_lsp_idx));
+    memcpy(scr.hb_nrg0, nrg0, sizeof(scr.hb_nrg0));
+    memcpy(scr.r16, r16, sizeof(scr.r16));
+    int total = 0;
+    for (int k = 0; k < 2; k++) total = sb::enc_store_high_band(&st, &scr, k, cfg[2], cfg[3], out, cap, nb);
+    return total;
 }
 // rate (b/s), DTX, expected loss (%) from the next packet on: the body of the device's control kernel on the host model's
 // state; -1 or any other out-of-range value leaves a setting alone
