@@ -421,6 +421,61 @@ int solo_b200_tx_pack_device(solo_b200_tx *q, const uint8_t *d_bits, int cap, co
 int solo_b200_tx_reset(solo_b200_tx *q, const int32_t *streams, const uint32_t *start, int n, void *cuda_stream);
 int solo_b200_tx_stats(solo_b200_tx *q, uint32_t *counters, void *cuda_stream);
 
+/* G.711 gateway: PSTN and SIP participants (PCMU / PCMA, 8 kHz) in 16 kHz rooms, for N streams on the device.  It is
+   independent of the codec batches: its uplink rows go into the mixer's input matrix beside the decoder's rows, its
+   downlink takes the mixer's output rows.  Created with framesize_ms 40 or 20 for the whole gateway, so that its rows line
+   up with the room's: spp16 = 16 * framesize_ms (640 or 320) samples of 16 kHz PCM, spp8 = 8 * framesize_ms (320 or 160)
+   G.711 bytes.  Each stream has a law, 0 = mu-law (PCMU) or 1 = A-law (PCMA): create sets it for every stream, reset per
+   stream.
+   Companding is ITU-T G.711 with exactly this integer mapping (that of the classic Sun / CCITT g711.c):
+     mu-law: v = x >> 2 (arithmetic); sign mask 0xFF for v >= 0, else 0x7F with v = -v; v = min(v, 8159) + 33; seg = the
+             first s in 0..7 with v < 0x40 << s (8 if none: code 0x7F ^ mask); code = ((seg << 4) | ((v >> (seg + 1)) & 0xF)) ^ mask.
+             Expansion of code c: u = ~c, t = (((u & 0xF) << 3) + 0x84) << ((u & 0x70) >> 4); x = u & 0x80 ? 0x84 - t : t - 0x84.
+     A-law : v = x >> 3; mask 0xD5 for v >= 0, else 0x55 with v = -v - 1; seg = the first s in 0..7 with v < 0x20 << s;
+             code = ((seg << 4) | ((v >> (seg < 2 ? 1 : seg)) & 0xF)) ^ mask.
+             Expansion: a = c ^ 0x55, seg = (a & 0x70) >> 4, t = ((a & 0xF) << 4) + (seg ? 0x108 : 8), t <<= seg - 1 for
+             seg > 1; x = a & 0x80 ? t : -t.
+   Any byte is a valid code, so no input can fault a kernel.
+   uplink (PSTN -> room): g711 uint8 [N][spp8] and lost int32 [N] (bit f: 20 ms frame f, bytes [160 f, 160 f + 160), did
+     not arrive; NULL: nothing lost) -> pcm int16 [N][spp16], level uint8 [N], flags uint8 [N].  Per stream:
+       1. x8 = the expansion of each byte under the stream's law; the 160 samples of a lost frame are 0;
+       2. the encoder's voice-activity detector runs on each 160-sample frame of x8 with the stream's detector state; flag
+          bit f = speech_activity_Q8 >= SKP_FIX_CONST(0.1, 8), the comparison the encoder codes its VAD flag from.  It runs
+          on lost frames too, but their bit f is 0 and bit 2 + f is set (concealed, as the decoder reports it);
+       3. pcm = the fixed-point synthesis filter bank of the codec (AGR_Sate_qmf_synth of the fixed-point build) over
+          (low band = x8, high band = 0) with the stream's memories: the 0-4 kHz signal at 16 kHz;
+       4. level = the RFC 6464 level of the pcm row (n = spp16), as the activity reports define it.
+     level and flags have the activity reports' format: they drop into the arrays solo_b200_mix_* reads, so a speaking
+     PSTN participant is ranked and picked as a talker like any other, and a lost frame is never mixed.
+   downlink (room -> PSTN): pcm int16 [N][spp16] (e.g. the mixer's output rows) -> g711 uint8 [N][spp8]: the low band of the
+     fixed-point QMF analysis (AGR_Sate_qmf_decomp of the fixed-point build, the encoder's band split) with the stream's
+     63-sample memory, compressed under the stream's law.  The high band (4-8 kHz) is dropped.
+   reset: for a participant joining or rejoining a stream: the listed streams (host array of n) become fresh streams with
+     law[i] (a host array of n; NULL or an entry of -1 takes the create law).  -1 with nothing done (solo_b200_last_error()
+     set) for a stream outside [0, N), one listed twice, or a law other than 0 / 1.  One kernel ordered on `cuda_stream`,
+     which the call then synchronises (that stream only).  From the next call a reset stream gives, in both directions,
+     exactly what a stream of a newly created gateway with that law gives.
+   Entry points:
+     *_host   : host arrays; run on the gateway's own CUDA stream and return when done.
+     *_device : device arrays; only enqueue work on `cuda_stream`.  They check the pointers: -1 before any launch for a
+                NULL row pointer, d_g711 or d_pcm not 16-byte aligned, or d_lost not 4-byte aligned.
+   Launches: an uplink is two kernels, a downlink one, a reset one (create one).
+   state_bytes: device bytes per stream. */
+typedef struct solo_b200_g711 solo_b200_g711;
+#define SOLO_B200_G711_ULAW 0
+#define SOLO_B200_G711_ALAW 1
+/* NULL (solo_b200_last_error() set) for a bad n_streams, framesize_ms, law or device. */
+solo_b200_g711 *solo_b200_g711_create(int n_streams, int framesize_ms, int law, int device);
+void solo_b200_g711_destroy(solo_b200_g711 *g);
+int solo_b200_g711_uplink_host(solo_b200_g711 *g, const uint8_t *g711, const int32_t *lost, int16_t *pcm, uint8_t *level,
+                               uint8_t *flags);
+int solo_b200_g711_uplink_device(solo_b200_g711 *g, const uint8_t *d_g711, const int32_t *d_lost, int16_t *d_pcm,
+                                 uint8_t *d_level, uint8_t *d_flags, void *cuda_stream);
+int solo_b200_g711_downlink_host(solo_b200_g711 *g, const int16_t *pcm, uint8_t *g711);
+int solo_b200_g711_downlink_device(solo_b200_g711 *g, const int16_t *d_pcm, uint8_t *d_g711, void *cuda_stream);
+int solo_b200_g711_reset(solo_b200_g711 *g, const int32_t *streams, int n, const int32_t *law, void *cuda_stream);
+int solo_b200_g711_state_bytes(void);
+
 /* Multi-GPU ingest through peer memory:after this call kernels launched on `device` may read and write buffers that live in
    `peer_device`'s memory (same process, or another process's allocation mapped with CUDA IPC).  The *_device entry points
    then accept such addresses for pcm / bits / nbytes / lostflag: the band-split kernel pulls its PCM rows over NVLink and

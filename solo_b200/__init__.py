@@ -8,4 +8,4 @@ library, or creating a codec without a GPU, raises.
 from .api import (DecoderBatch, EncoderBatch, SoloDecoder, SoloEncoder, SoloError, kernel_launches, lib, set_chunks,  # noqa: F401
                   profile_enable, profile_read, state_bytes, dec_state_bytes, split_packet, merge_packets, bitfile_pack,
                   bitfile_unpack, apply_loss_device, enable_peer_access, mix, mix_device, rooms_csr, RxQueue,
-                  RX_COUNTERS, TxQueue, TX_COUNTERS, mix_contributors, mix_contributors_device)
+                  RX_COUNTERS, TxQueue, TX_COUNTERS, mix_contributors, mix_contributors_device, G711Gateway)

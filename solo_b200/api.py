@@ -124,6 +124,15 @@ def lib():
         L.solo_b200_tx_stats.argtypes = [vp, vp, vp]
         L.solo_b200_mix_contributors_host.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
         L.solo_b200_mix_contributors_device.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
+        L.solo_b200_g711_create.restype = vp
+        L.solo_b200_g711_create.argtypes = [C.c_int] * 4
+        L.solo_b200_g711_destroy.argtypes = [vp]
+        L.solo_b200_g711_uplink_host.argtypes = [vp] * 6
+        L.solo_b200_g711_uplink_device.argtypes = [vp] * 7
+        L.solo_b200_g711_downlink_host.argtypes = [vp] * 3
+        L.solo_b200_g711_downlink_device.argtypes = [vp] * 4
+        L.solo_b200_g711_reset.argtypes = [vp, vp, C.c_int, vp, vp]
+        L.solo_b200_g711_state_bytes.restype = C.c_int
         _lib = L
     return _lib
 
@@ -821,6 +830,95 @@ class TxQueue:
     def close(self):
         if getattr(self, "h", None):
             lib().solo_b200_tx_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+
+# ---- G.711 gateway (include/solo_b200.h, solo_b200_g711_*) ------------------------------------------------------------
+G711_LAWS = {"pcmu": 0, "pcma": 1}    # SOLO_B200_G711_ULAW / SOLO_B200_G711_ALAW
+
+
+def _law(v):
+    if isinstance(v, str):
+        if v not in G711_LAWS:
+            raise SoloError("law must be one of %s, not %r" % (sorted(G711_LAWS), v))
+        return G711_LAWS[v]
+    return v
+
+
+class G711Gateway:
+    """PSTN and SIP participants (G.711 PCMU / PCMA at 8 kHz) in 16 kHz rooms, N streams on one GPU: the uplink turns
+    G.711 payloads into 16 kHz rows with level and VAD flags for the mixer, the downlink turns the mixer's rows into G.711
+    payloads (see solo_b200_g711_* in include/solo_b200.h)."""
+
+    def __init__(self, n, framesize_ms=40, law="pcmu", device=0):
+        self.n, self.framesize_ms = int(n), int(framesize_ms)
+        self.spp8, self.spp16 = 8 * self.framesize_ms, 16 * self.framesize_ms
+        self.h = lib().solo_b200_g711_create(self.n, self.framesize_ms, int(_law(law)), int(device))
+        if not self.h:
+            raise SoloError("solo_b200_g711_create failed: " + _err())
+
+    def uplink(self, payload, lost=None):
+        """payload uint8 [N, spp8] (G.711 bytes; 160 per 20 ms frame), lost int32 [N] (bit f: frame f did not arrive) or
+        None -> (pcm int16 [N, spp16], level uint8 [N], flags uint8 [N]) in the activity reports' format."""
+        g = np.ascontiguousarray(payload, np.uint8)
+        if g.shape != (self.n, self.spp8):
+            raise SoloError("G711Gateway.uplink: payload must be [%d, %d]" % (self.n, self.spp8))
+        lo = None
+        if lost is not None:
+            lo = np.ascontiguousarray(lost, np.int32)
+            if lo.shape != (self.n,):
+                raise SoloError("G711Gateway.uplink: lost must have %d entries" % self.n)
+        pcm = np.zeros((self.n, self.spp16), np.int16)
+        level, flags = np.zeros(self.n, np.uint8), np.zeros(self.n, np.uint8)
+        r = lib().solo_b200_g711_uplink_host(self.h, g.ctypes.data, None if lo is None else lo.ctypes.data, pcm.ctypes.data,
+                                             level.ctypes.data, flags.ctypes.data)
+        if r:
+            raise SoloError("g711_uplink_host failed (%d): %s" % (r, _err()))
+        return pcm, level, flags
+
+    def uplink_device(self, d_payload, d_lost, d_pcm, d_level, d_flags, stream=0):
+        """uplink on device arrays (addresses; d_lost = 0 for nothing lost), enqueued on `stream`: two kernel launches."""
+        r = lib().solo_b200_g711_uplink_device(self.h, d_payload, d_lost or None, d_pcm, d_level, d_flags, stream)
+        if r:
+            raise SoloError("g711_uplink_device failed (%d): %s" % (r, _err()))
+
+    def downlink(self, pcm):
+        """pcm int16 [N, spp16] (e.g. the mixer's output rows) -> payload uint8 [N, spp8]."""
+        x = np.ascontiguousarray(pcm, np.int16)
+        if x.shape != (self.n, self.spp16):
+            raise SoloError("G711Gateway.downlink: pcm must be [%d, %d]" % (self.n, self.spp16))
+        out = np.zeros((self.n, self.spp8), np.uint8)
+        r = lib().solo_b200_g711_downlink_host(self.h, x.ctypes.data, out.ctypes.data)
+        if r:
+            raise SoloError("g711_downlink_host failed (%d): %s" % (r, _err()))
+        return out
+
+    def downlink_device(self, d_pcm, d_payload, stream=0):
+        """downlink on device arrays (addresses), enqueued on `stream`: one kernel launch."""
+        r = lib().solo_b200_g711_downlink_device(self.h, d_pcm, d_payload, stream)
+        if r:
+            raise SoloError("g711_downlink_device failed (%d): %s" % (r, _err()))
+
+    def reset(self, streams, law=None, stream=0):
+        """Make the listed streams fresh streams with `law` ("pcmu" / "pcma", 0 / 1, -1 or None for the create law, or an
+        array with one entry per listed stream).  Ordered on `stream`; returns once that stream is done.  Raises
+        SoloError, with nothing done, for a stream outside [0, N), one listed twice or a bad law."""
+        s, keep = _stream_list(streams), []
+        if law is not None and not isinstance(law, str):
+            law = [_law(v) for v in np.broadcast_to(np.asarray(law, object), (len(s),))]
+        r = lib().solo_b200_g711_reset(self.h, s.ctypes.data, len(s), _settings("g711_reset", _law(law), len(s), keep), stream)
+        if r:
+            raise SoloError("g711_reset failed (%d): %s" % (r, _err()))
+
+    @staticmethod
+    def state_bytes():
+        return int(lib().solo_b200_g711_state_bytes())
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().solo_b200_g711_destroy(self.h)
             self.h = None
 
     __del__ = close

@@ -29,6 +29,9 @@
 // The send queue (solo_b200_tx_*, sb_tx.cuh) turns the encoder's rows into numbered datagrams packed back to back: a pack
 // is sb_tx_sizes_kernel (thread per stream), sb_tx_scan_kernel (one block) and sb_tx_pack_kernel (warp per stream).
 // sb_mix_contributors_kernel (thread per member) writes each downlink's CSRC list and RFC 6465 levels.
+// The G.711 gateway (solo_b200_g711_*, sb_g711.cuh) puts PSTN / SIP participants in 16 kHz rooms: an uplink is
+// sb_g711_vad_kernel (thread per stream) and sb_g711_synth_kernel (warp per stream), a downlink sb_g711_downlink_kernel
+// (warp per stream), create and reset sb_g711_reset_kernel.
 // Persistent per-stream state lives in device arrays (EncState / DecState) that never leave the GPU between packets;
 // the *_host entry points process a wave as a few chunks of streams on the batch's CUDA streams.  The host code below is the C ABI:
 // the batched entry points of include/solo_b200.h and the reference's six functions of include/AGR_JC1_SDK_API.h.
@@ -44,6 +47,7 @@
 #include "sb_activity.cuh"
 #include "sb_dec.cuh"
 #include "sb_enc.cuh"
+#include "sb_g711.cuh"
 #include "sb_mix.cuh"
 #include "sb_nsq_warp.cuh"
 #include "sb_rx.cuh"
@@ -492,6 +496,117 @@ __global__ void __launch_bounds__(SB_MIX_WARPS * 32, 6) sb_mix_kernel(const i16*
             dst[c] = make_int4(w[0], w[1], w[2], w[3]);
         }
     }
+}
+
+// ---- G.711 gateway (sb_g711.cuh) -------------------------------------------------------------------------------------------
+// Create and reset, one thread per stream: the listed streams (streams = NULL: every stream) as create makes them, each with
+// its law (-1 or a NULL array: law0).
+__global__ void __launch_bounds__(SB_TPB) sb_g711_reset_kernel(G711State* states, const i32* __restrict__ streams, int n,
+                                                               const i32* __restrict__ law, int law0) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    g711_state_init(&states[streams ? streams[i] : i], law && law[i] != -1 ? law[i] : law0);
+}
+
+// Uplink, voice activity: one thread per stream, as sb_enc_vad_kernel (the detector is a pure recurrence).  The thread
+// expands its row from 16-byte loads into a local frame buffer and writes the flags byte.
+__global__ void __launch_bounds__(SB_TPB) sb_g711_vad_kernel(G711State* states, const u8* __restrict__ codes, const i32* __restrict__ lost,
+                                                             u8* __restrict__ flags, int nf, int n) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const int law = states[s].law;
+    const i32 ls = lost ? lost[s] : 0;
+    __align__(16) i16 x8[2 * FRAME];
+    const uint4* src = reinterpret_cast<const uint4*>(codes + (size_t)s * nf * FRAME);
+    for (int c = 0; c < nf * FRAME / 16; c++) {
+        const uint4 q = src[c];
+        const u32 w[4] = {q.x, q.y, q.z, q.w};
+        for (int b = 0; b < 16; b++) x8[16 * c + b] = g711_up_sample(law, (u8)(w[b >> 2] >> (8 * (b & 3))), ls, 16 * c + b);
+    }
+    VadState v = states[s].vad;
+    i32 sa_Q8[2];
+    flags[s] = (u8)g711_vad(&v, x8, nf, ls, sa_Q8);
+    states[s].vad = v;
+}
+
+// Uplink, synthesis and level: one warp per stream.  Lanes expand 16 codes each (one 16-byte load) into the time-reversed
+// low band in shared memory, then run the decoder's fixed-point synthesis groups over it against a shared zero high band
+// (sb_dec_synth_kernel's DEC_FIX layout), store the row with 8-byte stores and reduce the row's energy for its level.
+#define SB_G711_WARPS 8
+__global__ void __launch_bounds__(SB_G711_WARPS * 32) sb_g711_synth_kernel(G711State* states, const u8* __restrict__ codes, const i32* __restrict__ lost,
+                                                                           i16* __restrict__ pcm, u8* __restrict__ level, int nf, int n) {
+    __shared__ i16 yy[SB_G711_WARPS][32 + 2 * FRAME];
+    __shared__ i16 zero[32 + 2 * FRAME];
+    __shared__ i16 coef[64];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < 32 + 2 * FRAME; i += blockDim.x) zero[i] = 0;
+    for (int i = threadIdx.x; i < 64; i += blockDim.x) coef[i] = SB_T(qmf_fix)[i];
+    __syncthreads();
+    const int s = blockIdx.x * SB_G711_WARPS + w;
+    if (s >= n) return;                           // whole warps
+    const int N2 = nf * FRAME;
+    G711State* st = &states[s];
+    const int law = st->law;
+    const i32 ls = lost ? lost[s] : 0;
+    i16* yy1 = yy[w];
+    if (lane < N2 / 16) {
+        const uint4 q = reinterpret_cast<const uint4*>(codes + (size_t)s * N2)[lane];
+        const u32 c4[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int b = 0; b < 16; b++) {
+            const int i = 16 * lane + b;
+            yy1[N2 - 1 - i] = g711_up_sample(law, (u8)(c4[b >> 2] >> (8 * (b & 3))), ls, i);
+        }
+    }
+    yy1[N2 + lane] = st->syn_mem[lane];
+    __syncwarp();
+    i16* out = pcm + (size_t)s * 2 * N2;
+    i64 e = 0;
+    for (int g = lane; g < N2 / 2; g += 32) {
+        i16 y[4];
+        qmf_synth_group_fix(yy1, zero, coef, N2, 2 * g, y);
+        store_pcm4(out, g, y);
+        e += (i64)((u32)(y[0] * y[0]) + (u32)(y[1] * y[1])) + (i64)((u32)(y[2] * y[2]) + (u32)(y[3] * y[3]));
+    }
+    st->syn_mem[lane] = yy1[lane];
+    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+    if (lane == 0) level[s] = (u8)rfc6464_level(e, 2 * N2);
+}
+
+// Downlink: one warp per stream, sb_enc_qmf_kernel's band split (history and row in shared memory, output pairs k = lane,
+// lane + 32, ...) with the low band compressed in lane and stored as one coalesced byte per lane; the high band is dropped.
+__global__ void __launch_bounds__(SB_G711_WARPS * 32) sb_g711_downlink_kernel(G711State* states, const i16* __restrict__ pcm, u8* __restrict__ codes,
+                                                                              int spp, int n) {
+    __shared__ i16 xs[SB_G711_WARPS][PACKET + 64];
+    __shared__ i16 coef[64];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < 64; i += blockDim.x) coef[i] = SB_T(qmf_fix)[i];
+    __syncthreads();
+    const int s = blockIdx.x * SB_G711_WARPS + w;
+    if (s >= n) return;
+    G711State* st = &states[s];
+    const int law = st->law;
+    i16* x = xs[w];
+    for (int i = lane; i < 63; i += 32) x[i] = st->ana_mem[62 - i];      // x[i] = mem[M - i - 2]
+    const int4* row = reinterpret_cast<const int4*>(pcm + (size_t)s * spp);
+    for (int c = lane; c < spp / 8; c += 32) {
+        const int4 q = row[c];
+        const int v[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int h = 0; h < 4; h++) {
+            x[63 + 8 * c + 2 * h] = (i16)((i16)(v[h] & 0xffff) >> 1);
+            x[64 + 8 * c + 2 * h] = (i16)(v[h] >> 17);
+        }
+    }
+    __syncwarp();
+    const int half = spp >> 1;
+    u8* out = codes + (size_t)s * half;
+    for (int k = lane; k < half; k += 32) {
+        i16 lo, hi;
+        qmf_output_pair(x, coef, k, &lo, &hi);
+        out[k] = g711_compress(law, lo);
+    }
+    for (int i = lane; i < 63; i += 32) st->ana_mem[i] = x[spp + 62 - i];    // mem[i] = x[N + M - 2 - i]
 }
 
 // ---- receive queue (sb_rx.cuh) -------------------------------------------------------------------------------------------
@@ -2355,6 +2470,130 @@ int solo_b200_mix_contributors_host(const int32_t* room_start, const int32_t* me
     const int r = s.finish();
     cudaStreamDestroy(st);
     return r;
+}
+
+// ---- G.711 gateway (sb_g711.cuh) ---------------------------------------------------------------------------------------------
+struct solo_b200_g711 {
+    int n, device, nf, law;     // nf: 20 ms frames per row (framesize_ms / 20); law: the create default
+    cudaStream_t st;            // the _host forms' stream
+    G711State* d_states;
+    DevBuf d_list;              // the Staging of the host calls (grown on use)
+    ~solo_b200_g711() {
+        if (st) cudaStreamDestroy(st);
+        cudaFree(d_states); cudaFree(d_list.d);
+    }
+};
+static int g711_reset_launch(solo_b200_g711* g, const i32* streams, int n, const i32* law, cudaStream_t st) {
+    sb_g711_reset_kernel<<<(n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(g->d_states, streams, n, law, g->law);
+    return launched("sb_g711_reset_kernel");
+}
+
+solo_b200_g711* solo_b200_g711_create(int n_streams, int framesize_ms, int law, int device) {
+    if (n_streams <= 0 || (framesize_ms != 40 && framesize_ms != 20) || (law != G711_ULAW && law != G711_ALAW)) {
+        snprintf(g_err, sizeof g_err, "g711_create: bad argument (n %d, framesize_ms %d, law %d)", n_streams, framesize_ms, law);
+        return nullptr;
+    }
+    if (require_gpu(device)) return nullptr;
+    solo_b200_g711* g = new solo_b200_g711();
+    g->n = n_streams; g->device = device; g->nf = framesize_ms / 20; g->law = law;
+    const bool ok = cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) == cudaSuccess &&
+                    cudaMalloc(&g->d_states, sizeof(G711State) * (size_t)n_streams) == cudaSuccess &&
+                    g711_reset_launch(g, nullptr, n_streams, nullptr, g->st) == 0 && cudaStreamSynchronize(g->st) == cudaSuccess;
+    if (!ok) {
+        snprintf(g_err, sizeof g_err, "g711_create: %s", cudaGetErrorString(cudaGetLastError()));
+        delete g;
+        return nullptr;
+    }
+    return g;
+}
+
+void solo_b200_g711_destroy(solo_b200_g711* g) {
+    if (!g) return;
+    cudaSetDevice(g->device);
+    cudaStreamSynchronize(g->st);
+    delete g;
+}
+
+int solo_b200_g711_state_bytes(void) { return (int)sizeof(G711State); }
+
+static int g711_uplink_launch(solo_b200_g711* g, const u8* codes, const i32* lost, i16* pcm, u8* level, u8* flags, cudaStream_t st) {
+    sb_g711_vad_kernel<<<(g->n + SB_TPB - 1) / SB_TPB, SB_TPB, 0, st>>>(g->d_states, codes, lost, flags, g->nf, g->n);
+    if (int e = launched("sb_g711_vad_kernel")) return e;
+    sb_g711_synth_kernel<<<(g->n + SB_G711_WARPS - 1) / SB_G711_WARPS, SB_G711_WARPS * 32, 0, st>>>(g->d_states, codes, lost, pcm, level, g->nf, g->n);
+    return launched("sb_g711_synth_kernel");
+}
+static int g711_downlink_launch(solo_b200_g711* g, const i16* pcm, u8* codes, cudaStream_t st) {
+    sb_g711_downlink_kernel<<<(g->n + SB_G711_WARPS - 1) / SB_G711_WARPS, SB_G711_WARPS * 32, 0, st>>>(g->d_states, pcm, codes, 2 * FRAME * g->nf, g->n);
+    return launched("sb_g711_downlink_kernel");
+}
+// the device forms' pointers: the rows 16-byte aligned (16-byte loads of the codes and of the downlink's PCM, 8-byte stores of
+// the uplink's PCM), lost 4-byte aligned or NULL
+static int g711_device_args_ok(const solo_b200_g711* g, const void* codes, const void* pcm, const void* lost, const char* who) {
+    if (!g || !codes || !pcm) { snprintf(g_err, sizeof g_err, "%s: bad argument", who); return 0; }
+    if ((((uintptr_t)codes | (uintptr_t)pcm) & 15) || ((uintptr_t)lost & 3)) {
+        snprintf(g_err, sizeof g_err, "%s: the G.711 and PCM rows must be 16-byte aligned and lost 4-byte aligned", who);
+        return 0;
+    }
+    return 1;
+}
+
+int solo_b200_g711_uplink_device(solo_b200_g711* g, const uint8_t* d_g711, const int32_t* d_lost, int16_t* d_pcm, uint8_t* d_level,
+                                 uint8_t* d_flags, void* cuda_stream) {
+    if (!g711_device_args_ok(g, d_g711, d_pcm, d_lost, "g711_uplink_device")) return -1;
+    if (!d_level || !d_flags) { snprintf(g_err, sizeof g_err, "g711_uplink_device: bad argument"); return -1; }
+    CK(cudaSetDevice(g->device));
+    return g711_uplink_launch(g, d_g711, d_lost, d_pcm, d_level, d_flags, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_g711_uplink_host(solo_b200_g711* g, const uint8_t* g711, const int32_t* lost, int16_t* pcm, uint8_t* level, uint8_t* flags) {
+    if (!g || !g711 || !pcm || !level || !flags) { snprintf(g_err, sizeof g_err, "g711_uplink_host: bad argument"); return -1; }
+    CK(cudaSetDevice(g->device));
+    const size_t n = (size_t)g->n, spp8 = (size_t)FRAME * g->nf;
+    const u8* d_codes; const i32* d_lost = nullptr; i16* d_pcm; u8 *d_level, *d_flags;
+    Staging s(g->st, "g711_uplink", &g->d_list);
+    s.span(d_codes, g711, nullptr, n * spp8);
+    if (lost) s.span(d_lost, lost, nullptr, 4 * n);
+    s.span(d_pcm, nullptr, pcm, 2 * n * 2 * spp8);
+    s.span(d_level, nullptr, level, n);
+    s.span(d_flags, nullptr, flags, n);
+    s.run([&] { return g711_uplink_launch(g, d_codes, d_lost, d_pcm, d_level, d_flags, g->st); });
+    return s.finish();
+}
+
+int solo_b200_g711_downlink_device(solo_b200_g711* g, const int16_t* d_pcm, uint8_t* d_g711, void* cuda_stream) {
+    if (!g711_device_args_ok(g, d_g711, d_pcm, nullptr, "g711_downlink_device")) return -1;
+    CK(cudaSetDevice(g->device));
+    return g711_downlink_launch(g, d_pcm, d_g711, (cudaStream_t)cuda_stream);
+}
+
+int solo_b200_g711_downlink_host(solo_b200_g711* g, const int16_t* pcm, uint8_t* g711) {
+    if (!g || !pcm || !g711) { snprintf(g_err, sizeof g_err, "g711_downlink_host: bad argument"); return -1; }
+    CK(cudaSetDevice(g->device));
+    const size_t n = (size_t)g->n, spp8 = (size_t)FRAME * g->nf;
+    const i16* d_pcm; u8* d_codes;
+    Staging s(g->st, "g711_downlink", &g->d_list);
+    s.span(d_pcm, pcm, nullptr, 2 * n * 2 * spp8);
+    s.span(d_codes, nullptr, g711, n * spp8);
+    s.run([&] { return g711_downlink_launch(g, d_pcm, d_codes, g->st); });
+    return s.finish();
+}
+
+int solo_b200_g711_reset(solo_b200_g711* g, const int32_t* streams, int n, const int32_t* law, void* cuda_stream) {
+    if (!list_args_ok(g, streams, n, "g711_reset") || !streams_ok(streams, n, g->n, "g711_reset")) return -1;
+    for (int i = 0; law && i < n; i++)
+        if (law[i] != -1 && law[i] != G711_ULAW && law[i] != G711_ALAW) {
+            snprintf(g_err, sizeof g_err, "g711_reset: law %d of stream %d is not 0 (mu-law) or 1 (A-law)", law[i], streams[i]);
+            return -1;
+        }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(g->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const i32 *d_streams, *d_law = nullptr;
+    Staging s(st, "g711_reset", &g->d_list);
+    s.span(d_streams, streams, nullptr, 4 * (size_t)n);
+    if (law) s.span(d_law, law, nullptr, 4 * (size_t)n);
+    s.run([&] { return g711_reset_launch(g, d_streams, n, d_law, st); });
+    return s.finish();
 }
 
 // ---- multi-GPU ingest through peer memory --------------------------------------------------------------------------------
